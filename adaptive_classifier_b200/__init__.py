@@ -1,4 +1,4 @@
-"""B200-native predict()/add_examples() hot path of codelion/adaptive-classifier.
+"""H100-native predict()/add_examples() hot path of codelion/adaptive-classifier.
 
 `import adaptive_classifier_b200 as adaptive_classifier` gives the public names of the reference package
 (/root/reference/src/adaptive_classifier/__init__.py:1-16).  Importing needs no GPU; constructing a classifier or

@@ -2,7 +2,7 @@
 
 This is the binding a maintainer of the reference would add (INTEGRATION.md).  PyTorch is used only for
 device memory and streams: every call passes raw device pointers + the current CUDA stream.
-There is NO CPU fallback: a missing library raises ImportError-like RuntimeError, a missing sm_100 device
+There is NO CPU fallback: a missing library raises ImportError-like RuntimeError, a missing sm_90 (H100) device
 makes every compute call raise AdaptiveB200Error.
 """
 from __future__ import annotations
@@ -512,7 +512,7 @@ class Encoder:
             sd, dims = distilbert_to_bert_state_dict(sd, c)
             return cls(sd, arch="bert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
         if mt not in ("bert", "roberta", "xlm-roberta"):
-            raise AdaptiveB200Error(f"encoder architecture '{mt}' is not implemented in the B200 path yet")
+            raise AdaptiveB200Error(f"encoder architecture '{mt}' is not implemented in the CUDA path yet")
         if getattr(c, "hidden_act", "gelu") != "gelu" or getattr(c, "position_embedding_type", "absolute") != "absolute":
             raise AdaptiveB200Error("only exact-erf GELU and absolute position embeddings are implemented")
         return cls(sd, arch="bert" if mt == "bert" else "roberta", layers=c.num_hidden_layers, hidden=c.hidden_size,

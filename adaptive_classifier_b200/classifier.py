@@ -2,7 +2,7 @@
 
 Drop-in for the predict()/predict_batch()/add_examples() hot path: same method names, arguments, return
 types, label-id rules, blending formulas and error behaviour (citations inline).  All arithmetic runs on
-the B200 through the C ABI: encoder (csrc/encoder.cu), prototype kNN (csrc/knn_*.cu), adaptive head +
+the H100 through the C ABI: encoder (csrc/encoder.cu), prototype kNN (csrc/knn_*.cu), adaptive head +
 AdamW/EWC (csrc/head.cu).  HuggingFace is used for checkpoint/tokenizer IO only.
 
 Out of scope (SURVEY.md section 2): ONNX export/ORT inference (use_onnx is accepted and ignored), strategic mode,
@@ -54,7 +54,7 @@ class AdaptiveClassifier:
         self.config = ModelConfig(config)
         if device is not None and not str(device).startswith("cuda"):
             raise _cabi.AdaptiveB200Error(
-                f"device={device!r}: adaptive_classifier_b200 runs on B200 GPUs only (no CPU fallback)")
+                f"device={device!r}: adaptive_classifier_b200 runs on H100 GPUs only (no CPU fallback)")
         if not torch.cuda.is_available():
             raise _cabi.AdaptiveB200Error("no CUDA device: adaptive_classifier_b200 has no CPU fallback")
         _cabi.check(_cabi.load_library().ac_device_check(), "ac_device_check")
@@ -82,7 +82,7 @@ class AdaptiveClassifier:
         self.strategic_optimizer = None
         self.strategic_evaluator = None
         if self.config.enable_strategic_mode:
-            raise _cabi.AdaptiveB200Error("strategic mode is out of scope of the B200 hot path (SURVEY.md section 2 #9)")
+            raise _cabi.AdaptiveB200Error("strategic mode is out of scope of the GPU hot path (SURVEY.md section 2 #9)")
 
     @property
     def strategic_mode(self) -> bool:
@@ -393,7 +393,7 @@ class AdaptiveClassifier:
     # ------------------------------------------------------------------------------------------ misc API
     def to(self, device: str) -> "AdaptiveClassifier":
         if not str(device).startswith("cuda"):
-            raise _cabi.AdaptiveB200Error("adaptive_classifier_b200 runs on B200 GPUs only")
+            raise _cabi.AdaptiveB200Error("adaptive_classifier_b200 runs on H100 GPUs only")
         if torch.device(device) != torch.device(self.device) and torch.device(device).index not in (None, torch.device(self.device).index):
             # the encoder handle and the prototype index live on the device they were built on
             raise _cabi.AdaptiveB200Error(f"moving a built classifier from {self.device} to {device} is not supported: construct it "

@@ -75,8 +75,8 @@ int sm_count() {
     static int n = 0;
     if (n == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     }
     return n;
 }
@@ -202,11 +202,12 @@ extern "C" int ac_device_check(void) {
         set_error("no CUDA device visible (%s); this library has no CPU fallback", cudaGetErrorString(e));
         return AC_E_CUDA;
     }
-    int dev = 0, major = 0;
+    int dev = 0, major = 0, minor = 0;
     AC_CUDA(cudaGetDevice(&dev));
     AC_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10) {
-        set_error("device compute capability %d.x is not sm_100 (B200); kernels are sm_100a only", major);
+    AC_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+    if (major != 9 || minor != 0) {
+        set_error("device compute capability %d.%d is not sm_90 (H100); kernels are sm_90a only", major, minor);
         return AC_E_CUDA;
     }
     return AC_OK;

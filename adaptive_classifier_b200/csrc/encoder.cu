@@ -4,19 +4,19 @@
 // /root/reference/src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel.forward:
 // embeddings modeling_bert.py:53-113, self-attention :143-207, output+LN :287-298, FFN :330-356).
 //
-// Precision: every tensor-core operand is fp16 (RNE from fp32), accumulation fp32 in TMEM, residual stream, LayerNorm,
+// Precision: every tensor-core operand is fp16 (RNE from fp32), accumulation fp32 (wgmma), residual stream, LayerNorm,
 // softmax and GELU in fp32.  fp16 carries the same 10-bit mantissa as tf32, so the measured error is the tf32 one
 // (oracle/precision_study.py: 1.7e-4 on squared-L2 distances, bf16 would be 1.4e-3 > the 1e-3 tolerance) at twice the
 // tensor rate and half the operand bytes.
 //
-//   projections   tcgen05 GEMM of gemm_tc.cuh (kind::f16) with compile-time-specialised fused epilogues:
+//   projections   wgmma GEMM of gemm_tc.cuh (.f16) with compile-time-specialised fused epilogues:
 //                 bias | bias+GELU(erf) | bias+residual, fp16 or fp32 output, V written TRANSPOSED per (sequence, head)
-//   attention     one CTA per (sequence, head): Q, K and V^T tiles by TMA, QK^T and PV as tcgen05 MMAs with the score
-//                 tile / output tile in TMEM, thread-per-query-row softmax in between (S <= 128, head_dim 64)
+//   attention     one CTA per (sequence, head): Q, K and V^T tiles by TMA, QK^T and PV as wgmma with the score tile
+//                 staged in shared memory, thread-per-query-row softmax in between (S <= 128, head_dim 64)
 //   LayerNorm     never materialised inside the layer stack: the residual epilogues keep the un-normalised sums y (fp32) and
 //                 per-row (sum, sumsq) partials, the consuming projections run on gamma-scaled weights and apply the
 //                 rank-1 correction r (acc - mu c1) + c0 in their epilogue ("deferred LayerNorm" below)
-#include "gemm_tc2.cuh"
+#include "gemm_tc.cuh"
 #include <cuda_fp16.h>
 #include <math_constants.h>
 #include <vector>
@@ -59,9 +59,7 @@ __device__ __forceinline__ float gelu_erf(float y) {
 //   DEFER: the A operand was the UN-normalised residual sum y (fp16) and the weights were packed as fp16(gamma * W):
 //       LayerNorm(y) W^T + b = r (acc - mu c1) + c0  with the row statistics (mu, r) of y, c1 = rowsum(W'), and
 //       `bias` holding c0 = W beta + b  (see "deferred LayerNorm" below)
-//   COLS:  accumulator columns one epilogue warp drains per tile (128 with 8 epilogue warps, 64 with 16): only the DEFER
-//          variant needs it, to know which chunk is the first of its slice
-template <int MODE, bool OUT_HALF, bool VT, bool DEFER = false, int COLS = GEMM_BLOCK_N / 2>
+template <int MODE, bool OUT_HALF, bool VT, bool DEFER = false>
 struct EpiLinear {
     static_assert(!DEFER || (OUT_HALF && MODE != 2), "the deferred-LayerNorm consumer epilogues write fp16 operands");
     const float *__restrict__ bias;       // [N]   (DEFER: c0)
@@ -86,6 +84,7 @@ struct EpiLinear {
     __device__ __forceinline__ float pre(const State &st, float acc, float b, float c1v) const {
         return DEFER ? fmaf(st.r, fmaf(-st.mu, c1v, acc), b) : acc + b;
     }
+    __device__ __forceinline__ bool skip_kernel() const { return false; }
     __device__ __forceinline__ void begin_cta(State &, int, int) const {}
     __device__ __forceinline__ void end_cta(State &, int, int) const {}
 
@@ -98,14 +97,14 @@ struct EpiLinear {
     // rows r8 + 8*i (i < 4) and the 16-byte column group c of each 16-column half.
     __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &ti, int row, int col0, int lane, int buf) const {
         if (DEFER) {
-            if (((col0 - ti.n0) & (COLS - 1)) == 0) {                  // first chunk of this warp's column slice
+            if (((col0 - ti.n0) & (GEMM_EPI_COLS - 1)) == 0) {         // first chunk of this warp's column slice
                 const float2 ms = (row < M) ? __ldg(row_stats + row) : make_float2(0.f, 0.f);
                 st.mu = ms.x;
                 st.r = ms.y;
             }
         }
         if (MODE != 2) return;
-        const int row_base = ti.m0 + ((threadIdx.x >> 5) & 3) * 32;
+        const int row_base = row - lane;
         const int r8 = lane >> 2, c = lane & 3;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -122,8 +121,8 @@ struct EpiLinear {
     }
 
     __device__ __forceinline__ void tile(State &st, const GemmTileInfo &ti, int row, int col0, const float (&v)[32],
-                                         uint8_t *stage, int lane, int buf, uint32_t /*taddr*/) const {
-        const int row_base = ti.m0 + ((threadIdx.x >> 5) & 3) * 32;        // first row of this warp's TMEM quarter
+                                         uint8_t *stage, int lane, int buf, const float * /*acc*/) const {
+        const int row_base = row - lane;                                     // first row of this warp's quarter
         if (row_base >= M || col0 >= N) return;                              // warp-uniform
         if (VT && col0 >= vt_col0) {
             // thread = token row: lanes hold 32 consecutive keys of (mostly) one sequence -> 64-byte coalesced stores
@@ -220,7 +219,7 @@ struct EpiLinear {
 //                                                row statistics and the pending LayerNorm's parameters
 //   writes y_new (fp32, IN PLACE over y_old: every element is read and written by the same thread), fp16(y_new) (the
 //   next GEMM's A operand, consumed through EpiLinear<.., DEFER = true>) and per-row partial (sum, sum of squares) of
-//   this warp's 128 columns into parts[column part][row]; ln_stats_kernel turns the parts into (mu, r).
+//   this warp's GEMM_EPI_COLS columns into parts[column part][row]; ln_stats_kernel turns the parts into (mu, r).
 //   HBM traffic per half layer at B*S = 65536, H = 768: read y 201 MB, write y 201 MB + fp16 101 MB = 503 MB instead of
 //   905 MB (GEMM epilogue 402 MB + LayerNorm kernel 503 MB); precision: oracle/deferred_ln_study.py (CPU emulation) and tests/test_gpu_parity.py (non-trivial gamma / beta).
 // ------------------------------------------------------------------------------------------------
@@ -231,20 +230,13 @@ struct EpiResidDefer {
     const float2 *__restrict__ stats_prev; // [M] (mu, r) of the old sums
     const float *__restrict__ gamma;       // [N] pending LayerNorm of the old sums
     const float *__restrict__ beta;        // [N]
-    float2 *parts;                         // [N / 128][part_stride] partial (sum, sumsq) of the new sums
+    float2 *parts;                         // [N / GEMM_EPI_COLS][part_stride] partial (sum, sumsq) of the new sums
     int64_t part_stride;
     int M, N, ld;
 
     static constexpr int kUnrollChunks = 4;
-    // The residual epilogues move 327 KB per 128 x 256 tile (fp32 sums read + written, fp16 copy written) against a 3-13 us
-    // mainloop: they are HBM-bound, and with one 4 KB chunk per warp in flight the 8 epilogue warps of an SM sustain ~25 GB/s
-    // (3.65 TB/s over the chip; out-proj 152 us against an 85 us traffic floor).  Requesting two chunks ahead needs a third
-    // 32-register buffer: with the 168 registers a 10-warp CTA can have (warps are allocated in fours) it spills, and measured
-    // SLOWER on a B200 (14.5-14.8 ms per step against 13.9-14.1: profiles/r02_variants.md), so the distance stays 1.
-    // Asking L2 for the next tile's rows one tile ahead (prefetch.global.L2, no registers) was also measured: 14.07 ms (one
-    // request per 128 bytes) and 14.21 ms (per 32-byte sector) against 13.90-13.94 ms without, same box, same run -- the step
-    // runs against the board's power cap (SM clock 1.5-1.7 GHz of 1.965), and extra requests in flight cost more clock than the
-    // shorter load latency returns.
+    // The residual epilogues are HBM-bound (fp32 sums read + written, fp16 copy written per element).  The old sums of the
+    // next 32-column chunk are requested one chunk ahead; a larger distance needs one more 32-register buffer per thread.
 #ifndef AC_RESID_PREFETCH
 #define AC_RESID_PREFETCH 1
 #endif
@@ -252,15 +244,16 @@ struct EpiResidDefer {
     struct State {
         float4 res[kPrefetchDist + 1][8];  // old sums of 32-column chunks (transposed-phase layout), one buffer more than the distance
         float2 ms[4];                      // (mu, r) of this lane's 4 rows (r8 + 8 i)
-        float sum[4], sq[4];               // running partials of the new sums over this warp's 128 columns
+        float sum[4], sq[4];               // running partials of the new sums over this warp's GEMM_EPI_COLS columns
     };
+    __device__ __forceinline__ bool skip_kernel() const { return false; }
     __device__ __forceinline__ void begin_cta(State &, int, int) const {}
     __device__ __forceinline__ void end_cta(State &, int, int) const {}
 
-    __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &ti, int, int col0, int lane, int buf) const {
-        const int row_base = ti.m0 + ((threadIdx.x >> 5) & 3) * 32;
+    __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &ti, int row, int col0, int lane, int buf) const {
+        const int row_base = row - lane;
         const int r8 = lane >> 2, c = lane & 3;
-        if (((col0 - ti.n0) & (GEMM_BLOCK_N / 2 - 1)) == 0) {           // first chunk of this warp's column half
+        if (((col0 - ti.n0) & (GEMM_EPI_COLS - 1)) == 0) {              // first chunk of this warp's column half
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int grow = row_base + r8 + 8 * i;
@@ -283,9 +276,9 @@ struct EpiResidDefer {
         }
     }
 
-    __device__ __forceinline__ void tile(State &st, const GemmTileInfo &ti, int, int col0, const float (&v)[32], uint8_t *stage,
-                                         int lane, int buf, uint32_t) const {
-        const int row_base = ti.m0 + ((threadIdx.x >> 5) & 3) * 32;
+    __device__ __forceinline__ void tile(State &st, const GemmTileInfo &ti, int row, int col0, const float (&v)[32], uint8_t *stage,
+                                         int lane, int buf, const float *) const {
+        const int row_base = row - lane;
         if (row_base >= M || col0 >= N) return;                              // warp-uniform
         const int r8 = lane >> 2, c = lane & 3;
 #pragma unroll
@@ -325,8 +318,8 @@ struct EpiResidDefer {
             }
             __syncwarp();
         }
-        if (((col0 - ti.n0) & (GEMM_BLOCK_N / 2 - 1)) == GEMM_BLOCK_N / 2 - 32) {   // last chunk of this warp's column half
-            const int part = col0 / (GEMM_BLOCK_N / 2);
+        if (((col0 - ti.n0) & (GEMM_EPI_COLS - 1)) == GEMM_EPI_COLS - 32) {   // last chunk of this warp's column half
+            const int part = col0 / GEMM_EPI_COLS;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 float s = st.sum[i], q = st.sq[i];
@@ -341,10 +334,9 @@ struct EpiResidDefer {
     }
 };
 
-// (sum, sumsq) partials of every 128-column part -> (mu, 1/sqrt(var + eps)) per row; parts are added in a fixed order.
-// Kept as a kernel of its own (24 launches of ~3 us per forward): folding these six loads + rsqrt into the consuming epilogues
-// was measured on a B200 and LOST 1 ms per step (35.5 k instead of 37.7 k queries/s, profiles/r02_bench_lnstats_folded.json):
-// the loads sit at the head of every tile's epilogue, which is the critical path of the HBM-bound residual GEMMs.
+// (sum, sumsq) partials of every GEMM_EPI_COLS-column part -> (mu, 1/sqrt(var + eps)) per row; parts are added in a fixed order.
+// Kept as a kernel of its own: folding these loads + rsqrt into the consuming epilogues puts them at the head of every tile's
+// epilogue, which is the critical path of the HBM-bound residual GEMMs.
 __global__ void ln_stats_kernel(const float2 *__restrict__ parts, int nparts, int64_t part_stride, int rows, int H, float eps,
                                 float2 *__restrict__ stats) {
     const int row = blockIdx.x * blockDim.x + threadIdx.x;
@@ -533,17 +525,79 @@ __global__ void to_half_kernel(const float *__restrict__ in, __half *__restrict_
 }
 
 // ------------------------------------------------------------------------------------------------
-// attention: one CTA (128 threads) per (sequence b, head h); S <= 128, head_dim == 64, fp16 operands.
-//   scores[128x128] = Q K^T        4 x tcgen05.mma kind::f16 (M128 N128 K16), accumulator TMEM cols [0,128)
-//   P = exp(scale*(s - max)) masked  thread = query row, tcgen05.ld 32x32b; P -> smem (swizzled fp16)
-//   out[128x64] = P V              8 x tcgen05.mma (M128 N64 K16), accumulator TMEM cols [0,64) (scores already drained)
+// attention: one CTA (128 threads = one warpgroup) per (sequence b, head h); S <= 128, head_dim == 64, fp16 operands.
+//   scores[128x128] = Q K^T        2 x 4 wgmma m64n128k16 (query rows 0-63, 64-127), fp32 fragments -> smem score tile
+//   P = exp(scale*(s - max)) masked  thread = query row, reads its score row; P held in registers, then -> smem (swizzled fp16)
+//   out[128x64] = P V              2 x 8 wgmma m64n64k16, fragments -> smem
 //   ctx[row, h*64 + :] = out / rowsum  (fp16: the A operand of the output projection)
-// smem: Q tile 16 KB | K tile 16 KB (TMA, 128B swizzle), reused for P (2 slabs x 16 KB); V^T 2 slabs x 8 KB by TMA
-// from the transposed buffer the QKV epilogue wrote.  48 KB + 128 TMEM columns per CTA -> 4 CTAs per SM.
+// smem: one 68 KB region that holds, in turn, the Q and K tiles (16 KB each, TMA, 128B swizzle), the fp32 score tile, P
+// (2 slabs x 16 KB) and the output tile; then V^T (2 slabs x 8 KB by TMA from the transposed buffer the QKV epilogue wrote).
+// 85 KB per CTA: two CTAs share an SM, so one CTA's softmax overlaps the other's loads and MMAs.
 // ------------------------------------------------------------------------------------------------
 constexpr int ATT_THREADS = 128;
-constexpr int ATT_SMEM = 48 * 1024 + 1024 /*align*/ + 64;
-constexpr int ATT_TMEM_COLS = 128;
+constexpr int ATT_S_LD = 128 + 4;                            // score tile row stride (floats): conflict-free row reads
+constexpr int ATT_S_BYTES = 128 * ATT_S_LD * 4;
+constexpr int ATT_REGION_BYTES = (ATT_S_BYTES + 1023) / 1024 * 1024;
+constexpr int ATT_SMEM = ATT_REGION_BYTES + 16 * 1024 + 1024 /*align*/ + 64;
+static_assert(2 * (ATT_SMEM + 1024) <= 228 * 1024, "two attention CTAs must fit one SM");
+
+// S[128 x 128] = Q K^T for the query tile sQ and key tile sK (both [128 rows x 128 B], 128B swizzle) -> sS (fp32, ld ATT_S_LD).
+// Issued by the whole warpgroup; returns once the products are in shared memory (the caller synchronises the CTA).
+__device__ __forceinline__ void att_scores(const uint8_t *sQ, const uint8_t *sK, float *sS) {
+    const uint64_t bd = wgmma_desc_sw128(smem_u32(sK));
+#pragma unroll 1
+    for (int half = 0; half < 2; ++half) {
+        float s[64];
+        const uint64_t a = wgmma_desc_sw128(smem_u32(sQ + half * 8192));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(s, a + 2 * k, bd + 2 * k, k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_store_acc(s, sS + half * 64 * ATT_S_LD, ATT_S_LD);
+    }
+}
+// O[128 x 64] (+)= P V with P = 2 slabs x [128 rows x 64 keys] and V^T = 2 slabs x [64 (d) x 64 keys] in shared memory
+__device__ __forceinline__ void att_pv(const uint8_t *sP, const uint8_t *sVt, float (&o)[2][32], bool accumulate) {
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+        wgmma_fence();
+#pragma unroll
+        for (int slab = 0; slab < 2; ++slab) {
+            const uint64_t a = wgmma_desc_sw128(smem_u32(sP + slab * 16384 + half * 8192));
+            const uint64_t bd = wgmma_desc_sw128(smem_u32(sVt + slab * 8192));
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_m64n64_f16(o[half], a + 2 * k, bd + 2 * k, accumulate || (slab | k) != 0);
+        }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+}
+// P row qrow (32 keys from column c) as fp16 into the swizzled P slabs: slab (c / 64), 4 x 16-byte chunks
+__device__ __forceinline__ void att_store_p(uint32_t sp_base, int qrow, int c, const uint32_t *pk) {
+    const uint32_t prow = sp_base + (c >> 6) * 16384 + (qrow >> 3) * 1024 + (qrow & 7) * 128;
+    const int ch0 = (c & 63) >> 3;
+#pragma unroll
+    for (int ch = 0; ch < 4; ++ch) {
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(prow + (((ch0 + ch) ^ (qrow & 7)) << 4)),
+                     "r"(pk[4 * ch]), "r"(pk[4 * ch + 1]), "r"(pk[4 * ch + 2]), "r"(pk[4 * ch + 3])
+                     : "memory");
+    }
+}
+// ctx[dst row, 0..63] = fp16(out row * inv), out row read from the smem tile
+__device__ __forceinline__ void att_write_row(const float *orow, float inv, __half *dst) {
+#pragma unroll
+    for (int c = 0; c < 64; c += 8) {
+        const float4 a = *reinterpret_cast<const float4 *>(orow + c);
+        const float4 b = *reinterpret_cast<const float4 *>(orow + c + 4);
+        __half2 h0 = __floats2half2_rn(a.x * inv, a.y * inv), h1 = __floats2half2_rn(a.z * inv, a.w * inv);
+        __half2 h2 = __floats2half2_rn(b.x * inv, b.y * inv), h3 = __floats2half2_rn(b.z * inv, b.w * inv);
+        uint4 pk;
+        pk.x = *reinterpret_cast<uint32_t *>(&h0); pk.y = *reinterpret_cast<uint32_t *>(&h1);
+        pk.z = *reinterpret_cast<uint32_t *>(&h2); pk.w = *reinterpret_cast<uint32_t *>(&h3);
+        *reinterpret_cast<uint4 *>(dst + c) = pk;
+    }
+}
 
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
@@ -552,11 +606,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                    // [128 rows x 128 B]
     uint8_t *sK = smem + 16 * 1024;        // [128 rows x 128 B]
-    uint8_t *sP = smem;                    // 2 slabs x [128 rows x 128 B (64 keys)]   (after QK^T retired)
-    uint8_t *sVt = smem + 32 * 1024;       // 2 slabs x [64 rows (d) x 128 B (64 keys)]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 48 * 1024);
-    uint64_t *bar_load = bars, *bar_s = bars + 1, *bar_o = bars + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 3);
+    float *sS = reinterpret_cast<float *>(smem);   // score tile, then output tile (after QK^T / PV retired)
+    uint8_t *sP = smem;                    // 2 slabs x [128 rows x 128 B (64 keys)]   (after every score row was read)
+    uint8_t *sVt = smem + ATT_REGION_BYTES;  // 2 slabs x [64 rows (d) x 128 B (64 keys)]
+    uint64_t *bar_load = reinterpret_cast<uint64_t *>(smem + ATT_REGION_BYTES + 16 * 1024);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int b = blockIdx.x / heads, h = blockIdx.x % heads;
@@ -566,19 +619,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
         tma_prefetch_desc(&tmap_qk);
         tma_prefetch_desc(&tmap_vt);
         mbar_init(bar_load, 1);
-        mbar_init(bar_s, 1);
-        mbar_init(bar_o, 1);
         fence_mbar_init();
     }
-    if (warp == 0) {
-        tmem_alloc(tmem_slot, ATT_TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
     if (tid == 0) {
         mbar_arrive_expect_tx(bar_load, 48 * 1024);
         const int r = static_cast<int>(row0);
@@ -587,23 +630,29 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
         const int vrow = (b * heads + h) * 64;                 // rows (b, h, d) of the transposed V buffer
         tma_load_2d(sVt, &tmap_vt, bar_load, 0, vrow);
         tma_load_2d(sVt + 8 * 1024, &tmap_vt, bar_load, 64, vrow);
-        // ---- S = Q K^T
-        mbar_wait_guarded(bar_load, 0);
-        tc_fence_after();
-        constexpr uint32_t idesc_s = umma_idesc(0 /*f16*/, 128, 128);
-        const uint64_t a = umma_desc_sw128(smem_u32(sQ));
-        const uint64_t bdesc = umma_desc_sw128(smem_u32(sK));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16(tmem_base, a + 2 * k, bdesc + 2 * k, idesc_s, k != 0);
-        tc_commit(bar_s);
     }
-    __syncwarp();
-    mbar_wait_guarded(bar_s, 0);
-    tc_fence_after();
+    // ---- S = Q K^T: both 64-row chains retire before the score tile overwrites Q and K
+    mbar_wait_guarded(bar_load, 0);
+    {
+        float s0[64], s1[64];
+        const uint64_t bd = wgmma_desc_sw128(smem_u32(sK));
+        const uint64_t a0 = wgmma_desc_sw128(smem_u32(sQ)), a1 = wgmma_desc_sw128(smem_u32(sQ + 8192));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(s0, a0 + 2 * k, bd + 2 * k, k != 0);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(s1, a1 + 2 * k, bd + 2 * k, k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncthreads();
+        wgmma_store_acc(s0, sS, ATT_S_LD);
+        wgmma_store_acc(s1, sS + 64 * ATT_S_LD, ATT_S_LD);
+    }
+    __syncthreads();
 
-    // ---- softmax: thread = query row (TMEM lane), two passes over the 128 score columns
+    // ---- softmax: thread = query row, two passes over the 128 score columns
     const int qrow = warp * 32 + lane;
-    const uint32_t t_s = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
+    const float *srow = sS + qrow * ATT_S_LD;
     // key validity (key < S and not padded) as four 32-bit words held by every thread: lane l of a warp tests key
     // 32*w + l once, ballots, and the loops below only test bits
     uint32_t kmask[4];
@@ -617,103 +666,58 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     float mx = -CUDART_INF_F;
 #pragma unroll 1
     for (int c = 0; c < 128; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_s + c, r);
-        tmem_ld_wait();
+        float r[32];
+        acc_row_ld32(srow + c, r);
         const uint32_t km = c == 0 ? kmask[0] : c == 32 ? kmask[1] : c == 64 ? kmask[2] : kmask[3];
 #pragma unroll
         for (int j = 0; j < 32; ++j)
-            if ((km >> j) & 1u) mx = fmaxf(mx, __uint_as_float(r[j]));
+            if ((km >> j) & 1u) mx = fmaxf(mx, r[j]);
     }
     float sum = 0.f;
-    const uint32_t sp_base = smem_u32(sP);
-#pragma unroll 1
-    for (int c = 0; c < 128; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_s + c, r);
-        tmem_ld_wait();
-        uint32_t pk[16];
-        const uint32_t km = c == 0 ? kmask[0] : c == 32 ? kmask[1] : c == 64 ? kmask[2] : kmask[3];
+    uint32_t pk[64];                       // the whole P row: P overwrites score rows other threads may still be reading
+#pragma unroll
+    for (int ci = 0; ci < 4; ++ci) {
+        float r[32];
+        acc_row_ld32(srow + 32 * ci, r);
+        const uint32_t km = kmask[ci];
         const float mxs = mx * scale_log2;
 #pragma unroll
         for (int j = 0; j < 32; j += 2) {
-            const float e0 = ((km >> j) & 1u) ? ex2_approx(fmaf(__uint_as_float(r[j]), scale_log2, -mxs)) : 0.f;
-            const float e1 = ((km >> (j + 1)) & 1u) ? ex2_approx(fmaf(__uint_as_float(r[j + 1]), scale_log2, -mxs)) : 0.f;
+            const float e0 = ((km >> j) & 1u) ? ex2_approx(fmaf(r[j], scale_log2, -mxs)) : 0.f;
+            const float e1 = ((km >> (j + 1)) & 1u) ? ex2_approx(fmaf(r[j + 1], scale_log2, -mxs)) : 0.f;
             sum += e0 + e1;
             __half2 hh = __floats2half2_rn(e0, e1);
-            pk[j >> 1] = *reinterpret_cast<uint32_t *>(&hh);
-        }
-        // slab (c / 64), row qrow: 4 x 16-byte chunks (8 keys each) starting at chunk (c % 64) / 8
-        const uint32_t prow = sp_base + (c >> 6) * 16384 + (qrow >> 3) * 1024 + (qrow & 7) * 128;
-        const int ch0 = (c & 63) >> 3;
-#pragma unroll
-        for (int ch = 0; ch < 4; ++ch) {
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(prow + (((ch0 + ch) ^ (qrow & 7)) << 4)),
-                         "r"(pk[4 * ch]), "r"(pk[4 * ch + 1]), "r"(pk[4 * ch + 2]), "r"(pk[4 * ch + 3])
-                         : "memory");
+            pk[16 * ci + (j >> 1)] = *reinterpret_cast<uint32_t *>(&hh);
         }
     }
-    // generic-proxy smem writes (P) -> visible to the tensor-core (async) proxy; all threads are done reading S
+    __syncthreads();                       // every score row has been read
+    const uint32_t sp_base = smem_u32(sP);
+#pragma unroll
+    for (int ci = 0; ci < 4; ++ci) att_store_p(sp_base, qrow, 32 * ci, pk + 16 * ci);
+    // generic-proxy smem writes (P) -> visible to the tensor-core (async) proxy
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
 
-    // ---- O = P V   (accumulates into TMEM columns [0,64): the score tile is dead)
-    if (tid == 0) {
-        constexpr uint32_t idesc_o = umma_idesc(0 /*f16*/, 128, 64);
-#pragma unroll
-        for (int slab = 0; slab < 2; ++slab) {
-            const uint64_t a = umma_desc_sw128(smem_u32(sP + slab * 16384));
-            const uint64_t bdesc = umma_desc_sw128(smem_u32(sVt + slab * 8192));
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(tmem_base, a + 2 * k, bdesc + 2 * k, idesc_o, (slab | k) != 0);
-        }
-        tc_commit(bar_o);
-    }
-    __syncwarp();
-    mbar_wait_guarded(bar_o, 0);
-    tc_fence_after();
-
+    // ---- O = P V, staged over P once every warp's MMAs have read it
+    float o[2][32];
+    att_pv(sP, sVt, o, false);
+    __syncthreads();
+    wgmma_store_acc(o[0], sS, ATT_S_LD);
+    wgmma_store_acc(o[1], sS + 64 * ATT_S_LD, ATT_S_LD);
+    __syncthreads();
     const float inv = (sum > 0.f) ? 1.f / sum : 0.f;
-#pragma unroll 1
-    for (int c = 0; c < 64; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_s + c, r);
-        tmem_ld_wait();
-        if (qrow < S) {
-            __half *dst = ctx + (row0 + qrow) * H + h * 64 + c;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-                __half2 h0 = __floats2half2_rn(__uint_as_float(r[j]) * inv, __uint_as_float(r[j + 1]) * inv);
-                __half2 h1 = __floats2half2_rn(__uint_as_float(r[j + 2]) * inv, __uint_as_float(r[j + 3]) * inv);
-                __half2 h2 = __floats2half2_rn(__uint_as_float(r[j + 4]) * inv, __uint_as_float(r[j + 5]) * inv);
-                __half2 h3 = __floats2half2_rn(__uint_as_float(r[j + 6]) * inv, __uint_as_float(r[j + 7]) * inv);
-                uint4 pk;
-                pk.x = *reinterpret_cast<uint32_t *>(&h0); pk.y = *reinterpret_cast<uint32_t *>(&h1);
-                pk.z = *reinterpret_cast<uint32_t *>(&h2); pk.w = *reinterpret_cast<uint32_t *>(&h3);
-                *reinterpret_cast<uint4 *>(dst + j) = pk;
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, ATT_TMEM_COLS);
-    }
+    if (qrow < S) att_write_row(srow, inv, ctx + (row0 + qrow) * H + h * 64);
 }
 
 // ------------------------------------------------------------------------------------------------
 // attention for 128 < S <= 512: one CTA per (sequence, head, 128-query block), key blocks of 128 streamed twice.
 //   pass A  row max over all key blocks        (QK^T only)
-//   pass B  P = exp(scale*(s - max)) per block, O += P V_block accumulated in TMEM, row sums in registers
-// Using the final max in pass B means the TMEM accumulator never has to be rescaled; the price is computing QK^T
-// twice (QK^T is half of the attention flops, attention is ~3 % of the encoder).  Serial per block (TMA -> MMA ->
+//   pass B  P = exp(scale*(s - max)) per block, O += P V_block accumulated in the wgmma registers, row sums in registers
+// Using the final max in pass B means the accumulator never has to be rescaled; the price is computing QK^T
+// twice (QK^T is half of the attention flops, attention is a few % of the encoder).  Serial per block (TMA -> MMA ->
 // softmax -> MMA); the S <= 128 kernel above is the tuned path of the benchmark configurations.
 // ------------------------------------------------------------------------------------------------
-constexpr int ATTL_SMEM = 80 * 1024 + 1024 + 64;
-constexpr int ATTL_TMEM_COLS = 256;
+constexpr int ATTL_SMEM = 80 * 1024 + ATT_S_BYTES + 1024 + 64;
 
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
@@ -724,9 +728,8 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
     uint8_t *sK = smem + 16 * 1024;        // [128 x 128 B] current key block
     uint8_t *sVt = smem + 32 * 1024;       // 2 slabs x [64 (d) x 128 B (64 keys)]
     uint8_t *sP = smem + 48 * 1024;        // 2 slabs x [128 x 128 B (64 keys)]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 80 * 1024);
-    uint64_t *bar_load = bars, *bar_s = bars + 1, *bar_o = bars + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 3);
+    float *sS = reinterpret_cast<float *>(smem + 80 * 1024);
+    uint64_t *bar_load = reinterpret_cast<uint64_t *>(smem + 80 * 1024 + ATT_S_BYTES);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int b = blockIdx.x / heads, h = blockIdx.x % heads;
@@ -739,27 +742,17 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
         tma_prefetch_desc(&tmap_qk);
         tma_prefetch_desc(&tmap_vt);
         mbar_init(bar_load, 1);
-        mbar_init(bar_s, 1);
-        mbar_init(bar_o, 1);
         fence_mbar_init();
     }
-    if (warp == 0) {
-        tmem_alloc(tmem_slot, ATTL_TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t t_s = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
     const int qrow = warp * 32 + lane;                            // row inside the query block
     const int qglob = qb * 128 + qrow;                            // position inside the sequence
+    const float *srow = sS + qrow * ATT_S_LD;
     const float scale_log2 = rsqrtf(64.f) * 1.44269504088896340736f;
-    constexpr uint32_t idesc_s = umma_idesc(0, 128, 128);
-    constexpr uint32_t idesc_o = umma_idesc(0, 128, 64);
 
-    uint32_t ph_load = 0, ph_s = 0, ph_o = 0;
+    uint32_t ph_load = 0;
     float mx = -CUDART_INF_F, sum = 0.f;
+    float o[2][32];
 
     for (int pass = 0; pass < 2; ++pass) {
         for (int j = 0; j < nkb; ++j) {
@@ -774,19 +767,11 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
                     tma_load_2d(sVt, &tmap_vt, bar_load, key0, vrow);
                     tma_load_2d(sVt + 8 * 1024, &tmap_vt, bar_load, key0 + 64, vrow);
                 }
-                mbar_wait_guarded(bar_load, ph_load);
-                tc_fence_after();
-                const uint64_t a = umma_desc_sw128(smem_u32(sQ));
-                const uint64_t bd = umma_desc_sw128(smem_u32(sK));
-#pragma unroll
-                for (int k = 0; k < 4; ++k) umma_f16(tmem_base, a + 2 * k, bd + 2 * k, idesc_s, k != 0);
-                tc_commit(bar_s);
             }
+            mbar_wait_guarded(bar_load, ph_load);
             ph_load ^= 1;
-            __syncwarp();
-            mbar_wait_guarded(bar_s, ph_s);
-            ph_s ^= 1;
-            tc_fence_after();
+            att_scores(sQ, sK, sS);
+            __syncthreads();
 
             // key validity bits of this block
             uint32_t kmask[4];
@@ -799,95 +784,47 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
             if (pass == 0) {
 #pragma unroll
                 for (int ci = 0; ci < 4; ++ci) {
-                    uint32_t r[32];
-                    tmem_ld_32x32(t_s + 32 * ci, r);
-                    tmem_ld_wait();
+                    float r[32];
+                    acc_row_ld32(srow + 32 * ci, r);
                     const uint32_t km = kmask[ci];
 #pragma unroll
                     for (int jj = 0; jj < 32; ++jj)
-                        if ((km >> jj) & 1u) mx = fmaxf(mx, __uint_as_float(r[jj]));
+                        if ((km >> jj) & 1u) mx = fmaxf(mx, r[jj]);
                 }
-                tc_fence_before();
-                __syncthreads();                                  // S columns and sK may be overwritten now
-                tc_fence_after();
+                __syncthreads();                                  // the score tile and sK may be overwritten now
             } else {
                 const uint32_t sp_base = smem_u32(sP);
                 const float mxs = mx * scale_log2;
 #pragma unroll
                 for (int ci = 0; ci < 4; ++ci) {
                     const int c = 32 * ci;
-                    uint32_t r[32];
-                    tmem_ld_32x32(t_s + c, r);
-                    tmem_ld_wait();
+                    float r[32];
+                    acc_row_ld32(srow + c, r);
                     const uint32_t km = kmask[ci];
                     uint32_t pk[16];
 #pragma unroll
                     for (int jj = 0; jj < 32; jj += 2) {
-                        const float e0 = ((km >> jj) & 1u) ? ex2_approx(fmaf(__uint_as_float(r[jj]), scale_log2, -mxs)) : 0.f;
-                        const float e1 = ((km >> (jj + 1)) & 1u) ? ex2_approx(fmaf(__uint_as_float(r[jj + 1]), scale_log2, -mxs)) : 0.f;
+                        const float e0 = ((km >> jj) & 1u) ? ex2_approx(fmaf(r[jj], scale_log2, -mxs)) : 0.f;
+                        const float e1 = ((km >> (jj + 1)) & 1u) ? ex2_approx(fmaf(r[jj + 1], scale_log2, -mxs)) : 0.f;
                         sum += e0 + e1;
                         __half2 hh = __floats2half2_rn(e0, e1);
                         pk[jj >> 1] = *reinterpret_cast<uint32_t *>(&hh);
                     }
-                    const uint32_t prow = sp_base + (c >> 6) * 16384 + (qrow >> 3) * 1024 + (qrow & 7) * 128;
-                    const int ch0 = (c & 63) >> 3;
-#pragma unroll
-                    for (int ch = 0; ch < 4; ++ch) {
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(prow + (((ch0 + ch) ^ (qrow & 7)) << 4)),
-                                     "r"(pk[4 * ch]), "r"(pk[4 * ch + 1]), "r"(pk[4 * ch + 2]), "r"(pk[4 * ch + 3])
-                                     : "memory");
-                    }
+                    att_store_p(sp_base, qrow, c, pk);
                 }
                 fence_proxy_async_smem();
-                tc_fence_before();
                 __syncthreads();
-                tc_fence_after();
-                if (tid == 0) {
-#pragma unroll
-                    for (int slab = 0; slab < 2; ++slab) {
-                        const uint64_t a = umma_desc_sw128(smem_u32(sP + slab * 16384));
-                        const uint64_t bd = umma_desc_sw128(smem_u32(sVt + slab * 8192));
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_f16(tmem_base + 128, a + 2 * k, bd + 2 * k, idesc_o, (j | slab | k) != 0);
-                    }
-                    tc_commit(bar_o);
-                }
-                __syncwarp();
-                mbar_wait_guarded(bar_o, ph_o);                   // sK / sVt / sP / S columns are free again
-                ph_o ^= 1;
-                tc_fence_after();
+                att_pv(sP, sVt, o, j != 0);
+                __syncthreads();                                  // sK / sVt / sP / the score tile are free again
             }
         }
     }
 
-    const float inv = (sum > 0.f) ? 1.f / sum : 0.f;
-#pragma unroll 1
-    for (int c = 0; c < 64; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_s + 128 + c, r);
-        tmem_ld_wait();
-        if (qglob < S) {
-            __half *dst = ctx + (row0 + qglob) * H + h * 64 + c;
-#pragma unroll
-            for (int jj = 0; jj < 32; jj += 8) {
-                __half2 h0 = __floats2half2_rn(__uint_as_float(r[jj]) * inv, __uint_as_float(r[jj + 1]) * inv);
-                __half2 h1 = __floats2half2_rn(__uint_as_float(r[jj + 2]) * inv, __uint_as_float(r[jj + 3]) * inv);
-                __half2 h2 = __floats2half2_rn(__uint_as_float(r[jj + 4]) * inv, __uint_as_float(r[jj + 5]) * inv);
-                __half2 h3 = __floats2half2_rn(__uint_as_float(r[jj + 6]) * inv, __uint_as_float(r[jj + 7]) * inv);
-                uint4 pk;
-                pk.x = *reinterpret_cast<uint32_t *>(&h0); pk.y = *reinterpret_cast<uint32_t *>(&h1);
-                pk.z = *reinterpret_cast<uint32_t *>(&h2); pk.w = *reinterpret_cast<uint32_t *>(&h3);
-                *reinterpret_cast<uint4 *>(dst + jj) = pk;
-            }
-        }
-    }
-    tc_fence_before();
+    wgmma_store_acc(o[0], sS, ATT_S_LD);
+    wgmma_store_acc(o[1], sS + 64 * ATT_S_LD, ATT_S_LD);
     __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, ATTL_TMEM_COLS);
-    }
+    const float inv = (sum > 0.f) ? 1.f / sum : 0.f;
+    if (qglob < S) att_write_row(srow, inv, ctx + (row0 + qglob) * H + h * 64);
 }
 
 // last layer, deferred flow: CLS rows of the attention context and of LN_pending(y) (two-pass statistics from the fp32 sums)
@@ -940,7 +877,7 @@ struct ac_encoder {
     int vt_B = -1, vt_S = -1;
     std::vector<CUtensorMap> p_wqkv_d, p_wo, p_w1_d, p_w2;
     CUtensorMap p_w1_last;
-    // row statistics (ping-pong) and the per-128-column partials the residual epilogues write
+    // row statistics (ping-pong) and the per-GEMM_EPI_COLS-column partials the residual epilogues write
     float2 *stats_a = nullptr, *stats_b = nullptr, *stats_id = nullptr, *parts = nullptr;
     float *ones = nullptr, *zeros = nullptr;
     std::vector<void *> allocs;
@@ -1074,7 +1011,7 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     TRY(dev_alloc(e, &e->stats_a, T));
     TRY(dev_alloc(e, &e->stats_b, T));
     TRY(dev_alloc(e, &e->stats_id, T));
-    TRY(dev_alloc(e, &e->parts, static_cast<size_t>(H / 128) * T));
+    TRY(dev_alloc(e, &e->parts, static_cast<size_t>(H / GEMM_EPI_COLS) * T));
     TRY(dev_alloc(e, &e->ones, H));
     TRY(dev_alloc(e, &e->zeros, H));
     fill_stats_identity_kernel<<<static_cast<unsigned>((T + 255) / 256), 256>>>(e->stats_id, static_cast<int64_t>(T));
@@ -1113,12 +1050,12 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     TRY(make_tmap_2d(&e->m_ffn_cls, e->ffn_cls, 2, e->Bc, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_M, 64));
     e->p_wqkv_d.resize(L); e->p_wo.resize(L); e->p_w1_d.resize(L); e->p_w2.resize(L);
     for (int l = 0; l < L; ++l) {
-        TRY(make_tmap_2d(&e->p_wqkv_d[l], e->wqkv_d[l], 2, 3 * H, H, static_cast<uint64_t>(H) * 2, GEMM2_B_ROWS, 64));
-        TRY(make_tmap_2d(&e->p_wo[l], e->wo[l], 2, H, H, static_cast<uint64_t>(H) * 2, GEMM2_B_ROWS, 64));
-        TRY(make_tmap_2d(&e->p_w1_d[l], e->w1_d[l], 2, I, H, static_cast<uint64_t>(H) * 2, GEMM2_B_ROWS, 64));
-        TRY(make_tmap_2d(&e->p_w2[l], e->w2[l], 2, H, I, static_cast<uint64_t>(I) * 2, GEMM2_B_ROWS, 64));
+        TRY(make_tmap_2d(&e->p_wqkv_d[l], e->wqkv_d[l], 2, 3 * H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+        TRY(make_tmap_2d(&e->p_wo[l], e->wo[l], 2, H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+        TRY(make_tmap_2d(&e->p_w1_d[l], e->w1_d[l], 2, I, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+        TRY(make_tmap_2d(&e->p_w2[l], e->w2[l], 2, H, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_N, 64));
     }
-    if (cfg->cls_only) TRY(make_tmap_2d(&e->p_w1_last, e->w1_last, 2, I, H, static_cast<uint64_t>(H) * 2, GEMM2_B_ROWS, 64));
+    if (cfg->cls_only) TRY(make_tmap_2d(&e->p_w1_last, e->w1_last, 2, I, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
     TRY(check_cuda(cudaDeviceSynchronize(), "encoder_create sync"));
 #undef TRY
     *out = e;
@@ -1128,14 +1065,12 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
 using EpiGelu = EpiLinear<1, true, false>;                  // bias + GELU, fp16 out                       (CLS-only tail)
 using EpiResid = EpiLinear<2, false, false>;                // bias + residual, fp32 out (pre-LayerNorm sum, CLS-only tail)
 using EpiQKVDefer = EpiLinear<0, true, true, true>;         // r (acc - mu c1) + c0, fp16 out, V third transposed
-using EpiGeluDefer16 = EpiLinear<1, true, false, true, 64>; // GELU(r (acc - mu c1) + c0), fp16 out; 16 epilogue warps x 64 columns
+using EpiGeluDefer = EpiLinear<1, true, false, true>;       // GELU(r (acc - mu c1) + c0), fp16 out
 
-// One encoder projection = one CTA-pair GEMM (gemm_tc2.cuh).  tb is the weight's 128-row-box map.  The bias + GELU epilogue of
-// FFN1 issues ~17 instructions per element, which two warps per scheduler cannot hide behind a K = 768 mainloop: it runs with
-// 16 epilogue warps (measured on a B200: -0.65 ms per 12-layer forward at B*S = 65536, profiles/r02_variants.md).
-template <class Epi, int kEpiWarps = GEMM_EPI_WARPS>
+// One encoder projection = one GEMM (gemm_tc.cuh).  tb is the weight's GEMM_BLOCK_N-row-box map.
+template <class Epi>
 static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, int N, int K, const Epi &epi, cudaStream_t s) {
-    return launch_gemm_tc2<Epi, false, GEMM_KIND_F16, kEpiWarps>(ta, tb, M, N, K, epi, s);
+    return launch_gemm_tc<Epi, false, GEMM_KIND_F16>(ta, tb, M, N, K, epi, s);
 }
 
 extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids,
@@ -1164,7 +1099,7 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
     }
     const int wpb = 8;
     const int row_blocks = (M + wpb - 1) / wpb;
-    const int nparts = H / 128;
+    const int nparts = H / GEMM_EPI_COLS;
     const int64_t pstride = static_cast<int64_t>(e->T);
 
     // e->x holds the un-normalised residual sums y, e->xh their fp16 copy; the LayerNorm still pending on y is carried as
@@ -1209,8 +1144,8 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
         if ((rc = launch_linear(e->m_ctx, e->p_wo[l], M, H, H, eo, s))) return rc;
         ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
         AC_LAUNCH_CHECK();
-        EpiGeluDefer16 e1{e->c0f[l], nullptr, e->ffn, M, I, I, 0, nullptr, 0, 0, 0, 0, e->c1f[l], e->stats_b};
-        if ((rc = launch_linear<EpiGeluDefer16, 16>(e->m_xh, e->p_w1_d[l], M, I, H, e1, s))) return rc;
+        EpiGeluDefer e1{e->c0f[l], nullptr, e->ffn, M, I, I, 0, nullptr, 0, 0, 0, 0, e->c1f[l], e->stats_b};
+        if ((rc = launch_linear(e->m_xh, e->p_w1_d[l], M, I, H, e1, s))) return rc;
         // FFN output projection + residual: y <- ffn W2^T + b2 + LN_attention_output(y)
         EpiResidDefer e2{e->b2[l], e->x, e->xh, e->stats_b, e->ln1w[l], e->ln1b[l], e->parts, pstride, M, H, H};
         if ((rc = launch_linear(e->m_ffn, e->p_w2[l], M, H, I, e2, s))) return rc;
@@ -1242,14 +1177,14 @@ extern "C" int ac_encoder_last_hidden(ac_encoder *e, float *out, int64_t n_float
     return AC_OK;
 }
 
-// generic tensor-core linear exposed for parity tests / roofline measurement (the encoder's CTA-pair GEMM with a plain epilogue).
+// generic tensor-core linear exposed for parity tests / roofline measurement (the encoder's GEMM with a plain epilogue).
 //   precision AC_PREC_TF32: X, W fp32 (used as stored, tf32 truncation by the MMA unless pre-rounded), Y fp32
 //   precision AC_PREC_F16 : X, W fp16, Y fp32 (out_half = 0) or fp16 (out_half = 1)
 template <int MODE, bool OUT_HALF, int KIND>
 static int linear_tc_dispatch(const CUtensorMap &ta, const CUtensorMap &tb, const float *bias, const float *residual, void *Y,
                               int M, int N, int K, int round_out, cudaStream_t s) {
     EpiLinear<MODE, OUT_HALF, false> e{bias, residual, Y, M, N, N, round_out, nullptr, 0, 0, 0, 0};
-    return launch_gemm_tc2<EpiLinear<MODE, OUT_HALF, false>, false, KIND>(ta, tb, M, N, K, e, s);
+    return launch_gemm_tc<EpiLinear<MODE, OUT_HALF, false>, false, KIND>(ta, tb, M, N, K, e, s);
 }
 
 extern "C" int ac_linear_tc(const void *X, const void *W, const float *bias, const float *residual, void *Y, int M, int N,
@@ -1265,7 +1200,7 @@ extern "C" int ac_linear_tc(const void *X, const void *W, const float *bias, con
     CUtensorMap ta, tb;
     const uint32_t bk = 128 / es;
     if ((rc = make_tmap_2d(&ta, X, es, M, K, static_cast<uint64_t>(K) * es, GEMM_BLOCK_M, bk))) return rc;
-    if ((rc = make_tmap_2d(&tb, W, es, N, K, static_cast<uint64_t>(K) * es, GEMM2_B_ROWS, bk))) return rc;
+    if ((rc = make_tmap_2d(&tb, W, es, N, K, static_cast<uint64_t>(K) * es, GEMM_BLOCK_N, bk))) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (precision == AC_PREC_TF32) {
         AC_REQUIRE(!out_half, "ac_linear_tc: tf32 path writes fp32");

@@ -1,42 +1,48 @@
-// gemm_tc.cuh -- persistent warp-specialised tcgen05 GEMM mainloop for sm_100a (B200).
+// gemm_tc.cuh -- persistent warp-specialised wgmma GEMM mainloop for sm_90a (H100).
 //
-//   D[M,N] (fp32, TMEM) = A[M,K] * B[N,K]^T      K-major operands, either
-//       kKind = GEMM_KIND_TF32 : fp32 containers holding tf32 values (kind::tf32, 32 elements per 128-byte k-block)
-//       kKind = GEMM_KIND_F16  : fp16 values                         (kind::f16,  64 elements per 128-byte k-block)
+//   D[M,N] (fp32) = A[M,K] * B[N,K]^T      K-major operands, either
+//       kKind = GEMM_KIND_TF32 : fp32 containers holding tf32 values (wgmma .tf32, 32 elements per 128-byte k-block)
+//       kKind = GEMM_KIND_F16  : fp16 values                         (wgmma .f16,  64 elements per 128-byte k-block)
 //   (same bytes per stage, same descriptors; fp16 has tf32's 10-bit mantissa at twice the tensor rate)
 //
-//   warp 0      : TMA producer   (cp.async.bulk.tensor.2d, 128B swizzle, 4-stage mbarrier ring)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (kind::tf32, 128 x BLOCK_N x 8)
-//   warps 2..9  : epilogue (tcgen05.ld 32x32b -> registers -> fused epilogue functor -> global); warp w owns TMEM
-//                 lane quarter w%4 and the column half (w-2)/4 of the 128 x 256 accumulator
+//   warpgroup 2 : TMA producer (one thread: cp.async.bulk.tensor.2d, 128B swizzle, 4-stage mbarrier ring)
+//   warpgroups 0, 1 : consumers.  Warpgroup g issues the wgmma m64n128 chain of tile rows [64 g, 64 g + 64) with the fp32
+//                 accumulator in registers, stores it into its half of a shared-memory accumulator tile, and then runs the
+//                 fused epilogue functor on it: warp w of the warpgroup drains rows 32 (2 g + w % 2) .. + 32 and the column
+//                 half w / 2 (64 columns = two chunks of 32), thread = one accumulator row.
 //
-// Two TMEM accumulator buffers (2 x 256 columns) let the epilogue of tile i overlap the MMAs of tile
-// i+1.  The epilogue is a functor; this 1-CTA mainloop serves the kNN scans (running per-query top-k' lists / threshold
-// collection over prototype tiles), the encoder linears run the CTA-pair variant of gemm_tc2.cuh with the same functor concept.
+// The two consumer warpgroups run independently (each waits only on its own rows), so one warpgroup's epilogue overlaps
+// the other's mainloop, and the producer keeps loading the next tile's stages during both.  This one kernel serves the
+// encoder linears and the kNN scans (running per-query top-k' lists / threshold collection over prototype tiles).
 #pragma once
 #include "common.cuh"
 
 namespace ac {
 
 constexpr int GEMM_BLOCK_M = 128;
-constexpr int GEMM_BLOCK_N = 256;
+constexpr int GEMM_BLOCK_N = 128;
 constexpr int GEMM_BLOCK_K = 32;                    // tf32: fp32 elements per 128-byte swizzle row
 constexpr int GEMM_KIND_TF32 = 0, GEMM_KIND_F16 = 1;
 __host__ __device__ constexpr int gemm_block_k(int kind) { return kind == GEMM_KIND_F16 ? 64 : 32; }
 constexpr int GEMM_STAGES = 4;
-constexpr int GEMM_UMMA_K = 8;                      // tf32: 32 bytes per MMA K-step
-constexpr int GEMM_EPI_WARPS = 8;
-constexpr int GEMM_THREADS = 64 + 32 * GEMM_EPI_WARPS;   // 320
-constexpr int GEMM_A_STAGE_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 4;   // 16 KB
-constexpr int GEMM_B_STAGE_BYTES = GEMM_BLOCK_N * GEMM_BLOCK_K * 4;   // 32 KB
+constexpr int GEMM_EPI_COLS = GEMM_BLOCK_N / 2;     // accumulator columns one epilogue warp drains per tile
+constexpr int GEMM_EPI_WARPS = 8;                   // the consumer warps
+constexpr int GEMM_PRODUCER_THREAD = 32 * GEMM_EPI_WARPS;
+constexpr int GEMM_THREADS = 32 * GEMM_EPI_WARPS + 128; // 384: two consumer warpgroups + the producer warpgroup
+constexpr int GEMM_A_STAGE_BYTES = GEMM_BLOCK_M * 128;  // 16 KB
+constexpr int GEMM_B_STAGE_BYTES = GEMM_BLOCK_N * 128;  // 16 KB
 constexpr int GEMM_STAGE_BYTES = GEMM_A_STAGE_BYTES + GEMM_B_STAGE_BYTES;
+// accumulator tile row stride: +4 floats keeps the thread-per-row 16-byte reads conflict-free
+constexpr int GEMM_ACC_LD = GEMM_BLOCK_N + 4;
+constexpr int GEMM_ACC_BYTES = GEMM_BLOCK_M * GEMM_ACC_LD * 4;  // 66 KB
 // per-epilogue-warp staging tile for the thread-row -> coalesced-row transpose: 32 rows x 80 bytes
 // (16 fp32 or 32 fp16 payload + 16 B pad: conflict-free 16-byte accesses for both the row writes and the
 // transposed reads)
 constexpr int GEMM_EPI_STAGE_ROW_BYTES = 80;
 constexpr int GEMM_EPI_STAGE_BYTES = 32 * GEMM_EPI_STAGE_ROW_BYTES;   // 2560 B per warp
-constexpr int GEMM_SMEM_BYTES = GEMM_STAGES * GEMM_STAGE_BYTES + GEMM_EPI_WARPS * GEMM_EPI_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int GEMM_TMEM_COLS = 512;
+constexpr int GEMM_SMEM_BYTES = GEMM_STAGES * GEMM_STAGE_BYTES + GEMM_ACC_BYTES + GEMM_EPI_WARPS * GEMM_EPI_STAGE_BYTES +
+                                1024 /*align slack*/ + 256 /*barriers*/;
+static_assert(GEMM_SMEM_BYTES <= 227 * 1024, "stage ring + accumulator tile do not fit");
 
 #ifndef AC_MBAR_WATCHDOG
 #define AC_MBAR_WATCHDOG 1
@@ -44,13 +50,11 @@ constexpr int GEMM_TMEM_COLS = 512;
 
 __device__ __forceinline__ void mbar_wait_guarded(uint64_t *bar, uint32_t parity) {
 #if AC_MBAR_WATCHDOG
-    // a broken pipeline must surface as a launch failure, never as a hung GPU box
+    // a broken pipeline must surface as a launch failure, never as a hung GPU.  No printf here: a function call in a
+    // kernel that issues wgmma makes ptxas serialise every wgmma of that kernel.
     uint32_t spins = 0;
     while (!mbar_try_wait(bar, parity)) {
-        if (++spins > (1u << 26)) {
-            printf("ac: mbarrier watchdog fired (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-            __trap();
-        }
+        if (++spins > (1u << 26)) __trap();
     }
 #else
     mbar_wait(bar, parity);
@@ -62,16 +66,21 @@ struct GemmTileInfo {
     int tile_iter;    // how many tiles this CTA has processed before this one
 };
 
+// column half (0 or 1) of the accumulator tile that the calling epilogue warp drains
+__device__ __forceinline__ int gemm_epi_chalf() { return ((threadIdx.x >> 5) >> 1) & 1; }
+
 // Epilogue concept (parameters live in the functor, per-thread running state in Epi::State):
 //   struct Epi { struct State {...};
-//                __device__ bool skip_kernel() const;   (gemm_tc_kernel only: true => every thread returns immediately)
+//                static constexpr int kUnrollChunks, kPrefetchDist;
+//                __device__ bool skip_kernel() const;   (true => every thread returns immediately)
 //                __device__ void begin_cta(State&, int warp_q, int lane) const;
 //                __device__ void prefetch(State&, const GemmTileInfo&, int row, int col0, int lane, int buf) const;
-//                      (issue the global loads chunk (col0) will need into State buffer `buf`; called one chunk ahead)
+//                      (issue the global loads chunk (col0) will need into State buffer `buf`; called kPrefetchDist chunks ahead)
 //                __device__ void tile(State&, const GemmTileInfo&, int row /*global m*/, int col0 /*global n of v[0]*/,
-//                                     const float (&v)[32], uint8_t *stage, int lane, int buf, uint32_t taddr) const;
-//                      (4x per tile per thread; taddr = TMEM address of v[0] for this warp, for re-reading single columns)
-//                      (stage = this warp's private 32 x 80-byte smem tile for transposing to coalesced rows)
+//                                     const float (&v)[32], uint8_t *stage, int lane, int buf, const float *acc) const;
+//                      (2x per tile per thread; acc = this thread's accumulator row in shared memory at column v[0], for
+//                       re-reading single columns; stage = this warp's private 32 x 80-byte smem tile for transposing to
+//                       coalesced rows; the 32 lanes of a warp hold rows row - lane .. row - lane + 31)
 //                __device__ void end_cta(State&, int warp_q, int lane) const; };
 //
 // Tile order: kMFastest = false -> n fastest (tiles of the same A row-block run concurrently and share A
@@ -80,21 +89,19 @@ struct GemmTileInfo {
 template <class Epi, bool kMFastest = false, int kKind = GEMM_KIND_TF32>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 int M, int N, int K, Epi epi) {
+               int M, int N, int K, Epi epi) {
     // device-conditional launch: an epilogue may declare the whole launch unnecessary (kNN pass 2 when every query was
-    // certified) from a device-side counter, before any barrier / TMEM state exists -- uniform over the grid
+    // certified) from a device-side counter, before any barrier state exists -- uniform over the grid
     if (epi.skip_kernel()) return;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *smem_a = smem;
     uint8_t *smem_b = smem + GEMM_STAGES * GEMM_A_STAGE_BYTES;
-    uint8_t *epi_stage = smem + GEMM_STAGES * GEMM_STAGE_BYTES;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + GEMM_STAGES * GEMM_STAGE_BYTES + GEMM_EPI_WARPS * GEMM_EPI_STAGE_BYTES);
+    float *acc_tile = reinterpret_cast<float *>(smem + GEMM_STAGES * GEMM_STAGE_BYTES);
+    uint8_t *epi_stage = smem + GEMM_STAGES * GEMM_STAGE_BYTES + GEMM_ACC_BYTES;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(epi_stage + GEMM_EPI_WARPS * GEMM_EPI_STAGE_BYTES);
     uint64_t *full_bar = bars;                        // [STAGES]
     uint64_t *empty_bar = bars + GEMM_STAGES;         // [STAGES]
-    uint64_t *tmem_full = bars + 2 * GEMM_STAGES;     // [2]
-    uint64_t *tmem_empty = bars + 2 * GEMM_STAGES + 2;  // [2]
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * GEMM_STAGES + 4);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -104,31 +111,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     constexpr int BK = gemm_block_k(kKind);            // elements per 128-byte k-block
     const int num_kb = (K + BK - 1) / BK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == GEMM_PRODUCER_THREAD) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_b);
         for (int s = 0; s < GEMM_STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], GEMM_EPI_WARPS);   // one arrival per consumer warp
         }
-        mbar_init(&tmem_full[0], 1);
-        mbar_init(&tmem_full[1], 1);
-        mbar_init(&tmem_empty[0], GEMM_EPI_WARPS);
-        mbar_init(&tmem_empty[1], GEMM_EPI_WARPS);
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, GEMM_TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (threadIdx.x >= GEMM_PRODUCER_THREAD) {
         // ---------------- TMA producer ----------------
-        if (lane == 0) {
+        if (threadIdx.x == GEMM_PRODUCER_THREAD) {
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -143,90 +139,80 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 }
             }
         }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer (one thread) ----------------
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc(kKind == GEMM_KIND_F16 ? 0u /*f16*/ : 2u /*tf32*/, GEMM_BLOCK_M, GEMM_BLOCK_N);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                mbar_wait_guarded(&tmem_empty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * GEMM_BLOCK_N;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait_guarded(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint64_t a_desc = umma_desc_sw128(smem_u32(smem_a + stage * GEMM_A_STAGE_BYTES));
-                    const uint64_t b_desc = umma_desc_sw128(smem_u32(smem_b + stage * GEMM_B_STAGE_BYTES));
-#pragma unroll
-                    for (int k = 0; k < GEMM_BLOCK_K / GEMM_UMMA_K; ++k) {
-                        // advance 32 bytes inside the 128B swizzle row: +2 in the (addr >> 4) field
-                        if (kKind == GEMM_KIND_F16) umma_f16(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (kb | k) != 0);
-                        else umma_tf32(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (kb | k) != 0);
-                    }
-                    tc_commit(&empty_bar[stage]);   // frees the smem stage once these MMAs retire
-                    if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
-                }
-                tc_commit(&tmem_full[acc]);         // accumulator complete -> epilogue
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else {
-        // ---------------- epilogue warps ----------------
-        const int q = warp & 3;                      // TMEM lane quarter this warp may access
-        const int chalf = (warp - 2) >> 2;           // which 128-column half of the accumulator this warp drains
-        typename Epi::State est;
-        epi.begin_cta(est, q, lane);
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-            GemmTileInfo ti;
-            ti.m0 = (kMFastest ? tile % tiles_m : tile / tiles_n) * GEMM_BLOCK_M;
-            ti.n0 = (kMFastest ? tile / tiles_m : tile % tiles_n) * GEMM_BLOCK_N;
-            ti.tile_iter = it;
-            const int row = ti.m0 + q * 32 + lane;
-            const int c_lo = chalf * (GEMM_BLOCK_N / 2);
-            // operands the epilogue needs from global memory (residual rows) are requested one chunk ahead; the first
-            // request goes out before the accumulator is even complete
-            epi.prefetch(est, ti, row, ti.n0 + c_lo, lane, 0);
-            mbar_wait_guarded(&tmem_full[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * GEMM_BLOCK_N;
-#pragma unroll (Epi::kUnrollChunks)
-            for (int ci = 0; ci < GEMM_BLOCK_N / 2 / 32; ++ci) {
-                const int c = c_lo + 32 * ci;
-                if (ci + 1 < GEMM_BLOCK_N / 2 / 32) epi.prefetch(est, ti, row, ti.n0 + c + 32, lane, (ci + 1) & 1);
-                uint32_t r[32];
-                tmem_ld_32x32(taddr + c, r);
-                tmem_ld_wait();
-                float v[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-                epi.tile(est, ti, row, ti.n0 + c, v, epi_stage + (warp - 2) * GEMM_EPI_STAGE_BYTES, lane, ci & 1, taddr + c);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-        epi.end_cta(est, q, lane);
+        return;     // no CTA-wide barrier follows: the consumers synchronise per warpgroup
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, GEMM_TMEM_COLS);
+    // ---------------- consumer warpgroups: wgmma mainloop, then the epilogue of their own 64 rows ----------------
+    const int wg = warp >> 2;                        // 0 or 1: tile rows [64 wg, 64 wg + 64)
+    const int q = 2 * wg + (warp & 1);               // 32-row quarter of the tile this warp drains
+    const int chalf = gemm_epi_chalf();
+    typename Epi::State est;
+    epi.begin_cta(est, q, lane);
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    const float *acc_row = acc_tile + (q * 32 + lane) * GEMM_ACC_LD;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        GemmTileInfo ti;
+        ti.m0 = (kMFastest ? tile % tiles_m : tile / tiles_n) * GEMM_BLOCK_M;
+        ti.n0 = (kMFastest ? tile / tiles_m : tile % tiles_n) * GEMM_BLOCK_N;
+        ti.tile_iter = it;
+        const int row = ti.m0 + q * 32 + lane;
+        const int c_lo = chalf * GEMM_EPI_COLS;
+        // operands the epilogue needs from global memory (residual rows) are requested kDist chunks ahead into kDist + 1
+        // register buffers; the first requests go out before the mainloop
+        constexpr int kDist = Epi::kPrefetchDist, kBufs = kDist + 1, kChunks = GEMM_EPI_COLS / 32;
+#pragma unroll
+        for (int d = 0; d < kDist; ++d)
+            if (d < kChunks) epi.prefetch(est, ti, row, ti.n0 + c_lo + 32 * d, lane, d % kBufs);
+
+        float acc[64];
+#pragma unroll
+        for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+        // one wgmma group stays in flight: the stage of k-block kb-1 is released once the group of kb has been issued and
+        // the group of kb-1 has retired
+        int prev_stage = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait_guarded(&full_bar[stage], phase);
+            const uint64_t a_desc = wgmma_desc_sw128(smem_u32(smem_a + stage * GEMM_A_STAGE_BYTES + wg * 64 * 128));
+            const uint64_t b_desc = wgmma_desc_sw128(smem_u32(smem_b + stage * GEMM_B_STAGE_BYTES));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                // advance 32 bytes inside the 128B swizzle row: +2 in the (addr >> 4) field
+                if (kKind == GEMM_KIND_F16) wgmma_m64n128_f16(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                else wgmma_m64n128_tf32(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            __syncwarp();
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // this warp's share has been consumed
+            prev_stage = stage;
+            if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+        named_bar_sync(1 + wg, 128);                 // this warpgroup's epilogue of the previous tile is done reading
+        wgmma_store_acc(acc, acc_tile + wg * 64 * GEMM_ACC_LD, GEMM_ACC_LD);
+        named_bar_sync(1 + wg, 128);
+#pragma unroll (Epi::kUnrollChunks)
+        for (int ci = 0; ci < kChunks; ++ci) {
+            const int c = c_lo + 32 * ci;
+            if (ci + kDist < kChunks) epi.prefetch(est, ti, row, ti.n0 + c + 32 * kDist, lane, (ci + kDist) % kBufs);
+            float v[32];
+            acc_row_ld32(acc_row + c, v);
+            epi.tile(est, ti, row, ti.n0 + c, v, epi_stage + warp * GEMM_EPI_STAGE_BYTES, lane, ci % kBufs, acc_row + c);
+        }
     }
+    epi.end_cta(est, q, lane);
 }
 
-// host-side launcher
+// host-side launcher.  ta: A map with a GEMM_BLOCK_M-row box, tb: B map with a GEMM_BLOCK_N-row box (128-byte rows).
 template <class Epi, bool kMFastest = false, int kKind = GEMM_KIND_TF32>
 int launch_gemm_tc(const CUtensorMap &ta, const CUtensorMap &tb, int M, int N, int K, const Epi &epi,
-                     cudaStream_t stream, int max_ctas = 0, int prof_cls = PROF_GEMM_LINEAR, double prof_bytes = 0.0) {
+                   cudaStream_t stream, int max_ctas = 0, int prof_cls = PROF_GEMM_LINEAR, double prof_bytes = 0.0) {
     auto kern = gemm_tc_kernel<Epi, kMFastest, kKind>;
     static bool attr_set[64] = {};   // per instantiation and per device
     int dev = 0;

@@ -90,9 +90,8 @@ rowdot_kernel(const float *__restrict__ X, const float *__restrict__ W, float *_
 
 // batched forward (M > 64 rows, the predict step at B = 512): Y[m,n] = epi( sum_k X[m,k] W[n,k] ), both operands K-major.
 // 64 x 64 tile, 256 threads x (4 x 4) outputs, K in slabs of 16 staged transposed in shared memory ([k][row], padded), next slab
-// prefetched into registers.  k is added in ascending order per output.  (rowdot_kernel<4> needed 255 registers -- a whole SM's
-// register file per CTA, so on the side stream it could not share an SM with the prototype scan -- and ran at 2.6 TFLOP/s:
-// 527 us for the three layers at B = 512, profiles/r02_knn_ncu.md; this kernel: see the same file.)
+// prefetched into registers.  k is added in ascending order per output.  (rowdot_kernel<4> needs 255 registers -- a whole SM's
+// register file per CTA, so on the side stream it could not share an SM with the prototype scan.)
 constexpr int SG_T = 64, SG_K = 16;
 __global__ void __launch_bounds__(256)
 sgemm_nt_kernel(const float *__restrict__ X, const float *__restrict__ W, float *__restrict__ Y, int M, int N, int K, SgemmEpi epi) {
@@ -288,7 +287,7 @@ static int plan_training(int batch, const ac_head_params *p, int n_steps, bool u
     AC_REQUIRE(p->D <= 2048 && p->H0 <= 2048 && p->H1 <= 2048, "%s: layer widths above 2048 are not supported", who);
     AC_REQUIRE(n_steps <= (1 << 20), "%s: at most 2^20 steps per launch", who);
     // one CTA per SM at most (cooperative launch: all CTAs resident).  The 8-row blocks of the three layers are dealt round robin:
-    // the reference's head (768 -> 768 -> 384 -> C <= 32) has 96 + 48 + 4 = 148 blocks, one per SM of a B200
+    // the reference's head (768 -> 768 -> 384 -> C <= 32) has 96 + 48 + 4 = 148 blocks, dealt over the 132 SMs of an H100
     ht::Args a{};
     plan_args(a, batch, p, 1);
     int G = sm_count();
@@ -298,7 +297,7 @@ static int plan_training(int batch, const ac_head_params *p, int n_steps, bool u
     // AdamW moments resident in shared memory if at least three ring stages still fit; then as many stages (<= 8) as there is room for
     const size_t limit = 220 * 1024;
     pl.smem_bytes = ~size_t(0);
-    constexpr int res_min_nst = 3;      // measured: moments resident with only two ring stages is slower than L2-resident with three
+    constexpr int res_min_nst = 3;      // resident moments must leave room for at least three ring stages; otherwise they stay in L2
     for (int res = update ? 1 : 0; res >= 0; --res) {
         a.res_mv = res;
         for (a.nst = 8; a.nst >= (res ? res_min_nst : 2); --a.nst) {
@@ -479,7 +478,7 @@ extern "C" int ac_head_train_plan(int batch, const ac_head_params *p, int *out5)
     int rc = plan_training(batch, p, 1, true, pl, "ac_head_train_plan");
     if (rc) return rc;
     out5[0] = pl.G; out5[1] = pl.nst; out5[2] = pl.res_mv; out5[3] = static_cast<int>(pl.smem_bytes);
-    out5[4] = 0;   // reserved (folding the loss phase into its consumers was measured slower: 46.4 vs 44.4 us per step)
+    out5[4] = 0;   // reserved
     return AC_OK;
 }
 

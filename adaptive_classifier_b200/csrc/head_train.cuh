@@ -8,13 +8,16 @@
 // and the DataLoader batching around it (one launch runs all steps of an epoch from a shuffled index list).
 //
 // Why one kernel: the head is 0.9 M parameters and a batch is 32 rows -- 171 MFLOP and 25 MB of optimizer traffic per step,
-// i.e. microseconds of work; the round-1 path launched ~21 dependent kernels per step (310 us measured on a B200).  Here the
-// grid stays resident for the whole epoch and a step is seven phases separated by six grid barriers (44 us per step measured):
+// i.e. microseconds of work, which ~21 dependent kernel launches per step would dominate.  Here the grid stays resident for
+// the whole epoch and a step is seven phases separated by six grid barriers (75 us per step on an H100 80GB HBM3, batch 32,
+// 21 classes: `cfg4.head_step_us_batch32` in profiles/h100_bench.json):
 //
 //   ownership   the rows of every weight matrix are cut into blocks of HT_RB = 8 rows, and the blocks of all three layers form
 //               ONE list of items dealt over the grid (item i -> CTA i % G).  The reference's head (768 -> 768 -> 384 -> C)
-//               has 96 + 48 + ceil(C / 8) items: with C <= 32 that is at most 148, one item per SM of a B200, so every CTA
-//               works for exactly one layer and the weight-gradient work of different layers runs side by side.  A CTA keeps
+//               has 96 + 48 + ceil(C / 8) items: with C <= 32 that is at most 148.  On the 132 SMs of an H100 the first
+//               items_total - 132 CTAs (15 at C = 21) own a layer-0 item and a layer-1 or layer-2 item, so in the phases where
+//               several layers work those CTAs do two items' work; the others work for one layer, and the weight-gradient
+//               work of different layers runs side by side.  A CTA keeps
 //               the rows of ITS item(s) -- parameters, gradient, biases, and the AdamW moments when they fit (res_mv; for the
 //               reference's head they stay owner-private in L2) -- in shared memory for the whole launch, computes the activations / gradients of exactly those rows and applies AdamW to them: parameters
 //               never move between CTAs, gradients and moments never leave shared memory (moments: when they fit, res_mv),
@@ -649,7 +652,7 @@ __global__ void __launch_bounds__(HT_THREADS, 1) head_train_kernel(const Args a)
 
         // ================= P4: da1 of the own rows (layer-1 blocks).  The layer-2 weight gradients need nothing newer than dz
         // either, but they wait for the next phase: there the layer-2 CTAs would idle while layer 0 works, here they would be
-        // the critical path (4.9 us against 2.6 us) =================
+        // the critical path =================
         for (int s = 0; s < a.slots; ++s) {
             const int i = cta + s * G;
             if (i >= a.items) break;

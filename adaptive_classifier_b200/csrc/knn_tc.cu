@@ -1,8 +1,8 @@
 // knn_tc.cu -- stage K, tensor path: brute-force squared-L2 kNN over a large prototype matrix.
 //
-//   pass 1        d~(q,p) = ||q||^2 + ||p||^2 - 2 q.p   with q.p on tcgen05 (kind::f16 over the fp16 shadow of the rows, or
-//                 kind::tf32 on the fp32 rows) through the GEMM mainloop of gemm_tc.cuh: M = queries (128 per CTA, fixed per
-//                 CTA), N = prototype rows streamed ONCE from HBM by TMA, fp32 accumulators in TMEM.
+//   pass 1        d~(q,p) = ||q||^2 + ||p||^2 - 2 q.p   with q.p on wgmma (.f16 over the fp16 shadow of the rows, or
+//                 .tf32 on the fp32 rows) through the GEMM mainloop of gemm_tc.cuh: M = queries (128 per CTA, fixed per
+//                 CTA), N = prototype rows streamed ONCE from HBM by TMA, fp32 accumulators staged in shared memory.
 //                 Epilogue EpiKnn: thread = query row; running top-16 (coarse key, row id) per (query, CTA, column half).
 //   k <= 16       merge the lists, exact fp32 re-rank of the best KP = 32 candidates in the oracle's lane order
 //                 (knn_exact.cu), CERTIFY: T = smallest coarse distance any non-candidate row can have, eps = rigorous bound
@@ -63,6 +63,7 @@ struct EpiKnn {
     int kt;                  // a list publishes its kt-th best key (k + 3 <= kt <= KC): see prefetch()
 
     static constexpr int kUnrollChunks = 1;
+    static constexpr int kPrefetchDist = 1;
     struct State {
         float key[KNN_KC];
         int32_t idx[KNN_KC];
@@ -78,7 +79,7 @@ struct EpiKnn {
         st.gt = CUDART_INF_F;
     }
 
-    // Every list (74 per query at B = 512) would on its own perform ~KC ln(n/KC) sorted inserts; sharing a bound
+    // Every list (2 x (SMs / query tiles) per query) would on its own perform ~KC ln(n/KC) sorted inserts; sharing a bound
     // across lists makes all of them reject what cannot matter any more.  Each list publishes its kt-th best key;
     // gt = min over lists.  Exclusion bound for the certification: T = min over lists of their FINAL kt-th best
     // (<= every published value, gt only decreases).  A row with key < T is never rejected (key < T <= gt(t) and
@@ -114,7 +115,7 @@ struct EpiKnn {
     }
 
     __device__ __forceinline__ void tile(State &st, const GemmTileInfo &, int /*row*/, int col0, const float (&v)[32],
-                                         uint8_t * /*stage*/, int /*lane*/, int buf, uint32_t taddr) const {
+                                         uint8_t * /*stage*/, int /*lane*/, int buf, const float *acc) const {
         // fast path: all lanes walk the same 32 prototype rows and only record which ones beat their query's bound
         const float pn_lane = buf ? st.pn[1] : st.pn[0];
         const float thr = fminf(st.key[KNN_KC - 1], st.gt);
@@ -126,22 +127,20 @@ struct EpiKnn {
             hits |= (key < thr) ? (1u << j) : 0u;
         }
         // slow path (rare once the bounds are tight): one copy of the insert network, the hit column is read again
-        // from TMEM because v[] cannot be indexed dynamically
+        // from the shared-memory accumulator tile because v[] cannot be indexed dynamically
         uint32_t uni = __reduce_or_sync(0xffffffffu, hits);
         while (uni) {
             const int j = __ffs(uni) - 1;
             uni &= uni - 1;
-            const uint32_t r = tmem_ld_32x1(taddr + j);
-            tmem_ld_wait();
-            const float key = fmaf(-2.f, __uint_as_float(r), __shfl_sync(0xffffffffu, pn_lane, j));
+            const float key = fmaf(-2.f, acc[j], __shfl_sync(0xffffffffu, pn_lane, j));
             const int64_t n = static_cast<int64_t>(col0) + j;
             if (((hits >> j) & 1u) && key < fminf(st.key[KNN_KC - 1], st.gt) && n < N) insert(st, key, static_cast<int32_t>(n));
         }
     }
 
     __device__ __forceinline__ void end_cta(State &st, int q, int lane) const {
-        // two epilogue warps share a query row (one per 128-column half of every tile): each owns a slot
-        const int chalf = ((threadIdx.x >> 5) - 2) >> 2;
+        // two epilogue warps share a query row (one per column half of every tile): each owns a slot
+        const int chalf = gemm_epi_chalf();
         const int mt = blockIdx.x % tiles_m;
         const int slot = (blockIdx.x / tiles_m) * 2 + chalf;
         const int row = mt * GEMM_BLOCK_M + q * 32 + lane;
@@ -166,6 +165,7 @@ struct EpiKnnCollect {
     int tiles_m;
 
     static constexpr int kUnrollChunks = 1;
+    static constexpr int kPrefetchDist = 1;
     struct State {
         float pn[2];
         float thr;
@@ -182,7 +182,7 @@ struct EpiKnnCollect {
         if (buf_) st.pn[1] = x; else st.pn[0] = x;
     }
     __device__ __forceinline__ void tile(State &st, const GemmTileInfo &, int row, int col0, const float (&v)[32], uint8_t *,
-                                         int, int buf_, uint32_t) const {
+                                         int, int buf_, const float *) const {
         const float pn_lane = buf_ ? st.pn[1] : st.pn[0];
         uint32_t hits = 0;
 #pragma unroll
@@ -238,8 +238,7 @@ __global__ void knn_prep_rows_kernel(const float *__restrict__ P, int64_t N, int
 }
 
 // max_n ||p_n||^2 (for the error bound) -> out[0] (zeroed by the caller); non-negative floats order like their bit patterns.
-// One grid-stride pass over the 4 MB of norms (~5 us at N = 1 M).  Accumulating the maximum in the scan epilogue instead was
-// measured: it costs the scan 2-4 % (0.02-0.03 ms); the round-1 pass over the norms with one CTA per 8 rows cost 0.11 ms.
+// One grid-stride pass over the norms, kept out of the scan epilogue, whose per-chunk work is on the scan's critical path.
 __global__ void knn_max_norm_kernel(const float *__restrict__ pn, int64_t N, float *__restrict__ out) {
     float m = 0.f;
     const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
@@ -377,11 +376,12 @@ __global__ void knn_add_stats_kernel(const int32_t *__restrict__ in, int32_t *__
 // ------------------------------------------------------------------------------------------------
 constexpr int KNN_SMALL_K = 16;        // certification path (lists of KNN_KC per (query, CTA, half))
 // k > 16: queries per pass.  tau (the bound on the k-th distance) is the k-th smallest key among the merged lists, so it is
-// tight only if no list had to drop a top-k row for lack of room (16 entries).  Two query tiles per pass give every query
-// 2 x 74 lists over interleaved row tiles: with k = 1000 a list holds ~6.8 top-k rows on average (P(> 16) ~ 1e-3).  512 queries
-// per pass = 74 lists of 13.5 expected rows overflowed lists on 66 of 512 queries on the 1000-rows-per-class benchmark index
-// (tau jumped to the next cluster and the band held > 2048 rows).  Measured at 512 x 1 M x 768, k = 1000 on a B200: 4.35 ms per
-// search with 128 queries per pass (the scan of one tile is HBM-bound: 0.48 ms per pass over 1.5 GB), 3.03 ms with 256.
+// tight only if no list had to drop a top-k row for lack of room (16 entries).  A list sees ~k / (lists per query) top-k rows.
+// Two query tiles per pass give every query 2 x (SMs / 2) = 132 lists on an H100 over interleaved row tiles: at k = 1000 a list
+// holds ~7.6 top-k rows on average, well under 16.  Four tiles per pass would halve the lists per query (~15 rows per list, so
+// lists overflow and tau loosens); one tile per pass would scan the prototype matrix twice as often.  On an H100 80GB HBM3,
+// 256 queries per pass run the k = 1000 search of 512 queries over 1 M x 768 rows in 4.7 ms with no overflowing query
+// (`k_equals_C` in profiles/h100_bench.json).
 #ifndef AC_KNN_QUERY_BLOCK
 #define AC_KNN_QUERY_BLOCK 256
 #endif

@@ -29,7 +29,7 @@ class EWC:
     def _blocks(self):
         names = [n for n, p in self.model.named_parameters() if p.requires_grad]
         if len(names) != 6:
-            raise _cabi.AdaptiveB200Error("EWC on the B200 path supports the reference's 3-layer head only")
+            raise _cabi.AdaptiveB200Error("EWC on the CUDA path supports the reference's 3-layer head only")
         return names
 
     def _as_block(self, tensors: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
@@ -58,7 +58,7 @@ class EWC:
             probs = torch.softmax(outputs, dim=1)
             sampled = torch.multinomial(probs, 1).squeeze(-1)
             if sigmoid_head:
-                raise _cabi.AdaptiveB200Error("Fisher for the sigmoid head is not implemented on the B200 path")
+                raise _cabi.AdaptiveB200Error("Fisher for the sigmoid head is not implemented on the CUDA path")
             _cabi.head_grad(x, sampled, pblock, loss_kind=_cabi.AC_LOSS_CE, fisher=fblock,
                             inv_n_batches=1.0 / n_batches)
         names = self._blocks()

@@ -1,6 +1,6 @@
 """Host-side mirror of /root/reference/src/adaptive_classifier/memory.py (PrototypeMemory).
 
-Same bookkeeping, attribute names and error behaviour; `self.index` is a FlatL2Index living in B200 HBM
+Same bookkeeping, attribute names and error behaviour; `self.index` is a FlatL2Index living in GPU HBM
 (csrc/knn_exact.cu, csrc/knn_tc.cu) instead of faiss.IndexFlatL2.  Label aggregation and the
 `exp(-d)` -> softmax post-processing follow memory.py:117-134 exactly (on the device).
 """
@@ -23,7 +23,7 @@ logger = logging.getLogger(__name__)
 
 def _device() -> torch.device:
     if not torch.cuda.is_available():
-        raise _cabi.AdaptiveB200Error("adaptive_classifier_b200 needs a B200 GPU; there is no CPU fallback")
+        raise _cabi.AdaptiveB200Error("adaptive_classifier_b200 needs an H100 GPU; there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 
 

@@ -50,12 +50,12 @@ class _CudaHeadMixin:
         lins = _linears(self.model)
         if len(lins) != 3:
             raise _cabi.AdaptiveB200Error(
-                f"the B200 head kernels implement the reference's 3-layer head (got {len(lins)} Linear layers)")
+                f"the CUDA head kernels implement the reference's 3-layer head (got {len(lins)} Linear layers)")
         out = {}
         for i, lin in enumerate(lins):
             for nm, t in ((f"W{i}", lin.weight), (f"b{i}", lin.bias)):
                 if not t.is_cuda:
-                    raise _cabi.AdaptiveB200Error("adaptive head parameters must live on the B200 (no CPU path)")
+                    raise _cabi.AdaptiveB200Error("adaptive head parameters must live on the GPU (no CPU path)")
                 if not t.data.is_contiguous():
                     t.data = t.data.contiguous()
                 out[nm] = t.data

@@ -1,4 +1,4 @@
-"""Multi-label front end on top of the B200 hot path.
+"""Multi-label front end on top of the H100 hot path.
 
 Behavioural mirror of /root/reference/src/adaptive_classifier/multilabel.py (MultiLabelAdaptiveHead :15-68,
 MultiLabelAdaptiveClassifier :71-426): sigmoid head, per-label / size-adaptive thresholds, min/max number of
@@ -193,7 +193,7 @@ class MultiLabelAdaptiveClassifier(AdaptiveClassifier):
 
     def _train_new_classes(self, old_head, new_classes):
         # The reference inherits the single-label routine here and thereby applies CrossEntropyLoss to sigmoid outputs
-        # (SURVEY.md Appendix A.10).  The B200 head kernels have no CE-on-probabilities step; the multi-label path
+        # (SURVEY.md Appendix A.10).  The CUDA head kernels have no CE-on-probabilities step; the multi-label path
         # retrains with its BCE loop instead (documented deviation, DESIGN.md section 8).
         self._train_adaptive_head()
 

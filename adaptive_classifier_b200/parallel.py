@@ -12,7 +12,7 @@
 `ShardedPipeline` is the product path (bench.py at N > 1): it drives the SAME C pipeline as N = 1 phase by phase
 (`ac_pipeline_encode` / `_search_shard` / `_finish_sharded`) with the two collectives in between on the same stream; nothing
 synchronises with the host.  The two collectives are plain NCCL: the messages are small (1.5 MB and 30 KB per peer at 512
-queries), so the cost is launch latency, not NVLink bandwidth -- measured in DESIGN.md section 7.
+queries), so the cost is expected to be launch latency, not NVLink bandwidth (not measured on H100).
 
 `ShardedIndex` is the same exchange at the index level (any k, used by tests and by callers that only need the search); its
 search / pack / merge callables are injectable so that the host logic (sharding arithmetic, collectives, chunk layout, merge

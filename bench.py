@@ -1,18 +1,20 @@
 #!/usr/bin/env python
 """bench.py -- queries/sec of predict() on the BASELINE.json workload (see DESIGN.md "Measurement").
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 A step = one predict pass (E encoder -> K prototype kNN -> H head -> blend, top-5 labels) over one batch of
 512 synthetic 128-token queries PER GPU against a 1M x 768 fp32 prototype matrix (1000 classes), the
-configuration BASELINE.json's metric is quoted on (configs[2]); it fits one B200, and at N > 1 the matrix is
+configuration BASELINE.json's metric is quoted on (configs[2]); it fits one H100 (80 GB), and at N > 1 the matrix is
 row-sharded while every rank keeps its own 512 queries (weak scaling; --strong keeps the GLOBAL batch at 512).
 One JSON line on rank 0.  Before the timed region the step's kNN result of 16 queries is checked against the CPU oracle
 (and, at N > 1, the merged sharded result against the unsharded search): `parity_checked`.
 At N = 1 the line also carries sub-results measured after the headline (never inside its timed region): `k_equals_C`
 (predict() semantics, k = 1000), `cfg4` (BASELINE configs[3], the add_examples loop), `gpu_library_baseline` (HF BertModel in
 torch eager on the same GPU) and `cpu_baseline` (the oracle port on the host cores).
+--dump-outputs DIR writes what the last timed step returned (top-5 class ids as float64, their scores as float32) to
+DIR/top_classes.npy and DIR/top_scores.npy: the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -37,11 +39,12 @@ def peaks():
         j = json.load(open(p))
         return {"hbm_gbs": j["hbm_gbs"], "bf16_tflops": j["bf16_tflops"],
                 "bf16_tflops_sustained": j.get("bf16_tflops_sustained", j["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3, 989 dense fp16/bf16 TFLOP/s (700 W card); never reached in practice
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -252,7 +255,7 @@ def sub_k_equals_c(torch, _cabi, enc, P, p_sqnorm, p_half, row_class, hp, ids_de
 
 
 def sub_gpu_library_baseline(torch, ids_dev, enc_ms):
-    """stage E comparator of SURVEY 2b: the reference's own encoder call (HF BertModel, torch eager, SDPA) on the same B200"""
+    """stage E comparator of SURVEY 2b: the reference's own encoder call (HF BertModel, torch eager, SDPA) on the same GPU"""
     from adaptive_classifier_b200 import workload as wl
     out = {}
     try:
@@ -289,7 +292,7 @@ def sub_gpu_library_baseline(torch, ids_dev, enc_ms):
 def sub_cfg4(examples):
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import bench_add_examples as bae
-    return bae.run(examples=examples, call=256, seq=128, quiet=True)
+    return bae.run(examples=examples, call=256, seq=128, quiet=True, hbm_peak=peaks())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -305,7 +308,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--no-extras", action="store_true", help="skip the sub-results (k = C, cfg4, HF-eager comparator)")
     ap.add_argument("--cfg4-examples", type=int, default=50_000, help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (top-5 class ids, scores) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1 (the timed region and --dump-outputs need a step)")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -334,7 +341,7 @@ def main():
     from adaptive_classifier_b200.parallel import ShardedPipeline, shard_bounds
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device; the CUDA path has no CPU fallback (use --impl reference for the CPU arm)")
     _cabi.load_library()          # fails loudly if the in-tree .so is missing
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
@@ -406,13 +413,15 @@ def main():
         if G > 1:
             dist.barrier()
 
+    last = {}
+
     def timed(fn, steps):
         barrier(); torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0 = time.time()
         e0.record()
         for _ in range(steps):
-            fn()
+            last["out"] = fn()
         e1.record()
         torch.cuda.synchronize(); barrier()
         t1 = time.time()
@@ -461,6 +470,12 @@ def main():
     l0 = _cabi.launch_count()
     ms, t0, t1 = timed(step_device, args.steps)
     launches = _cabi.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        oc, osc = last["out"]              # before step_host below reuses the pipeline's output buffers
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "top_classes.npy"), oc.cpu().numpy().astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "top_scores.npy"), osc.cpu().numpy().astype(np.float32))
     _cabi.profile_enable(False)
     prof = {c: _cabi.profile_read(c) for c in range(5)}
     clocks = sampler.stop(t0, t1) if rank == 0 else None
@@ -518,14 +533,15 @@ def main():
         "gpu_launches": int(launches),
         "clocks": clocks,
         "parity": parity,
-        "roofline": {"bound": "tensor", "kernel": "gemm_tc2_kernel<Epi..., kind::f16> (encoder projections as CTA-pair tcgen05 GEMMs: fp16 operands, "
-                                                  "fp32 TMEM accumulators, LayerNorm / GELU / residual fused into the epilogues)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel<Epi..., f16> (encoder projections as wgmma GEMMs: fp16 operands, "
+                                                  "fp32 accumulators, LayerNorm / GELU / residual fused into the epilogues)",
                      "achieved": gemm_tflops, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
                      "frac": gemm_tflops / pk["bf16_tflops_sustained"],
                      "traffic": tj.get("dram_bytes_per_launch"), "traffic_source": tj.get("source", "no ncu capture of this build committed"),
-                     "peak_source": f"{pk['source']} cuBLAS bf16 GEMM, sustained (kernel timed inside a long step)",
+                     "peak_source": ("measured cuBLAS bf16 GEMM, sustained (MEASURED_PEAKS.json)" if pk["source"] == "measured"
+                                     else f"{pk['source']}, dense fp16/bf16 (not a measurement)"),
                      "launches": gemm["launches"], "ms_total": gemm["ms"], "share_of_step": gemm["ms"] / ms},
-        "roofline_knn": {"kernel": "gemm_tc_kernel<EpiKnn, kind::f16> (pass 1 of the prototype scan: tcgen05 coarse distances over the fp16 "
+        "roofline_knn": {"kernel": "gemm_tc_kernel<EpiKnn, f16> (pass 1 of the prototype scan: wgmma coarse distances over the fp16 "
                                    "shadow, per-(query, CTA) top-16 lists)",
                          "ms_per_launch": knn_ms,
                          "frac_algorithmic": knn_alg_gbs / pk["hbm_gbs"], "algorithmic_gbs": knn_alg_gbs,

@@ -3,7 +3,7 @@
     python examples/basic_usage.py /path/to/local/bert-checkpoint      # any BERT/RoBERTa/DistilBERT-shaped HF directory
 
 No network is needed: pass a local checkpoint directory (tests/test_gpu_classifier.py fabricates one from
-tests/golden/golden_classifier.npz).  Needs a B200; there is no CPU fallback.
+tests/golden/golden_classifier.npz).  Needs an H100; there is no CPU fallback.
 """
 import sys
 

@@ -1,5 +1,5 @@
 /*
- * adaptive_b200.h -- C ABI of libadaptive_b200.so (hand-written sm_100a CUDA).
+ * adaptive_b200.h -- C ABI of libadaptive_b200.so (hand-written sm_90a CUDA).
  *
  * Drop-in boundary for the predict()/add_examples() hot path of codelion/adaptive-classifier.
  * The reference has no FFI of its own: the seams are Python object calls into third-party
@@ -13,7 +13,7 @@
  *   - all matrices are row-major, fp32, ids int64 unless stated; no hidden allocation after
  *     `*_create` / explicit workspaces.
  *   - return value: 0 = ok, negative = error (AC_E_*); text via ac_last_error() (thread-local).
- *   - no CPU fallback exists: with no usable sm_100 device every compute call returns AC_E_CUDA.
+ *   - no CPU fallback exists: with no usable sm_90 (H100) device every compute call returns AC_E_CUDA.
  */
 #ifndef ADAPTIVE_B200_H
 #define ADAPTIVE_B200_H
@@ -30,14 +30,14 @@ typedef void *ac_stream_t;
 enum {
     AC_OK = 0,
     AC_E_INVALID = -1,   /* bad argument (shape, null pointer, k > limit ...) */
-    AC_E_CUDA = -2,      /* CUDA runtime / launch failure, or no sm_100 device */
+    AC_E_CUDA = -2,      /* CUDA runtime / launch failure, or no sm_90 device */
     AC_E_WORKSPACE = -3, /* workspace too small */
     AC_E_UNSUPPORTED = -4
 };
 
 int ac_version(void);                 /* ABI version, currently 1 */
 const char *ac_last_error(void);      /* thread-local message of the last failing call */
-int ac_device_check(void);            /* 0 when the current device is sm_100 (B200), else AC_E_CUDA */
+int ac_device_check(void);            /* 0 when the current device is sm_90 (H100), else AC_E_CUDA */
 
 
 /* ------------------------------------------------------------------------------------------
@@ -49,7 +49,7 @@ int ac_device_check(void);            /* 0 when the current device is sm_100 (B2
 enum {
     AC_KNN_AUTO = 0,
     AC_KNN_EXACT = 1,   /* fp32 SIMT exact scan + radix select (any k <= AC_KNN_MAX_K)       */
-    AC_KNN_TENSOR = 2   /* tcgen05 coarse pass (kind::f16 over the fp16 shadow, or kind::tf32) + exact fp32 re-rank,
+    AC_KNN_TENSOR = 2   /* wgmma coarse pass (.f16 over the fp16 shadow, or .tf32) + exact fp32 re-rank,
                            k <= AC_KNN_TENSOR_MAX_K.  k <= 16: per-query certification against the rigorous coarse
                            error bound; uncertified queries -- and every query when k > 16 -- take a second,
                            device-conditional tensor pass that collects the provable superset {d~ <= tau + 2 eps},
@@ -67,7 +67,7 @@ int ac_knn_workspace_bytes(int B, int64_t N, int D, int k, int algo, size_t *byt
  * Distances are the exact fp32 lane-ordered sum restated in oracle/knn_oracle.c (bit-identical).
  * p_sqnorm[N] (nullable) = cached ||p||^2 for the tensor path; computed into the workspace if NULL.
  * p_half (nullable) = fp16 shadow copy of P[N,D] (ac_knn_make_shadow): the tensor path then runs its coarse pass as
- *   tcgen05 kind::f16 over 2.N.D bytes (D %% 64 == 0); candidates are still re-ranked on the fp32 rows, so the
+ *   wgmma .f16 over 2.N.D bytes (D %% 64 == 0); candidates are still re-ranked on the fp32 rows, so the
  *   result is the same bits either way.
  * stats (nullable, device int32[4], ACCUMULATED): [0] queries that needed the second tensor pass, [1] queries whose
  *   2-eps band overflowed the candidate buffer (their rows of out_d/out_i are NOT exact: the caller must redo them with
@@ -197,8 +197,8 @@ int ac_ewc_penalty(const ac_head_params *p, const ac_head_params *fisher, const 
  * ------------------------------------------------------------------------------------------ */
 enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1 };
 enum {
-    AC_PREC_TF32 = 0,   /* tcgen05 kind::tf32 on fp32 storage (kNN coarse pass, ac_linear_tc tests) */
-    AC_PREC_F16 = 1     /* tcgen05 kind::f16 with fp16 operands (RNE from fp32; same 10-bit mantissa as tf32),
+    AC_PREC_TF32 = 0,   /* wgmma .tf32 on fp32 storage (kNN coarse pass, ac_linear_tc tests) */
+    AC_PREC_F16 = 1     /* wgmma .f16 with fp16 operands (RNE from fp32; same 10-bit mantissa as tf32),
                            fp32 accumulation; the encoder's precision: 1.7e-4 on distances, bf16 would be 1.4e-3 */
 };
 
@@ -291,7 +291,7 @@ int ac_pipeline_predict_device(ac_pipeline *pl, const int32_t *ids_dev, const in
                                int32_t *out_cls_dev, float *out_score_dev, ac_stream_t stream);
 /* HOST buffers at the boundary (bench.py `e2e`): H2D of ids and D2H of the [B,k] result inside the call.  The device part of the
  * step is replayed as a CUDA graph from the third call with a batch size on (first: ordinary launches, second: capture) -- at B = 1
- * the ~110 launches of a step cost more host time than GPU time (0.92 instead of 1.15 ms per query).  Results are identical to the
+ * the ~110 launches of a step cost more host time than GPU time.  Results are identical to the
  * eager step; AC_PIPELINE_GRAPH=0 in the environment, or enabled per-kernel profiling (ac_profile_enable), keeps the step eager. */
 int ac_pipeline_predict_host(ac_pipeline *pl, const int32_t *ids_host, int B, int32_t *out_cls_host,
                              float *out_score_host, ac_stream_t stream);
@@ -316,7 +316,7 @@ int ac_pipeline_debug_copy(ac_pipeline *pl, int B, float *emb_out, float *knn_d_
 /* ------------------------------------------------------------------------------------------
  * Measurement hooks (bench.py): number of kernels launched by this library so far, and optional
  * CUDA-event timing of the dominant kernels on their launching stream.
- * classes: 0 encoder tcgen05 GEMM, 1 attention, 2 kNN tensor pass 1, 3 kNN exact scan, 4 kNN tensor pass 2 (device-conditional)
+ * classes: 0 encoder wgmma GEMM, 1 attention, 2 kNN tensor pass 1, 3 kNN exact scan, 4 kNN tensor pass 2 (device-conditional)
  * ------------------------------------------------------------------------------------------ */
 long long ac_launch_count(void);
 int ac_profile_enable(int on);

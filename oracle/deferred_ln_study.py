@@ -55,7 +55,7 @@ def deferred_forward(sd, ids, num_heads=12, eps=1e-12):
         Wp = r16(W * g[None, :])                       # fp16(gamma * W), packed once at encoder_create
         c1 = Wp.sum(1)                                 # fp32 row sums of the packed weight
         c0 = W @ b + bias                              # fp32
-        acc = r16(y) @ Wp.t()                          # tcgen05 kind::f16, fp32 accumulate
+        acc = r16(y) @ Wp.t()                          # f16 tensor-core MMA, fp32 accumulate
         return r * (acc - mu * c1[None, :]) + c0[None, :]
 
     def ln_on_the_fly(y, mu, r, g, b):

@@ -15,7 +15,7 @@ for RoBERTa position ids) and PINNED against the installed HF module itself
 (tests/test_oracle_cpu.py::test_encoder_oracle_matches_hf, max abs diff < 2e-6 on unit CLS rows).
 
 `round_fn` lets the precision study (oracle/precision_study.py) emulate tensor-core operand
-rounding (bf16 / tf32 / split-bf16) to choose the tcgen05 operand format per GEMM.
+rounding (bf16 / tf32 / split-bf16) to choose the tensor-core operand format per GEMM.
 """
 from __future__ import annotations
 
@@ -129,7 +129,7 @@ def round_bf16(t: Tensor) -> Tensor:
 
 
 def round_tf32(t: Tensor) -> Tensor:
-    """Round-to-nearest-even to 10 explicit mantissa bits (tcgen05 kind::tf32 reads the top 19 bits:
+    """Round-to-nearest-even to 10 explicit mantissa bits (the tf32 MMA reads the top 19 bits:
     hardware TRUNCATES fp32 operands; see `trunc_tf32`)."""
     i = t.contiguous().view(torch.int32)
     bias = ((i >> 13) & 1) + 0x0FFF

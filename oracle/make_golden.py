@@ -36,6 +36,17 @@ sys.path.insert(0, ROOT)
 OUT = os.path.join(ROOT, "tests", "golden")
 
 
+def save_split(name, arrays):
+    """golden_<name>.npz + the checkpoint weights (bert_*) in _bert0 / _bert1 (layer 1): every file stays under 1 MB;
+    tests/golden_npz.py loads them back as one mapping"""
+    parts = {"": {}, "_bert0": {}, "_bert1": {}}
+    for k, v in arrays.items():
+        suffix = "" if not k.startswith("bert_") or k == "bert_config" else ("_bert1" if ".layer.1." in k else "_bert0")
+        parts[suffix][k] = v
+    for suffix, p in parts.items():
+        np.savez_compressed(os.path.join(OUT, f"{name}{suffix}.npz"), **p)
+
+
 def unit(x):
     return x / x.norm(dim=-1, keepdim=True)
 
@@ -166,15 +177,15 @@ def gen_classifier():
     head_sd = {("head_" + k): v.detach().numpy() for k, v in clf.adaptive_head.state_dict().items()}
     model_sd = {("bert_" + k): v.detach().numpy() for k, v in model.state_dict().items()}
     protos = np.stack([clf.memory.prototypes[l].numpy() for l in sorted(clf.memory.prototypes)])
-    np.savez_compressed(
-        os.path.join(OUT, "golden_classifier.npz"),
+    save_split(
+        "golden_classifier", dict(
         vocab=np.array(vocab), texts=np.array(texts), labels=np.array(labels), test_texts=np.array(test_texts),
         label_names=np.array(label_names), input_ids=enc["input_ids"].numpy(), attention_mask=enc["attention_mask"].numpy(),
         emb_train=emb_train, emb_test=emb_test, prototypes=protos, proto_labels=np.array(sorted(clf.memory.prototypes)),
         training_history=json.dumps(clf.training_history), train_steps=clf.train_steps,
         pred_labels=pl, pred_scores=ps, pred_k1_labels=p1l, pred_k1_scores=p1s, predb_labels=pbl, predb_scores=pbs,
         train_top1=np.array([label_names.index(l) for l in train_top1]),
-        bert_config=json.dumps(cfg.to_dict()), **head_sd, **model_sd)
+        bert_config=json.dumps(cfg.to_dict()), **head_sd, **model_sd))
     print("golden_classifier ok; labels", label_names, "pred[0]", pred[0])
 
 
@@ -460,7 +471,7 @@ def gen_training():
     out["vocab"] = np.array(vocab)
     for k, v in clf.model.state_dict().items():
         out["bert_" + k] = v.detach().numpy()
-    np.savez_compressed(os.path.join(OUT, "golden_training.npz"), **out)
+    save_split("golden_training", out)
     print("golden_training ok: h3 steps", len(out["h3_loss"]), "epochs", len(out["h3_steps_per_epoch"]),
           "| h4 steps", len(out["h4_loss"]), "epochs", len(out["h4_steps_per_epoch"]), "rows", out["h4_X"].shape,
           "| fisher batches", len(out["h4_fisher_batch_sizes"]), "| ml steps", len(out["ml_loss"]), "preds", preds[:2])

@@ -2,8 +2,8 @@
 north_star tolerance (distances / logits within 1e-3 of the fp32 CPU path)?
 
 Emulates operand rounding of every GEMM (QKV/out/FFN projections, QK^T, PV) with fp32 accumulation:
-  bf16      : one tcgen05 kind::f16 pass, bf16 operands
-  tf32      : one tcgen05 kind::tf32 pass (hardware truncates fp32 operands to 10 mantissa bits)
+  bf16      : one tensor-core f16-kind pass, bf16 operands
+  tf32      : one tensor-core tf32 pass (hardware truncates fp32 operands to 10 mantissa bits)
   bf16x3    : split a = a_hi + a_lo (both bf16); a_hi*b_hi + a_hi*b_lo + a_lo*b_hi  (3 passes)
 Reports max/mean |delta| on the unit CLS rows and the induced error on squared-L2 distances
 to random unit prototypes.  Result table is pasted into DESIGN.md.

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine with one)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -17,7 +17,7 @@ def pytest_collection_modifyitems(config, items):
     import torch
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="needs a B200 (no CUDA device here)")
+    skip = pytest.mark.skip(reason="needs an H100 (no CUDA device here)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

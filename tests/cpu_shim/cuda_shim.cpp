@@ -28,7 +28,7 @@ void run_blocks(const std::vector<dim3> &blocks, dim3 grid, dim3 block, const st
     if (tpb % 32 != 0) { fprintf(stderr, "cuda_shim: block size must be a multiple of 32\n"); abort(); }
     std::vector<std::unique_ptr<Block>> blks;
     std::vector<std::unique_ptr<Fiber>> fibers;
-    static std::vector<uint8_t *> smem_pool;                    // 256 KB of "shared memory" and a TMEM per resident block
+    static std::vector<uint8_t *> smem_pool;                    // 256 KB of "shared memory" per resident block
     static std::vector<float (*)[512]> tmem_pool;
     static std::vector<Block *> cluster_members;
     cluster_members.clear();

@@ -61,7 +61,7 @@ struct Warp {
 struct Block {
     FiberBarrier bar;
     std::vector<Warp> warps;
-    // resources of the functional tensor-path model (tc_emul.h): dynamic shared memory (1024-byte aligned), TMEM, and the
+    // resources of the functional tensor-path model (tc_emul.h): dynamic shared memory (1024-byte aligned), tensor memory, and the
     // position of this CTA inside its cluster (all blocks of one run_blocks() call form the cluster)
     uint8_t *dyn_smem = nullptr;
     float (*tmem)[512] = nullptr;

@@ -90,7 +90,7 @@ def test_head_training_kernel_on_the_cpu_emulation():
              "40 40 20 5 50 20 9 0 0.1 1 1 9",
              "264 136 68 11 70 32 28 0 0.1 1 1 10",
              "520 264 68 11 30 30 4 0 0.0 0 0 6",       # several 256-column chunks per product
-             "128 128 64 130 64 32 5 0 0.2 1 1 11"]     # CE with more than 128 classes (logit tail re-read)    # one ownership block per CTA (the B200 layout of the reference's head)
+             "128 128 64 130 64 32 5 0 0.2 1 1 11"]     # CE with more than 128 classes (logit tail re-read)    # one ownership block per CTA
     for c in cases:
         out = subprocess.run([exe] + c.split(), capture_output=True, text=True, timeout=600)
         assert out.returncode == 0 and "MATCH" in out.stdout, (c, out.stdout[-600:], out.stderr[-300:])

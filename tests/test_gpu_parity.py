@@ -53,7 +53,7 @@ def test_linear_tc_matches_fp64(cabi, M, N, K, epi):
 @pytest.mark.parametrize("M,N,K,epi,out_half", [(256, 256, 64, 0, True), (1000, 768, 768, 2, False), (4096, 3072, 768, 1, True),
                                                   (300, 80, 128, 0, False), (128, 2304, 768, 0, True), (77, 768, 3072, 2, False)])
 def test_linear_f16_matches_fp64(cabi, M, N, K, epi, out_half):
-    """the encoder's GEMM: fp16 operands (exact products), fp32 accumulation in TMEM, fused epilogues"""
+    """the encoder's GEMM: fp16 operands (exact products), fp32 accumulation, fused epilogues"""
     g = torch.Generator().manual_seed(M + N + K + 1)
     X = torch.randn(M, K, generator=g).half()
     W = (torch.randn(N, K, generator=g) * 0.05).half()

@@ -13,6 +13,7 @@ import tempfile
 import numpy as np
 import pytest
 import torch
+import golden_npz
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -22,7 +23,7 @@ NAMES = {"W0": "model.0.weight", "b0": "model.0.bias", "W1": "model.3.weight", "
 
 @pytest.fixture(scope="module")
 def g():
-    return np.load(os.path.join(GOLD, "golden_training.npz"))
+    return golden_npz.load("golden_training")
 
 
 @pytest.fixture(scope="module")

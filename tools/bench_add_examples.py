@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE.json configs[3]: add_examples() continual loop -- 50k new examples, EWC-penalised head update, bert-base, 1xB200.
+"""BASELINE.json configs[3]: add_examples() continual loop -- 50k new examples, EWC-penalised head update, bert-base, one GPU.
 
 Synthetic pre-tokenised sequences (SURVEY.md section 8(d)): 20 classes, 196 calls of 256 examples, a 21st class introduced at
 call 100 so that _train_new_classes (+ Fisher / EWC) is traversed; from call ~79 on every class is over max_examples_per_class
@@ -18,7 +18,8 @@ import time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
-def run(examples=50176, call=256, seq=128, quiet=False, cpu_sample=True):
+def run(examples=50176, call=256, seq=128, quiet=False, cpu_sample=True, hbm_peak=None):
+    """hbm_peak: {'hbm_gbs': ..., 'source': ...} of the GPU this runs on (bench.py peaks()); without it no HBM floor is reported"""
     import copy
     import numpy as np
     import torch
@@ -105,7 +106,8 @@ def run(examples=50176, call=256, seq=128, quiet=False, cpu_sample=True):
         "head_optimizer_steps": steps_total, "new_class_calls": new_class_calls,
         "head_step_us_batch32": step_us, "head_steps_per_s_batch32": 1e6 / step_us,
         "head_step_roofline": {"bound": "hbm/latency", "algorithmic_bytes_per_step": 7 * 4 * P_params,
-                               "floor_us_at_measured_hbm_peak": 7 * 4 * P_params / 6581.9e9 * 1e6,
+                               "floor_us_at_hbm_peak": (7 * 4 * P_params / (hbm_peak["hbm_gbs"] * 1e9) * 1e6) if hbm_peak else None,
+                               "hbm_peak_source": hbm_peak["source"] if hbm_peak else None,
                                "note": "0.9 M parameters x (theta, g, m, v read; theta, m, v written); the kernel keeps theta and g in shared "
                                        "memory and m, v in L2, so the step is bound by six grid barriers + L2 operand streaming, not HBM"},
         "classes": len(clf.label_to_id), "stored_examples": stats["total_examples"],

@@ -21,7 +21,7 @@ KEEP = [
     "dram__bytes_read.sum",
     "dram__bytes_write.sum",
     "sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active",
-    "sm__inst_executed_pipe_tensor",            # prefix match: the sm_100 spelling differs between ncu releases
+    "sm__inst_executed_pipe_tensor",            # prefix match: the spelling differs between ncu releases
     "lts__throughput.avg.pct_of_peak_sustained_elapsed",
     "gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed",
     "l1tex__t_requests_pipe_lsu_mem_global_op_st.sum",
