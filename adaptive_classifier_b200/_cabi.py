@@ -23,7 +23,8 @@ AC_KNN_MAX_K = 2048
 AC_KNN_TENSOR_MAX_K = 1024
 AC_ACT_LOGITS, AC_ACT_SOFTMAX, AC_ACT_SIGMOID = 0, 1, 2
 AC_LOSS_CE, AC_LOSS_BCE = 0, 1
-AC_ARCH_BERT, AC_ARCH_ROBERTA = 0, 1
+AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT = 0, 1, 2
+AC_ENCODER_MAX_S = 512
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
 
 EXPORTS = [
@@ -61,7 +62,9 @@ class TrainCfg(Structure):
 class EncoderConfig(Structure):
     _fields_ = [("arch", c_int), ("layers", c_int), ("hidden", c_int), ("heads", c_int), ("intermediate", c_int),
                 ("vocab", c_int), ("max_pos", c_int), ("type_vocab", c_int), ("pad_idx", c_int),
-                ("ln_eps", c_float), ("precision", c_int), ("max_tokens", c_int), ("cls_only", c_int)]
+                ("ln_eps", c_float), ("precision", c_int), ("max_tokens", c_int), ("cls_only", c_int),
+                ("sliding_window", c_int), ("layer_sliding", POINTER(ctypes.c_int32)),
+                ("rope_full", c_void_p), ("rope_sliding", c_void_p)]
 
 
 _PP = POINTER(c_void_p)
@@ -73,7 +76,8 @@ class EncoderWeights(Structure):
                 ("q_w", _PP), ("q_b", _PP), ("k_w", _PP), ("k_b", _PP), ("v_w", _PP), ("v_b", _PP),
                 ("ao_w", _PP), ("ao_b", _PP), ("ao_ln_w", _PP), ("ao_ln_b", _PP),
                 ("ff1_w", _PP), ("ff1_b", _PP), ("ff2_w", _PP), ("ff2_b", _PP),
-                ("out_ln_w", _PP), ("out_ln_b", _PP)]
+                ("out_ln_w", _PP), ("out_ln_b", _PP),
+                ("attn_norm_w", _PP), ("final_norm_w", c_void_p), ("wqkv", _PP), ("wi", _PP)]
 
 
 _lib = None
@@ -456,12 +460,52 @@ def distilbert_to_bert_state_dict(sd: dict, c):
     return out, dims
 
 
+def modernbert_rope_table(theta: float, n_pos: int = AC_ENCODER_MAX_S, head_dim: int = 64) -> torch.Tensor:
+    """[n_pos, head_dim] fp32 table the encoder's RoPE epilogue reads: row p = cos | sin of the head_dim / 2 frequencies at
+    position p, computed with HF ModernBertRotaryEmbedding's own formula (default rope type, attention scaling 1)."""
+    inv_freq = 1.0 / (theta ** (torch.arange(0, head_dim, 2, dtype=torch.int64).to(dtype=torch.float) / head_dim))
+    pos = torch.arange(n_pos).float()
+    freqs = (inv_freq[None, :, None].float() @ pos[None, None, :]).transpose(1, 2)[0]      # [n_pos, head_dim / 2]
+    return torch.cat((freqs.cos(), freqs.sin()), dim=-1).contiguous()
+
+
+def modernbert_settings(c) -> dict:
+    """Encoder arguments of a ModernBertConfig; raises AdaptiveB200Error naming any setting the CUDA path does not implement
+    (checked before any device call)."""
+    if getattr(c, "hidden_activation", "gelu") != "gelu":
+        raise AdaptiveB200Error(f"ModernBERT hidden_activation={c.hidden_activation!r}: only exact-erf 'gelu' is implemented")
+    for flag in ("norm_bias", "attention_bias", "mlp_bias"):
+        if getattr(c, flag, False):
+            raise AdaptiveB200Error(f"ModernBERT {flag}=True is not implemented (the published checkpoints have no biases)")
+    heads = c.num_attention_heads
+    head_dim = getattr(c, "head_dim", None) or c.hidden_size // heads
+    if head_dim != 64 or c.hidden_size != heads * 64:
+        raise AdaptiveB200Error(f"ModernBERT head_dim={head_dim}: only head_dim 64 is implemented")
+    types = list(c.layer_types)
+    if len(types) != c.num_hidden_layers or not set(types) <= {"full_attention", "sliding_attention"}:
+        raise AdaptiveB200Error(f"ModernBERT layer_types={types!r}: only full_attention / sliding_attention are implemented")
+    theta = {}
+    for lt in ("full_attention", "sliding_attention"):
+        rp = c.rope_parameters[lt]
+        if rp.get("rope_type", "default") != "default":
+            raise AdaptiveB200Error(f"ModernBERT rope_type={rp.get('rope_type')!r} ({lt}): only 'default' RoPE is implemented")
+        theta[lt] = float(rp["rope_theta"])
+    window = int(c.sliding_window)
+    if "sliding_attention" in types and window < 1:
+        raise AdaptiveB200Error(f"ModernBERT sliding_window={window}: the half-window must be >= 1")
+    return dict(layers=c.num_hidden_layers, hidden=c.hidden_size, heads=heads, intermediate=c.intermediate_size,
+                vocab=c.vocab_size, ln_eps=c.norm_eps, pad_idx=(c.pad_token_id if c.pad_token_id is not None else 0),
+                sliding_window=window, layer_sliding=[1 if t == "sliding_attention" else 0 for t in types],
+                rope_theta=(theta["full_attention"], theta["sliding_attention"]))
+
+
 class Encoder:
-    """Owner of an ac_encoder handle built from an HF BERT/RoBERTa state_dict (CUDA fp32 tensors)."""
+    """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors)."""
 
     def __init__(self, sd: dict, *, arch: str, layers: int, hidden: int, heads: int, intermediate: int, vocab: int,
-                 max_pos: int, type_vocab: int, ln_eps: float, pad_idx: int = 0, max_tokens: int = 65536,
-                 device="cuda", cls_only: bool = True):
+                 max_pos: int = AC_ENCODER_MAX_S, type_vocab: int = 1, ln_eps: float, pad_idx: int = 0,
+                 max_tokens: int = 65536, device="cuda", cls_only: bool = True, sliding_window: int = 0,
+                 layer_sliding=None, rope_theta=None):
         L = load_library()
         self._L = L
         self.hidden = hidden
@@ -480,22 +524,39 @@ class Encoder:
             return ctypes.cast(a, _PP)
 
         w = EncoderWeights()
-        w.word_emb = g("embeddings.word_embeddings.weight")
-        w.pos_emb = g("embeddings.position_embeddings.weight")
-        w.type_emb = g("embeddings.token_type_embeddings.weight")
-        w.emb_ln_w = g("embeddings.LayerNorm.weight")
-        w.emb_ln_b = g("embeddings.LayerNorm.bias")
-        p = "encoder.layer.{}."
-        w.q_w, w.q_b = arr(p + "attention.self.query.weight"), arr(p + "attention.self.query.bias")
-        w.k_w, w.k_b = arr(p + "attention.self.key.weight"), arr(p + "attention.self.key.bias")
-        w.v_w, w.v_b = arr(p + "attention.self.value.weight"), arr(p + "attention.self.value.bias")
-        w.ao_w, w.ao_b = arr(p + "attention.output.dense.weight"), arr(p + "attention.output.dense.bias")
-        w.ao_ln_w, w.ao_ln_b = arr(p + "attention.output.LayerNorm.weight"), arr(p + "attention.output.LayerNorm.bias")
-        w.ff1_w, w.ff1_b = arr(p + "intermediate.dense.weight"), arr(p + "intermediate.dense.bias")
-        w.ff2_w, w.ff2_b = arr(p + "output.dense.weight"), arr(p + "output.dense.bias")
-        w.out_ln_w, w.out_ln_b = arr(p + "output.LayerNorm.weight"), arr(p + "output.LayerNorm.bias")
-        cfg = EncoderConfig(AC_ARCH_BERT if arch == "bert" else AC_ARCH_ROBERTA, layers, hidden, heads, intermediate,
-                            vocab, max_pos, type_vocab, pad_idx, ln_eps, AC_PREC_F16, max_tokens, 1 if cls_only else 0)
+        if arch == "modernbert":
+            # HF ModernBertModel names; mlp_norm travels in ao_ln_w, attn.Wo in ao_w, mlp.Wo in ff2_w (include/adaptive_b200.h)
+            w.word_emb = g("embeddings.tok_embeddings.weight")
+            w.emb_ln_w = g("embeddings.norm.weight")
+            w.final_norm_w = g("final_norm.weight")
+            p = "layers.{}."
+            w.ao_w, w.ao_ln_w, w.ff2_w = arr(p + "attn.Wo.weight"), arr(p + "mlp_norm.weight"), arr(p + "mlp.Wo.weight")
+            w.wqkv, w.wi = arr(p + "attn.Wqkv.weight"), arr(p + "mlp.Wi.weight")
+            an = (c_void_p * layers)(None, *[g(f"layers.{l}.attn_norm.weight") for l in range(1, layers)])  # layer 0: Identity
+            ls = (ctypes.c_int32 * layers)(*layer_sliding)
+            rope = [modernbert_rope_table(t).to(dev) for t in rope_theta]
+            keep.update(an=an, ls=ls, rope=rope)
+            w.attn_norm_w = ctypes.cast(an, _PP)
+            cfg = EncoderConfig(AC_ARCH_MODERNBERT, layers, hidden, heads, intermediate, vocab, AC_ENCODER_MAX_S, 1, pad_idx,
+                                ln_eps, AC_PREC_F16, max_tokens, 1 if cls_only else 0, sliding_window,
+                                ctypes.cast(ls, POINTER(ctypes.c_int32)), rope[0].data_ptr(), rope[1].data_ptr())
+        else:
+            w.word_emb = g("embeddings.word_embeddings.weight")
+            w.pos_emb = g("embeddings.position_embeddings.weight")
+            w.type_emb = g("embeddings.token_type_embeddings.weight")
+            w.emb_ln_w = g("embeddings.LayerNorm.weight")
+            w.emb_ln_b = g("embeddings.LayerNorm.bias")
+            p = "encoder.layer.{}."
+            w.q_w, w.q_b = arr(p + "attention.self.query.weight"), arr(p + "attention.self.query.bias")
+            w.k_w, w.k_b = arr(p + "attention.self.key.weight"), arr(p + "attention.self.key.bias")
+            w.v_w, w.v_b = arr(p + "attention.self.value.weight"), arr(p + "attention.self.value.bias")
+            w.ao_w, w.ao_b = arr(p + "attention.output.dense.weight"), arr(p + "attention.output.dense.bias")
+            w.ao_ln_w, w.ao_ln_b = arr(p + "attention.output.LayerNorm.weight"), arr(p + "attention.output.LayerNorm.bias")
+            w.ff1_w, w.ff1_b = arr(p + "intermediate.dense.weight"), arr(p + "intermediate.dense.bias")
+            w.ff2_w, w.ff2_b = arr(p + "output.dense.weight"), arr(p + "output.dense.bias")
+            w.out_ln_w, w.out_ln_b = arr(p + "output.LayerNorm.weight"), arr(p + "output.LayerNorm.bias")
+            cfg = EncoderConfig(AC_ARCH_BERT if arch == "bert" else AC_ARCH_ROBERTA, layers, hidden, heads, intermediate,
+                                vocab, max_pos, type_vocab, pad_idx, ln_eps, AC_PREC_F16, max_tokens, 1 if cls_only else 0)
         h = c_void_p()
         with torch.cuda.device(dev):
             check(L.ac_encoder_create(ctypes.byref(cfg), ctypes.byref(w), ctypes.byref(h)), "ac_encoder_create")
@@ -504,9 +565,14 @@ class Encoder:
 
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
-        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel (post-LN blocks, head_dim 64)."""
+        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel (post-LN blocks) or ModernBertModel (pre-LN,
+        RoPE, GeGLU, sliding-window layers); head_dim 64."""
         c = model.config
         mt = getattr(c, "model_type", "bert")
+        if mt == "modernbert":
+            dims = modernbert_settings(c)
+            return cls(dict(model.state_dict()), arch="modernbert", max_tokens=max_tokens, device=device, cls_only=cls_only,
+                       **dims)
         sd = {k: v for k, v in model.state_dict().items()}
         if mt == "distilbert":
             sd, dims = distilbert_to_bert_state_dict(sd, c)

@@ -1,8 +1,9 @@
-// encoder.cu -- stage E: BERT / RoBERTa post-LN encoder forward -> unit-norm CLS rows.
+// encoder.cu -- stage E: BERT / RoBERTa post-LN and ModernBERT pre-LN encoder forward -> unit-norm CLS rows.
 //
 // Replaces `self.model(**inputs).last_hidden_state[:, 0, :]` + F.normalize at
 // /root/reference/src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel.forward:
-// embeddings modeling_bert.py:53-113, self-attention :143-207, output+LN :287-298, FFN :330-356).
+// embeddings modeling_bert.py:53-113, self-attention :143-207, output+LN :287-298, FFN :330-356;
+// HF ModernBertModel.forward in models/modernbert/modeling_modernbert.py: see forward_modernbert).
 //
 // Precision: every tensor-core operand is fp16 (RNE from fp32), accumulation fp32 (wgmma), residual stream, LayerNorm,
 // softmax and GELU in fp32.  fp16 carries the same 10-bit mantissa as tf32, so the measured error is the tf32 one
@@ -19,6 +20,7 @@
 #include "gemm_tc.cuh"
 #include <cuda_fp16.h>
 #include <math_constants.h>
+#include <algorithm>
 #include <vector>
 
 namespace ac {
@@ -59,9 +61,17 @@ __device__ __forceinline__ float gelu_erf(float y) {
 //   DEFER: the A operand was the UN-normalised residual sum y (fp16) and the weights were packed as fp16(gamma * W):
 //       LayerNorm(y) W^T + b = r (acc - mu c1) + c0  with the row statistics (mu, r) of y, c1 = rowsum(W'), and
 //       `bias` holding c0 = W beta + b  (see "deferred LayerNorm" below)
-template <int MODE, bool OUT_HALF, bool VT, bool DEFER = false>
+//   MODE 3 (GeGLU, ModernBERT's mlp.Wi): the weight rows were interleaved in 32-row groups by pack_defer_kernel, so a
+//       warp's 64-column slice holds [input cols 32 g .. 32 g + 31 | gate cols 32 g .. 32 g + 31]; the gate chunk re-reads
+//       the input chunk from the shared accumulator tile and writes fp16(GELU_erf(input) * gate) to columns 32 g.. of Y
+//       (N = 2 I accumulator columns, I output columns, ldy = I)
+//   ROPE (ModernBERT's Wqkv): columns < vt_col0 (the q and k thirds) are rotated in fp32 before the fp16 rounding,
+//       pairs (d, d + 32) of a head = the two 32-column chunks of one warp's slice; the partner is re-read from the
+//       accumulator tile.  Position = token index inside its sequence (row % S), table row = [cos(32) | sin(32)].
+template <int MODE, bool OUT_HALF, bool VT, bool DEFER = false, bool ROPE = false>
 struct EpiLinear {
     static_assert(!DEFER || (OUT_HALF && MODE != 2), "the deferred-LayerNorm consumer epilogues write fp16 operands");
+    static_assert((MODE != 3 && !ROPE) || OUT_HALF, "the GeGLU / RoPE epilogues write fp16 operands");
     const float *__restrict__ bias;       // [N]   (DEFER: c0)
     const float *__restrict__ residual;   // [M, ldy] (MODE 2)
     void *Y;                              // [M, ldy] fp16 or fp32
@@ -71,6 +81,7 @@ struct EpiLinear {
     int vt_col0, S, S_pad, H;
     const float *__restrict__ c1;         // DEFER only: [N] row sums of the packed weight
     const float2 *__restrict__ row_stats; // DEFER only: [M] (mu, 1/sqrt(var + eps)) of the A rows
+    const float *__restrict__ rope;       // ROPE only: [S, 64] cos | sin per position
 
     static constexpr int kUnrollChunks = 4;   // `buf` must be a compile-time constant (register double buffer)
     static constexpr int kPrefetchDist = 1;
@@ -121,7 +132,7 @@ struct EpiLinear {
     }
 
     __device__ __forceinline__ void tile(State &st, const GemmTileInfo &ti, int row, int col0, const float (&v)[32],
-                                         uint8_t *stage, int lane, int buf, const float * /*acc*/) const {
+                                         uint8_t *stage, int lane, int buf, const float *acc) const {
         const int row_base = row - lane;                                     // first row of this warp's quarter
         if (row_base >= M || col0 >= N) return;                              // warp-uniform
         if (VT && col0 >= vt_col0) {
@@ -142,6 +153,11 @@ struct EpiLinear {
             return;
         }
         if (OUT_HALF) {
+            if (MODE == 3 && (col0 & 32) == 0) return;                      // input chunk: consumed by its gate chunk
+            const int ocol0 = MODE == 3 ? (col0 - 32) / 2 : col0, oN = MODE == 3 ? N / 2 : N;
+            const bool rot = ROPE && col0 < vt_col0;
+            const int pofs = (col0 & 32) ? -32 : 32;                         // partner chunk (RoPE half / GeGLU input)
+            const float *rrow = ROPE ? rope + static_cast<int64_t>(row < M ? row % S : 0) * 64 : nullptr;
             // stage 32 rows x 32 halves (64 B payload per 80-byte row), then lane (r4 = lane/4 .. 8 rows per pass, c8 = lane%4)
             uint4 *srow = reinterpret_cast<uint4 *>(stage + lane * GEMM_EPI_STAGE_ROW_BYTES);
 #pragma unroll
@@ -155,6 +171,35 @@ struct EpiLinear {
                 y[2] = act(pre(st, v[8 * j + 2], ba.z, ca.z)); y[3] = act(pre(st, v[8 * j + 3], ba.w, ca.w));
                 y[4] = act(pre(st, v[8 * j + 4], bb.x, cb.x)); y[5] = act(pre(st, v[8 * j + 5], bb.y, cb.y));
                 y[6] = act(pre(st, v[8 * j + 6], bb.z, cb.z)); y[7] = act(pre(st, v[8 * j + 7], bb.w, cb.w));
+                if (MODE == 3 || rot) {
+                    const int pc = col0 + pofs + 8 * j;
+                    const float4 a0 = *reinterpret_cast<const float4 *>(acc + pofs + 8 * j);
+                    const float4 a1 = *reinterpret_cast<const float4 *>(acc + pofs + 8 * j + 4);
+                    const float4 pba = __ldg(reinterpret_cast<const float4 *>(bias + pc));
+                    const float4 pbb = __ldg(reinterpret_cast<const float4 *>(bias + pc + 4));
+                    const float4 pca = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + pc)) : make_float4(0, 0, 0, 0);
+                    const float4 pcb = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + pc + 4)) : make_float4(0, 0, 0, 0);
+                    float p[8];
+                    p[0] = pre(st, a0.x, pba.x, pca.x); p[1] = pre(st, a0.y, pba.y, pca.y);
+                    p[2] = pre(st, a0.z, pba.z, pca.z); p[3] = pre(st, a0.w, pba.w, pca.w);
+                    p[4] = pre(st, a1.x, pbb.x, pcb.x); p[5] = pre(st, a1.y, pbb.y, pcb.y);
+                    p[6] = pre(st, a1.z, pbb.z, pcb.z); p[7] = pre(st, a1.w, pbb.w, pcb.w);
+                    if (MODE == 3) {
+#pragma unroll
+                        for (int k = 0; k < 8; ++k) y[k] = gelu_erf(p[k]) * y[k];          // y = gate, p = input
+                    } else {
+                        // HF apply_rotary_pos_emb: x cos + rotate_half(x) sin, rotate_half = (-x[32:], x[:32])
+                        const float4 c0v = __ldg(reinterpret_cast<const float4 *>(rrow + 8 * j));
+                        const float4 c1v = __ldg(reinterpret_cast<const float4 *>(rrow + 8 * j + 4));
+                        const float4 s0v = __ldg(reinterpret_cast<const float4 *>(rrow + 32 + 8 * j));
+                        const float4 s1v = __ldg(reinterpret_cast<const float4 *>(rrow + 32 + 8 * j + 4));
+                        const float cs[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
+                        const float sn[8] = {s0v.x, s0v.y, s0v.z, s0v.w, s1v.x, s1v.y, s1v.z, s1v.w};
+                        const float sg = (col0 & 32) ? 1.f : -1.f;
+#pragma unroll
+                        for (int k = 0; k < 8; ++k) y[k] = __fadd_rn(__fmul_rn(y[k], cs[k]), __fmul_rn(sg * p[k], sn[k]));
+                    }
+                }
                 uint4 pk;
                 __half2 h0 = __floats2half2_rn(y[0], y[1]), h1 = __floats2half2_rn(y[2], y[3]);
                 __half2 h2 = __floats2half2_rn(y[4], y[5]), h3 = __floats2half2_rn(y[6], y[7]);
@@ -169,8 +214,8 @@ struct EpiLinear {
             for (int i = 0; i < 4; ++i) {
                 const int rr = r8 + 8 * i;
                 const int grow = row_base + rr;
-                const int col = col0 + 8 * c;
-                if (grow < M && col + 8 <= N) {
+                const int col = ocol0 + 8 * c;
+                if (grow < M && col + 8 <= oN) {
                     const uint4 pk = *reinterpret_cast<const uint4 *>(stage + rr * GEMM_EPI_STAGE_ROW_BYTES + 16 * c);
                     *reinterpret_cast<uint4 *>(Yh + static_cast<int64_t>(grow) * ldy + col) = pk;
                 }
@@ -363,16 +408,19 @@ __global__ void fill_value_kernel(float *__restrict__ p, int n, float v) {
 
 // weight packing of a deferred-LayerNorm consumer (one warp per output row n):
 //   Wp[n,k] = fp16(gamma[k] W[n,k]),  c1[n] = sum_k Wp[n,k] (fp32),  c0[n] = sum_k beta[k] W[n,k] + bias[n]
-// gamma / beta NULL = identity LayerNorm (layer 0 consumes the already normalised embeddings)
+// gamma / beta NULL = identity LayerNorm (layer 0 consumes the already normalised embeddings), bias NULL = 0.
+// glu != 0 (GeGLU weight [2I, H], N = 2I): packed row n takes source row (n / 64) 32 + n % 32 of the input half for
+// n % 64 < 32, the same row of the gate half otherwise -- the row order EpiLinear<3, ..> expects
 __global__ void pack_defer_kernel(const float *__restrict__ W, const float *__restrict__ bias, const float *__restrict__ gamma,
                                   const float *__restrict__ beta, int N, int K, __half *__restrict__ Wp, float *__restrict__ c1,
-                                  float *__restrict__ c0) {
+                                  float *__restrict__ c0, int glu = 0) {
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (n >= N) return;
+    const int src = glu ? (n >> 6) * 32 + (n & 31) + ((n & 32) ? N / 2 : 0) : n;
     float s1 = 0.f, s0 = 0.f;
     for (int k = lane; k < K; k += 32) {
-        const float w = W[static_cast<int64_t>(n) * K + k];
+        const float w = W[static_cast<int64_t>(src) * K + k];
         const __half h = __float2half_rn(gamma ? gamma[k] * w : w);
         Wp[static_cast<int64_t>(n) * K + k] = h;
         s1 += __half2float(h);
@@ -382,7 +430,7 @@ __global__ void pack_defer_kernel(const float *__restrict__ W, const float *__re
     s0 = warp_sum(s0);
     if (lane == 0) {
         c1[n] = s1;
-        c0[n] = s0 + bias[n];
+        c0[n] = s0 + (bias ? bias[src] : 0.f);
     }
 }
 
@@ -446,6 +494,7 @@ __global__ void layernorm_kernel(const float *__restrict__ in, const float *__re
 }
 
 // modeling_bert.py:53-113 / modeling_roberta.py:146-159: (word + type) + position -> LayerNorm
+// modeling_modernbert.py ModernBertEmbeddings: pos = type = NULL, LayerNorm(word) (b = zeros: norm_bias=False)
 __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *__restrict__ type_ids,
                                 const float *__restrict__ word, const float *__restrict__ pos,
                                 const float *__restrict__ type, const float *__restrict__ w,
@@ -477,6 +526,10 @@ __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *
         if (i < nv) {
             const int col = (lane + 32 * i) * 4;
             const float4 a = __ldg(reinterpret_cast<const float4 *>(word + static_cast<int64_t>(id) * H + col));
+            if (!pos) {
+                x[i] = a;
+                continue;
+            }
             const float4 t = __ldg(reinterpret_cast<const float4 *>(type + static_cast<int64_t>(tt) * H + col));
             const float4 q = __ldg(reinterpret_cast<const float4 *>(pos + static_cast<int64_t>(p) * H + col));
             x[i].x = (a.x + t.x) + q.x;
@@ -599,9 +652,20 @@ __device__ __forceinline__ void att_write_row(const float *orow, float inv, __ha
     }
 }
 
+// sliding-window band of query q over keys [k0, k0 + 32): bit j set when |q - (k0 + j)| <= w; w = 0: no band (all set)
+__device__ __forceinline__ uint32_t band_bits(int q, int k0, int w) {
+    if (w <= 0) return 0xffffffffu;
+    const int lo = q - w - k0, hi = q + w - k0;
+    if (hi < 0 || lo > 31) return 0u;
+    const uint32_t up = hi >= 31 ? 0xffffffffu : (2u << hi) - 1u;        // bits 0 .. hi
+    const uint32_t dn = lo <= 0 ? 0xffffffffu : ~((1u << lo) - 1u);       // bits lo .. 31
+    return up & dn;
+}
+
+// window: ModernBERT sliding_attention half-window (keys |q - key| <= window), 0 = full attention
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
-                 const int32_t *__restrict__ mask, int B, int S, int heads, int H, __half *__restrict__ ctx) {
+                 const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                    // [128 rows x 128 B]
@@ -654,13 +718,13 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     const int qrow = warp * 32 + lane;
     const float *srow = sS + qrow * ATT_S_LD;
     // key validity (key < S and not padded) as four 32-bit words held by every thread: lane l of a warp tests key
-    // 32*w + l once, ballots, and the loops below only test bits
+    // 32*w + l once, ballots, and the loops below only test bits; the sliding-window band is per query row
     uint32_t kmask[4];
 #pragma unroll
     for (int w4 = 0; w4 < 4; ++w4) {
         const int key = 32 * w4 + lane;
         const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
-        kmask[w4] = __ballot_sync(0xffffffffu, ok);
+        kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(qrow, 32 * w4, window);
     }
     const float scale_log2 = rsqrtf(64.f) * 1.44269504088896340736f;
     float mx = -CUDART_INF_F;
@@ -721,7 +785,7 @@ constexpr int ATTL_SMEM = 80 * 1024 + ATT_S_BYTES + 1024 + 64;
 
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
-                      const int32_t *__restrict__ mask, int B, int S, int heads, int H, __half *__restrict__ ctx) {
+                      const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                    // [128 x 128 B]
@@ -779,7 +843,7 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
             for (int w4 = 0; w4 < 4; ++w4) {
                 const int key = key0 + 32 * w4 + lane;
                 const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
-                kmask[w4] = __ballot_sync(0xffffffffu, ok);
+                kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(qglob, key0 + 32 * w4, window);
             }
             if (pass == 0) {
 #pragma unroll
@@ -879,7 +943,11 @@ struct ac_encoder {
     CUtensorMap p_w1_last;
     // row statistics (ping-pong) and the per-GEMM_EPI_COLS-column partials the residual epilogues write
     float2 *stats_a = nullptr, *stats_b = nullptr, *stats_id = nullptr, *parts = nullptr;
-    float *ones = nullptr, *zeros = nullptr;
+    float *ones = nullptr, *zeros = nullptr;   // ones [H]; zeros [max(3H, 2I)]: beta / bias of the bias-free ModernBERT
+    // ModernBERT: per-layer half-window (0 = full attention), RoPE tables [AC_ENCODER_MAX_S, 64] (full, sliding), final_norm.
+    // Wqkv packs into wqkv_d / c1qkv / c0qkv, Wi (interleaved, 2I rows) into w1_d / c1f / c0f, mlp_norm into ln1w.
+    std::vector<int> window;
+    float *rope[2] = {nullptr, nullptr}, *final_norm = nullptr;
     std::vector<void *> allocs;
     int last_B = 0, last_S = 0;
     bool last_cls_only = false;
@@ -893,8 +961,8 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
     return AC_OK;
 }
 
-// softmax(Q K^T / 8 + mask) V out of e->qk / e->vT into e->ctx
-static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, cudaStream_t s) {
+// softmax(Q K^T / 8 + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention
+static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, cudaStream_t s) {
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden;
     // per-device: the attribute is a property of the (function, device) pair
@@ -909,10 +977,11 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, cu
     // algorithmic flops of softmax(QK^T)V at the true sequence length (the 128-wide tile does more)
     const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * static_cast<double>(S) * S * 64, 0.0, s);
     if (S <= 128)
-        attention_kernel<<<B * c.heads, ATT_THREADS, ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, e->ctx);
+        attention_kernel<<<B * c.heads, ATT_THREADS, ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window,
+                                                                    e->ctx);
     else
         attention_long_kernel<<<dim3(B * c.heads, (S + 127) / 128), ATT_THREADS, ATTL_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S,
-                                                                                                c.heads, H, e->ctx);
+                                                                                                c.heads, H, window, e->ctx);
     prof_end(slot, s);
     AC_LAUNCH_CHECK();
     return AC_OK;
@@ -949,8 +1018,60 @@ extern "C" int ac_encoder_destroy(ac_encoder *enc) {
     return AC_OK;
 }
 
+// ModernBERT weights (modeling_modernbert.py).  Wqkv consumes the un-normalised residual sums pending attn_norm (identity
+// for layer 0), Wi the sums pending mlp_norm: both packed as deferred-LayerNorm consumers with beta = bias = 0.
+static int pack_modernbert(ac_encoder *e, const ac_encoder_config *cfg, const ac_encoder_weights *w) {
+    const int H = cfg->hidden, I = cfg->intermediate, L = cfg->layers;
+    const size_t HH = static_cast<size_t>(H) * H;
+    int rc;
+#define CHK(x) do { if ((rc = (x))) return rc; } while (0)
+    CHK(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
+    CHK(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
+    CHK(pack_f32(e, &e->final_norm, w->final_norm_w, H));
+    CHK(pack_f32(e, &e->rope[0], cfg->rope_full, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
+    CHK(pack_f32(e, &e->rope[1], cfg->rope_sliding, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
+    e->window.assign(L, 0);
+    e->wqkv_d.assign(L, nullptr); e->c1qkv.assign(L, nullptr); e->c0qkv.assign(L, nullptr); e->wo.assign(L, nullptr);
+    e->ln1w.assign(L, nullptr); e->w1_d.assign(L, nullptr); e->c1f.assign(L, nullptr); e->c0f.assign(L, nullptr);
+    e->w2.assign(L, nullptr);
+    for (int l = 0; l < L; ++l) {
+        e->window[l] = cfg->layer_sliding[l] ? cfg->sliding_window : 0;
+        CHK(dev_alloc(e, &e->wqkv_d[l], 3 * HH));
+        CHK(dev_alloc(e, &e->c1qkv[l], 3 * static_cast<size_t>(H)));
+        CHK(dev_alloc(e, &e->c0qkv[l], 3 * static_cast<size_t>(H)));
+        pack_defer_kernel<<<(3 * H + 7) / 8, 256>>>(w->wqkv[l], nullptr, l ? w->attn_norm_w[l] : nullptr, nullptr, 3 * H, H,
+                                                    e->wqkv_d[l], e->c1qkv[l], e->c0qkv[l]);
+        CHK(check_cuda(cudaGetLastError(), "pack_defer_kernel Wqkv"));
+        CHK(pack_f16(e, &e->wo[l], w->ao_w[l], HH));
+        CHK(pack_f32(e, &e->ln1w[l], w->ao_ln_w[l], H));
+        CHK(dev_alloc(e, &e->w1_d[l], 2 * static_cast<size_t>(I) * H));
+        CHK(dev_alloc(e, &e->c1f[l], 2 * static_cast<size_t>(I)));
+        CHK(dev_alloc(e, &e->c0f[l], 2 * static_cast<size_t>(I)));
+        pack_defer_kernel<<<(2 * I + 7) / 8, 256>>>(w->wi[l], nullptr, w->ao_ln_w[l], nullptr, 2 * I, H, e->w1_d[l], e->c1f[l],
+                                                    e->c0f[l], 1);
+        CHK(check_cuda(cudaGetLastError(), "pack_defer_kernel Wi"));
+        CHK(pack_f16(e, &e->w2[l], w->ff2_w[l], static_cast<size_t>(H) * I));
+    }
+    if (cfg->cls_only) {
+        // plain interleaved Wi of the last layer: the CLS-only tail materialises mlp_norm (c1 / c0 are not used)
+        float *c1 = nullptr, *c0 = nullptr;
+        CHK(dev_alloc(e, &e->w1_last, 2 * static_cast<size_t>(I) * H));
+        CHK(dev_alloc(e, &c1, 2 * static_cast<size_t>(I)));
+        CHK(dev_alloc(e, &c0, 2 * static_cast<size_t>(I)));
+        pack_defer_kernel<<<(2 * I + 7) / 8, 256>>>(w->wi[L - 1], nullptr, nullptr, nullptr, 2 * I, H, e->w1_last, c1, c0, 1);
+        CHK(check_cuda(cudaGetLastError(), "pack_defer_kernel Wi (last layer)"));
+    }
+#undef CHK
+    return AC_OK;
+}
+
 extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_weights *w, ac_encoder **out) {
     AC_REQUIRE(cfg && w && out, "ac_encoder_create: null argument");
+    const bool mb = cfg->arch == AC_ARCH_MODERNBERT;
+    AC_REQUIRE(!mb || (cfg->max_pos == AC_ENCODER_MAX_S && cfg->layer_sliding && cfg->sliding_window > 0 && cfg->rope_full &&
+                       cfg->rope_sliding && w->wqkv && w->wi && w->final_norm_w && (cfg->layers == 1 || w->attn_norm_w)),
+               "ac_encoder_create: ModernBERT needs max_pos = %d, layer_sliding, sliding_window > 0, both RoPE tables, "
+               "wqkv, wi, final_norm_w and attn_norm_w", AC_ENCODER_MAX_S);
     AC_REQUIRE(cfg->precision == AC_PREC_F16, "ac_encoder_create: only AC_PREC_F16 (fp16 operands, fp32 accumulate) is implemented");
     AC_REQUIRE(cfg->hidden % 128 == 0 && cfg->hidden <= 1024, "ac_encoder_create: hidden=%d must be a multiple of 128, <= 1024", cfg->hidden);
     AC_REQUIRE(cfg->heads > 0 && cfg->hidden / cfg->heads == 64 && cfg->hidden % cfg->heads == 0,
@@ -964,59 +1085,66 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     const size_t T = static_cast<size_t>((cfg->max_tokens + 127) / 128 * 128);
     e->T = T;
 #define TRY(x) do { rc = (x); if (rc) { ac_encoder_destroy(e); return rc; } } while (0)
-    TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
-    TRY(pack_f32(e, &e->pos, w->pos_emb, static_cast<size_t>(cfg->max_pos) * H));
-    TRY(pack_f32(e, &e->type, w->type_emb, static_cast<size_t>(cfg->type_vocab) * H));
-    TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
-    TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, H));
-    e->wqkv_d.assign(L, nullptr); e->wo.assign(L, nullptr); e->w1_d.assign(L, nullptr); e->w2.assign(L, nullptr);
-    e->c1qkv.assign(L, nullptr); e->c0qkv.assign(L, nullptr); e->c1f.assign(L, nullptr); e->c0f.assign(L, nullptr);
-    e->bo.assign(L, nullptr); e->ln1w.assign(L, nullptr); e->ln1b.assign(L, nullptr);
-    e->b2.assign(L, nullptr); e->ln2w.assign(L, nullptr); e->ln2b.assign(L, nullptr);
-    const size_t HH = static_cast<size_t>(H) * H;
-    for (int l = 0; l < L; ++l) {
-        // fused QKV operand [3H, H]: the projection of layer l consumes the sums whose pending LayerNorm is the output
-        // LayerNorm of layer l-1 (identity for layer 0: the embeddings arrive normalised)
-        TRY(dev_alloc(e, &e->wqkv_d[l], 3 * HH));
-        TRY(dev_alloc(e, &e->c1qkv[l], 3 * static_cast<size_t>(H)));
-        TRY(dev_alloc(e, &e->c0qkv[l], 3 * static_cast<size_t>(H)));
-        const float *ws[3] = {w->q_w[l], w->k_w[l], w->v_w[l]};
-        const float *bs[3] = {w->q_b[l], w->k_b[l], w->v_b[l]};
-        const float *pg = l ? w->out_ln_w[l - 1] : nullptr, *pb = l ? w->out_ln_b[l - 1] : nullptr;
-        for (int j = 0; j < 3; ++j) {
-            pack_defer_kernel<<<(H + 7) / 8, 256>>>(ws[j], bs[j], pg, pb, H, H, e->wqkv_d[l] + j * HH, e->c1qkv[l] + j * H,
-                                                    e->c0qkv[l] + j * H);
-            TRY(check_cuda(cudaGetLastError(), "pack_defer_kernel qkv"));
+    e->cfg.layer_sliding = nullptr;   // copied into e->window / e->rope by pack_modernbert
+    e->cfg.rope_full = e->cfg.rope_sliding = nullptr;
+    if (mb) {
+        TRY(pack_modernbert(e, cfg, w));
+    } else {
+        TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
+        TRY(pack_f32(e, &e->pos, w->pos_emb, static_cast<size_t>(cfg->max_pos) * H));
+        TRY(pack_f32(e, &e->type, w->type_emb, static_cast<size_t>(cfg->type_vocab) * H));
+        TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
+        TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, H));
+        e->wqkv_d.assign(L, nullptr); e->wo.assign(L, nullptr); e->w1_d.assign(L, nullptr); e->w2.assign(L, nullptr);
+        e->c1qkv.assign(L, nullptr); e->c0qkv.assign(L, nullptr); e->c1f.assign(L, nullptr); e->c0f.assign(L, nullptr);
+        e->bo.assign(L, nullptr); e->ln1w.assign(L, nullptr); e->ln1b.assign(L, nullptr);
+        e->b2.assign(L, nullptr); e->ln2w.assign(L, nullptr); e->ln2b.assign(L, nullptr);
+        const size_t HH = static_cast<size_t>(H) * H;
+        for (int l = 0; l < L; ++l) {
+            // fused QKV operand [3H, H]: the projection of layer l consumes the sums whose pending LayerNorm is the output
+            // LayerNorm of layer l-1 (identity for layer 0: the embeddings arrive normalised)
+            TRY(dev_alloc(e, &e->wqkv_d[l], 3 * HH));
+            TRY(dev_alloc(e, &e->c1qkv[l], 3 * static_cast<size_t>(H)));
+            TRY(dev_alloc(e, &e->c0qkv[l], 3 * static_cast<size_t>(H)));
+            const float *ws[3] = {w->q_w[l], w->k_w[l], w->v_w[l]};
+            const float *bs[3] = {w->q_b[l], w->k_b[l], w->v_b[l]};
+            const float *pg = l ? w->out_ln_w[l - 1] : nullptr, *pb = l ? w->out_ln_b[l - 1] : nullptr;
+            for (int j = 0; j < 3; ++j) {
+                pack_defer_kernel<<<(H + 7) / 8, 256>>>(ws[j], bs[j], pg, pb, H, H, e->wqkv_d[l] + j * HH, e->c1qkv[l] + j * H,
+                                                        e->c0qkv[l] + j * H);
+                TRY(check_cuda(cudaGetLastError(), "pack_defer_kernel qkv"));
+            }
+            TRY(pack_f16(e, &e->wo[l], w->ao_w[l], HH));
+            TRY(pack_f32(e, &e->bo[l], w->ao_b[l], H));
+            TRY(pack_f32(e, &e->ln1w[l], w->ao_ln_w[l], H));
+            TRY(pack_f32(e, &e->ln1b[l], w->ao_ln_b[l], H));
+            // FFN1 of layer l consumes the sums pending the attention-output LayerNorm of layer l
+            TRY(dev_alloc(e, &e->w1_d[l], static_cast<size_t>(I) * H));
+            TRY(dev_alloc(e, &e->c1f[l], I));
+            TRY(dev_alloc(e, &e->c0f[l], I));
+            pack_defer_kernel<<<(I + 7) / 8, 256>>>(w->ff1_w[l], w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], I, H, e->w1_d[l], e->c1f[l],
+                                                    e->c0f[l]);
+            TRY(check_cuda(cudaGetLastError(), "pack_defer_kernel ffn1"));
+            TRY(pack_f16(e, &e->w2[l], w->ff2_w[l], static_cast<size_t>(H) * I));
+            TRY(pack_f32(e, &e->b2[l], w->ff2_b[l], H));
+            TRY(pack_f32(e, &e->ln2w[l], w->out_ln_w[l], H));
+            TRY(pack_f32(e, &e->ln2b[l], w->out_ln_b[l], H));
         }
-        TRY(pack_f16(e, &e->wo[l], w->ao_w[l], HH));
-        TRY(pack_f32(e, &e->bo[l], w->ao_b[l], H));
-        TRY(pack_f32(e, &e->ln1w[l], w->ao_ln_w[l], H));
-        TRY(pack_f32(e, &e->ln1b[l], w->ao_ln_b[l], H));
-        // FFN1 of layer l consumes the sums pending the attention-output LayerNorm of layer l
-        TRY(dev_alloc(e, &e->w1_d[l], static_cast<size_t>(I) * H));
-        TRY(dev_alloc(e, &e->c1f[l], I));
-        TRY(dev_alloc(e, &e->c0f[l], I));
-        pack_defer_kernel<<<(I + 7) / 8, 256>>>(w->ff1_w[l], w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], I, H, e->w1_d[l], e->c1f[l],
-                                                e->c0f[l]);
-        TRY(check_cuda(cudaGetLastError(), "pack_defer_kernel ffn1"));
-        TRY(pack_f16(e, &e->w2[l], w->ff2_w[l], static_cast<size_t>(H) * I));
-        TRY(pack_f32(e, &e->b2[l], w->ff2_b[l], H));
-        TRY(pack_f32(e, &e->ln2w[l], w->out_ln_w[l], H));
-        TRY(pack_f32(e, &e->ln2b[l], w->out_ln_b[l], H));
+        if (cfg->cls_only) {
+            TRY(pack_f16(e, &e->w1_last, w->ff1_w[L - 1], static_cast<size_t>(I) * H));
+            TRY(pack_f32(e, &e->b1_last, w->ff1_b[L - 1], I));
+        }
     }
-    if (cfg->cls_only) {
-        TRY(pack_f16(e, &e->w1_last, w->ff1_w[L - 1], static_cast<size_t>(I) * H));
-        TRY(pack_f32(e, &e->b1_last, w->ff1_b[L - 1], I));
-    }
+    const int nzeros = std::max(3 * H, 2 * I);
     TRY(dev_alloc(e, &e->stats_a, T));
     TRY(dev_alloc(e, &e->stats_b, T));
     TRY(dev_alloc(e, &e->stats_id, T));
     TRY(dev_alloc(e, &e->parts, static_cast<size_t>(H / GEMM_EPI_COLS) * T));
     TRY(dev_alloc(e, &e->ones, H));
-    TRY(dev_alloc(e, &e->zeros, H));
+    TRY(dev_alloc(e, &e->zeros, nzeros));
     fill_stats_identity_kernel<<<static_cast<unsigned>((T + 255) / 256), 256>>>(e->stats_id, static_cast<int64_t>(T));
     fill_value_kernel<<<(H + 255) / 256, 256>>>(e->ones, H, 1.f);
-    fill_value_kernel<<<(H + 255) / 256, 256>>>(e->zeros, H, 0.f);
+    fill_value_kernel<<<(nzeros + 255) / 256, 256>>>(e->zeros, nzeros, 0.f);
     TRY(check_cuda(cudaGetLastError(), "deferred-LayerNorm constants"));
     e->vt_elems = 2 * T * H;     // (b, h, d) rows x S_pad keys, S_pad = roundup(S, 8) <= 2*S for S >= 8
     TRY(dev_alloc(e, &e->x, T * H));
@@ -1049,13 +1177,14 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     TRY(make_tmap_2d(&e->m_ctx_cls, e->ctx_cls, 2, e->Bc, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_M, 64));
     TRY(make_tmap_2d(&e->m_ffn_cls, e->ffn_cls, 2, e->Bc, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_M, 64));
     e->p_wqkv_d.resize(L); e->p_wo.resize(L); e->p_w1_d.resize(L); e->p_w2.resize(L);
+    const int n1 = mb ? 2 * I : I;    // rows of the first FFN weight (ModernBERT: GeGLU input + gate)
     for (int l = 0; l < L; ++l) {
         TRY(make_tmap_2d(&e->p_wqkv_d[l], e->wqkv_d[l], 2, 3 * H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
         TRY(make_tmap_2d(&e->p_wo[l], e->wo[l], 2, H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
-        TRY(make_tmap_2d(&e->p_w1_d[l], e->w1_d[l], 2, I, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+        TRY(make_tmap_2d(&e->p_w1_d[l], e->w1_d[l], 2, n1, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
         TRY(make_tmap_2d(&e->p_w2[l], e->w2[l], 2, H, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_N, 64));
     }
-    if (cfg->cls_only) TRY(make_tmap_2d(&e->p_w1_last, e->w1_last, 2, I, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+    if (cfg->cls_only) TRY(make_tmap_2d(&e->p_w1_last, e->w1_last, 2, n1, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
     TRY(check_cuda(cudaDeviceSynchronize(), "encoder_create sync"));
 #undef TRY
     *out = e;
@@ -1067,10 +1196,81 @@ using EpiResid = EpiLinear<2, false, false>;                // bias + residual, 
 using EpiQKVDefer = EpiLinear<0, true, true, true>;         // r (acc - mu c1) + c0, fp16 out, V third transposed
 using EpiGeluDefer = EpiLinear<1, true, false, true>;       // GELU(r (acc - mu c1) + c0), fp16 out
 
+using EpiQKVRopeDefer = EpiLinear<0, true, true, true, true>;   // deferred LN + RoPE on q, k; V third transposed
+using EpiGegluDefer = EpiLinear<3, true, false, true>;        // GELU(input) * gate of the deferred-LN Wi, fp16 out
+using EpiGeglu = EpiLinear<3, true, false>;                   // the same on materialised LayerNorm rows (CLS-only tail)
+
 // One encoder projection = one GEMM (gemm_tc.cuh).  tb is the weight's GEMM_BLOCK_N-row-box map.
 template <class Epi>
 static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, int N, int K, const Epi &epi, cudaStream_t s) {
     return launch_gemm_tc<Epi, false, GEMM_KIND_F16>(ta, tb, M, N, K, epi, s);
+}
+
+// ModernBERT (modeling_modernbert.py ModernBertModel.forward): pre-LN blocks
+//     y += Wo attn(rope(Wqkv attn_norm(y)))        y += mlp.Wo GeGLU(Wi mlp_norm(y))        out = final_norm(y)
+// No LayerNorm is pending on the residual path, so the residual epilogues add the raw old sums (EpiResidDefer with the
+// identity LayerNorm: stats (0, 1), gamma 1, beta 0) and only the consuming projections apply attn_norm / mlp_norm deferred.
+static int forward_modernbert(ac_encoder *e, const int32_t *ids, const int32_t *mask, int B, int S, float *out_unit_cls,
+                              cudaStream_t s) {
+    const ac_encoder_config &c = e->cfg;
+    const int H = c.hidden, I = c.intermediate, M = B * S;
+    const int S_pad = (S + 7) / 8 * 8;
+    const int wpb = 8;
+    const int row_blocks = (M + wpb - 1) / wpb;
+    const int nparts = H / GEMM_EPI_COLS;
+    const int64_t pstride = static_cast<int64_t>(e->T);
+    int rc;
+    embed_ln_kernel<<<row_blocks, wpb * 32, 0, s>>>(ids, nullptr, e->word, nullptr, nullptr, e->emb_ln_w, e->zeros, c.ln_eps, B, S,
+                                                    H, c.arch, c.pad_idx, c.vocab, c.max_pos, c.type_vocab, e->x, e->xh);
+    AC_LAUNCH_CHECK();
+    const float2 *st_in = e->stats_id;     // layer 0: attn_norm is Identity
+    for (int l = 0; l < c.layers; ++l) {
+        const float *rope = e->rope[e->window[l] ? 1 : 0];
+        EpiQKVRopeDefer eq{e->c0qkv[l], nullptr, e->qk, M, 3 * H, 2 * H, 0, e->vT, 2 * H, S, S_pad, H, e->c1qkv[l], st_in, rope};
+        if ((rc = launch_linear(e->m_xh, e->p_wqkv_d[l], M, 3 * H, H, eq, s))) return rc;
+        if ((rc = launch_attention(e, mask, B, S, e->window[l], s))) return rc;
+        if (l == c.layers - 1 && c.cls_only && static_cast<size_t>(B) <= e->Bc) {
+            // CLS-only tail: y_cls += Wo ctx_cls; mlp_norm materialised; GeGLU; y_cls += mlp.Wo h; final_norm; normalise
+            const int cb = (B + wpb - 1) / wpb;
+            gather_cls_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, e->ctx_cls, e->x_cls);
+            AC_LAUNCH_CHECK();
+            EpiResid eo{e->zeros, e->x_cls, e->tmp_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
+            if ((rc = launch_linear(e->m_ctx_cls, e->p_wo[l], B, H, H, eo, s))) return rc;
+            layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->tmp_cls, e->ln1w[l], e->zeros, c.ln_eps, B, H, nullptr, e->xh_cls);
+            AC_LAUNCH_CHECK();
+            EpiGeglu e1{e->zeros, nullptr, e->ffn_cls, B, 2 * I, I, 0, nullptr, 0, 0, 0, 0};
+            if ((rc = launch_linear(e->m_xh_cls, e->p_w1_last, B, 2 * I, H, e1, s))) return rc;
+            EpiResid e2{e->zeros, e->tmp_cls, e->x_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
+            if ((rc = launch_linear(e->m_ffn_cls, e->p_w2[l], B, H, I, e2, s))) return rc;
+            layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->x_cls, e->final_norm, e->zeros, c.ln_eps, B, H, e->tmp_cls, nullptr);
+            AC_LAUNCH_CHECK();
+            if ((rc = launch_cls_normalize(e->tmp_cls, B, 1, H, out_unit_cls, s))) return rc;
+            e->last_B = B;
+            e->last_S = S;
+            e->last_cls_only = true;
+            return AC_OK;
+        }
+        EpiResidDefer eo{e->zeros, e->x, e->xh, e->stats_id, e->ones, e->zeros, e->parts, pstride, M, H, H};
+        if ((rc = launch_linear(e->m_ctx, e->p_wo[l], M, H, H, eo, s))) return rc;
+        ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
+        AC_LAUNCH_CHECK();
+        EpiGegluDefer e1{e->c0f[l], nullptr, e->ffn, M, 2 * I, I, 0, nullptr, 0, 0, 0, 0, e->c1f[l], e->stats_b};
+        if ((rc = launch_linear(e->m_xh, e->p_w1_d[l], M, 2 * I, H, e1, s))) return rc;
+        EpiResidDefer e2{e->zeros, e->x, e->xh, e->stats_id, e->ones, e->zeros, e->parts, pstride, M, H, H};
+        if ((rc = launch_linear(e->m_ffn, e->p_w2[l], M, H, I, e2, s))) return rc;
+        ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_a);
+        AC_LAUNCH_CHECK();
+        st_in = e->stats_a;
+    }
+    // full hidden state requested (cls_only = 0): final_norm on every row
+    layernorm_kernel<<<row_blocks, wpb * 32, 0, s>>>(e->x, e->final_norm, e->zeros, c.ln_eps, M, H, e->tmp, nullptr);
+    AC_LAUNCH_CHECK();
+    if ((rc = launch_cls_normalize(e->tmp, B, S, H, out_unit_cls, s))) return rc;
+    e->last_B = B;
+    e->last_S = S;
+    e->last_cls_only = false;
+    e->last_hidden = e->tmp;
+    return AC_OK;
 }
 
 extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids,
@@ -1097,6 +1297,7 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
             return rc;
         e->vt_B = B; e->vt_S = S;
     }
+    if (c.arch == AC_ARCH_MODERNBERT) return forward_modernbert(e, ids, mask, B, S, out_unit_cls, s);
     const int wpb = 8;
     const int row_blocks = (M + wpb - 1) / wpb;
     const int nparts = H / GEMM_EPI_COLS;
@@ -1113,7 +1314,7 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
     for (int l = 0; l < c.layers; ++l) {
         EpiQKVDefer eq{e->c0qkv[l], nullptr, e->qk, M, 3 * H, 2 * H, 0, e->vT, 2 * H, S, S_pad, H, e->c1qkv[l], st_in};
         if ((rc = launch_linear(e->m_xh, e->p_wqkv_d[l], M, 3 * H, H, eq, s))) return rc;
-        if ((rc = launch_attention(e, mask, B, S, s))) return rc;
+        if ((rc = launch_attention(e, mask, B, S, 0, s))) return rc;
         if (l == c.layers - 1 && c.cls_only && static_cast<size_t>(B) <= e->Bc) {
             // ---- CLS-only tail of the last layer (classifier.py:1272 pools row 0): M = B rows.  LN_pending is materialised on
             // the CLS rows and the tail runs on ordinary LayerNorm kernels and the plain (not gamma-scaled) FFN1 weight

@@ -17,6 +17,25 @@ def bert_base_state_dict(seed: int = 1234, **cfg_over):
     return m, cfg
 
 
+def modernbert_base(seed: int = 1234):
+    """HF ModernBertModel(ModernBertConfig()) == ModernBERT-base architecture (22 x 768, 12 heads, GeGLU I = 1152, vocab 50368,
+    sliding half-window 64 on two of every three layers), random init under torch.manual_seed(seed)."""
+    from transformers import ModernBertConfig, ModernBertModel
+    torch.manual_seed(seed)
+    cfg = ModernBertConfig()
+    m = ModernBertModel(cfg)
+    m.eval()
+    return m, cfg
+
+
+def modernbert_ids(B: int, S: int, seed: int = 7) -> torch.Tensor:
+    """uniform in [1000, 50000), [CLS]=50281 first, [SEP]=50282 last, never the pad id 50283; int32 [B,S] on the host."""
+    g = torch.Generator().manual_seed(seed)
+    ids = torch.randint(1000, 50000, (B, S), generator=g, dtype=torch.int64)
+    ids[:, 0], ids[:, -1] = 50281, 50282
+    return ids.to(torch.int32)
+
+
 def synthetic_ids(B: int, S: int, vocab: int = 30522, seed: int = 7) -> torch.Tensor:
     """uniform in [1000, vocab), [CLS]=101 first, [SEP]=102 last, no padding; int32 [B,S] on the host."""
     g = torch.Generator().manual_seed(seed)

@@ -193,9 +193,10 @@ int ac_ewc_penalty(const ac_head_params *p, const ac_head_params *fisher, const 
 
 /* ------------------------------------------------------------------------------------------
  * Stage E -- encoder.  Replaces `self.model(**inputs).last_hidden_state[:,0,:]` + F.normalize at
- *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel forward).
+ *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel / ModernBertModel forward).
  * ------------------------------------------------------------------------------------------ */
-enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1 };
+enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2 };
+#define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts (the reference truncates at 512) */
 enum {
     AC_PREC_TF32 = 0,   /* wgmma .tf32 on fp32 storage (kNN coarse pass, ac_linear_tc tests) */
     AC_PREC_F16 = 1     /* wgmma .f16 with fp16 operands (RNE from fp32; same 10-bit mantissa as tf32),
@@ -212,9 +213,20 @@ typedef struct {
     int max_tokens;      /* workspace is sized for B*S <= max_tokens */
     int cls_only;        /* != 0: the last layer's output projection / FFN / LayerNorms run on the CLS rows only
                             (classifier.py:1272 uses nothing else); 0 keeps the full last hidden state */
+    /* AC_ARCH_MODERNBERT only (ignored otherwise).  max_pos must be AC_ENCODER_MAX_S (RoPE has no position table). */
+    int sliding_window;          /* half-window w = local_attention / 2: a sliding layer's query i sees keys |i - j| <= w */
+    const int32_t *layer_sliding;  /* HOST array [layers]: 1 = sliding_attention, 0 = full_attention (config.layer_types) */
+    const float *rope_full;      /* DEVICE [AC_ENCODER_MAX_S, 64] fp32 RoPE table of the full-attention layers:      */
+    const float *rope_sliding;   /*   row = position, [0, 32) cos, [32, 64) sin of the 32 frequencies (HF
+                                       ModernBertRotaryEmbedding's formula, built by the caller); the sliding layers' table */
 } ac_encoder_config;
 
-/* device pointers to the HF state_dict tensors (fp32, HF layout [out,in]) */
+/* device pointers to the HF state_dict tensors (fp32, HF layout [out,in]).
+ * AC_ARCH_MODERNBERT (models/modernbert/modeling_modernbert.py, every bias absent) uses only
+ *   word_emb   embeddings.tok_embeddings      emb_ln_w  embeddings.norm
+ *   ao_w       layers.l.attn.Wo               ao_ln_w   layers.l.mlp_norm
+ *   ff2_w      layers.l.mlp.Wo
+ * and the fields after out_ln_b; every other pointer may be NULL. */
 typedef struct {
     const float *word_emb, *pos_emb, *type_emb, *emb_ln_w, *emb_ln_b;
     /* arrays of `layers` device pointers each (host arrays of device pointers) */
@@ -222,6 +234,11 @@ typedef struct {
     const float *const *ao_w, *const *ao_b, *const *ao_ln_w, *const *ao_ln_b;
     const float *const *ff1_w, *const *ff1_b, *const *ff2_w, *const *ff2_b;
     const float *const *out_ln_w, *const *out_ln_b;
+    /* AC_ARCH_MODERNBERT */
+    const float *const *attn_norm_w;  /* [layers] layers.l.attn_norm (entry 0 unused: layer 0's attn_norm is Identity) */
+    const float *final_norm_w;        /* final_norm */
+    const float *const *wqkv;         /* [layers] layers.l.attn.Wqkv [3H, H], q, k, v thirds */
+    const float *const *wi;           /* [layers] layers.l.mlp.Wi [2I, H], input rows then gate rows */
 } ac_encoder_weights;
 
 typedef struct ac_encoder ac_encoder;
@@ -230,7 +247,8 @@ typedef struct ac_encoder ac_encoder;
 int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_weights *w, ac_encoder **out);
 int ac_encoder_destroy(ac_encoder *enc);
 
-/* ids[B,S] int32 token ids, mask[B,S] int32 (1 keep / 0 pad; NULL = all ones), type_ids nullable.
+/* ids[B,S] int32 token ids, mask[B,S] int32 (1 keep / 0 pad; NULL = all ones), type_ids nullable (ignored by
+ * AC_ARCH_MODERNBERT, whose RoPE positions are 0..S-1 for every sequence, padded or not).  S <= AC_ENCODER_MAX_S.
  * out_unit_cls[B,H] = L2-normalised (eps 1e-12) CLS row of the last hidden state. */
 int ac_encoder_forward_cls(ac_encoder *enc, const int32_t *ids, const int32_t *mask,
                            const int32_t *type_ids, int B, int S, float *out_unit_cls,
