@@ -22,7 +22,9 @@ AC_KNN_AUTO, AC_KNN_EXACT, AC_KNN_TENSOR = 0, 1, 2
 AC_KNN_MAX_K = 2048
 AC_KNN_TENSOR_MAX_K = 1024
 AC_ACT_LOGITS, AC_ACT_SOFTMAX, AC_ACT_SIGMOID = 0, 1, 2
-AC_LOSS_CE, AC_LOSS_BCE = 0, 1
+AC_LOSS_CE, AC_LOSS_BCE, AC_LOSS_CE_STRATEGIC = 0, 1, 2
+AC_COST_LINEAR, AC_COST_SEPARABLE = 0, 1
+AC_STRATEGIC_CANDIDATES = 50
 AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT = 0, 1, 2
 AC_ENCODER_MAX_S = 512
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
@@ -32,6 +34,7 @@ EXPORTS = [
     "ac_knn_workspace_bytes", "ac_knn_l2_topk", "ac_knn_make_shadow", "ac_row_sqnorm", "ac_topk_merge", "ac_proto_scores",
     "ac_segment_mean", "ac_memory_append_prune",
     "ac_head_forward", "ac_head_train_workspace_bytes", "ac_head_train_step", "ac_head_train_epoch", "ac_head_phase_timing", "ac_head_train_plan", "ac_head_grad", "ac_ewc_penalty",
+    "ac_strategic_workspace_bytes", "ac_strategic_best_response", "ac_head_train_strategic_workspace_bytes", "ac_head_train_strategic",
     "ac_encoder_create", "ac_encoder_destroy", "ac_encoder_forward_cls", "ac_encoder_last_hidden", "ac_linear_tc",
     "ac_proto_class_scores", "ac_proto_class_scores_n", "ac_blend_dense", "ac_topk_desc_workspace_bytes", "ac_topk_desc", "ac_blend_topk",
     "ac_pipeline_create", "ac_pipeline_destroy", "ac_pipeline_predict_device", "ac_pipeline_predict_host",
@@ -56,7 +59,13 @@ class TrainCfg(Structure):
                 ("step", c_int), ("loss_kind", c_int), ("dropout_p", c_float),
                 ("mask0", c_void_p), ("mask1", c_void_p), ("seed", c_uint64),
                 ("ewc_fisher", POINTER(HeadParams)), ("ewc_star", POINTER(HeadParams)),
-                ("ewc_lambda", c_float), ("ewc_C_old", c_int)]
+                ("ewc_lambda", c_float), ("ewc_C_old", c_int),
+                ("n_regular", c_int), ("strategic_lambda", c_float)]
+
+
+class StrategicCfg(Structure):
+    _fields_ = [("cost_kind", c_int), ("c1", c_void_p), ("c2", c_void_p), ("delta", c_float * 10),
+                ("dropout_p", c_float), ("seed", c_uint64), ("step", c_int)]
 
 
 class EncoderConfig(Structure):
@@ -116,6 +125,13 @@ def load_library() -> ctypes.CDLL:
                                POINTER(HeadParams), c_float, c_void_p, c_void_p, c_size_t, c_void_p]
     L.ac_ewc_penalty.argtypes = [POINTER(HeadParams), POINTER(HeadParams), POINTER(HeadParams), c_float, c_float,
                                  c_int, c_void_p, c_void_p]
+    L.ac_strategic_workspace_bytes.argtypes = [c_int, POINTER(HeadParams), POINTER(c_size_t)]
+    L.ac_strategic_best_response.argtypes = [c_void_p, c_int, POINTER(HeadParams), POINTER(StrategicCfg), c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_size_t, c_void_p]
+    L.ac_head_train_strategic_workspace_bytes.argtypes = [c_int, POINTER(HeadParams), POINTER(c_size_t)]
+    L.ac_head_train_strategic.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(HeadParams), POINTER(HeadParams),
+                                          POINTER(HeadParams), POINTER(TrainCfg), POINTER(StrategicCfg), c_void_p, c_void_p,
+                                          c_size_t, c_void_p]
     L.ac_encoder_create.argtypes = [POINTER(EncoderConfig), POINTER(EncoderWeights), POINTER(c_void_p)]
     L.ac_encoder_destroy.argtypes = [c_void_p]
     L.ac_encoder_forward_cls.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
@@ -307,8 +323,9 @@ def head_forward(X: torch.Tensor, p: dict, act: int = AC_ACT_LOGITS) -> torch.Te
 
 def head_train_step(X, targets, p, m, v, *, step, loss_kind=AC_LOSS_CE, lr=1e-3, betas=(0.9, 0.999), eps=1e-8,
                     weight_decay=0.01, max_norm=1.0, dropout_p=0.1, masks=None, seed=0,
-                    ewc=None, out_stats=None):
+                    ewc=None, out_stats=None, n_regular=0, strategic_lambda=0.0):
     """One optimizer step in place on p/m/v.  ewc = (fisher_dict, star_dict, lambda, C_old) or None.
+    loss_kind=AC_LOSS_CE_STRATEGIC: X = [x ; br] with n_regular rows each, targets repeated.
     Returns the device tensor [task_loss, ewc_penalty, grad_norm]."""
     L = load_library()
     X = _f32c(X)
@@ -318,6 +335,7 @@ def head_train_step(X, targets, p, m, v, *, step, loss_kind=AC_LOSS_CE, lr=1e-3,
     cfg.lr, cfg.beta1, cfg.beta2, cfg.eps = lr, betas[0], betas[1], eps
     cfg.weight_decay, cfg.max_norm = weight_decay, max_norm
     cfg.step, cfg.loss_kind, cfg.dropout_p, cfg.seed = step, loss_kind, dropout_p, seed
+    cfg.n_regular, cfg.strategic_lambda = int(n_regular), float(strategic_lambda)
     keep = []
     if masks is not None:
         m0, m1 = _f32c(masks[0]), _f32c(masks[1])
@@ -409,6 +427,79 @@ def head_grad(X, targets, p, *, loss_kind=AC_LOSS_CE, grad_out=None, fisher=None
                          ctypes.byref(g) if g is not None else None, ctypes.byref(f) if f is not None else None,
                          float(inv_n_batches), loss.data_ptr(), ws.data_ptr(), ws.numel(), stream_ptr()), "ac_head_grad")
     return loss
+
+
+_DELTAS = None
+
+
+def strategic_deltas() -> list:
+    """The 10 feature moves of the reference's candidate set (strategic.py:110), with its fp32 bits."""
+    global _DELTAS
+    if _DELTAS is None:
+        _DELTAS = torch.linspace(-2.0, 2.0, 10).tolist()
+    return _DELTAS
+
+
+def _strategic_cfg(cost_kind, c1, c2, dropout_p, seed, step):
+    sc = StrategicCfg()
+    sc.cost_kind = int(cost_kind)
+    sc.c1 = c1.data_ptr()
+    sc.c2 = c2.data_ptr() if c2 is not None else None
+    for j, d in enumerate(strategic_deltas()):
+        sc.delta[j] = d
+    sc.dropout_p, sc.seed, sc.step = float(dropout_p), int(seed), int(step)
+    return sc
+
+
+def strategic_best_response(X, p, cost_kind, c1, c2=None, *, dropout_p=0.0, seed=0, step=0, want_rows=True):
+    """Best response of every row of X [B, D] against the head p: (choice int32 [B], utility fp32 [B], Y [B, D] or None).
+    c1, c2: CUDA fp32 [D] cost coefficients (c2 only for AC_COST_SEPARABLE)."""
+    L = load_library()
+    X = _f32c(X)
+    B = X.shape[0]
+    hp = head_params_struct(p)
+    c1 = _f32c(c1)
+    c2 = _f32c(c2) if c2 is not None else None
+    sc = _strategic_cfg(cost_kind, c1, c2, dropout_p, seed, step)
+    nbytes = c_size_t(0)
+    check(L.ac_strategic_workspace_bytes(B, ctypes.byref(hp), ctypes.byref(nbytes)), "ac_strategic_workspace_bytes")
+    ws = _workspace(nbytes.value, X.device)
+    choice = torch.empty((B,), dtype=torch.int32, device=X.device)
+    util = torch.empty((B,), dtype=torch.float32, device=X.device)
+    Y = torch.empty_like(X) if want_rows else None
+    check(L.ac_strategic_best_response(X.data_ptr(), B, ctypes.byref(hp), ctypes.byref(sc), choice.data_ptr(), util.data_ptr(),
+                                       ptr(Y), ws.data_ptr(), ws.numel(), stream_ptr()), "ac_strategic_best_response")
+    return choice, util, Y
+
+
+def head_train_strategic(X, targets, perms, p, m, v, *, cost_kind, c1, c2=None, lr, strategic_lambda, dropout_p=0.1, seed=0,
+                         betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, max_norm=1.0):
+    """classifier.py:1602-1647 in one call: perms int64 [epochs * n] (the DataLoader orders), fresh moments m / v (step 1 first).
+    Returns the device step statistics [steps, 3] = (strategic loss, 0, grad norm before clipping)."""
+    L = load_library()
+    X = _f32c(X)
+    n = X.shape[0]
+    epochs = perms.numel() // n
+    hp, hm, hv = head_params_struct(p), head_params_struct(m), head_params_struct(v)
+    cfg = TrainCfg()
+    cfg.lr, cfg.beta1, cfg.beta2, cfg.eps = lr, betas[0], betas[1], eps
+    cfg.weight_decay, cfg.max_norm = weight_decay, max_norm
+    cfg.step, cfg.loss_kind, cfg.dropout_p, cfg.seed = 1, AC_LOSS_CE_STRATEGIC, dropout_p, seed
+    cfg.strategic_lambda = float(strategic_lambda)
+    c1 = _f32c(c1)
+    c2 = _f32c(c2) if c2 is not None else None
+    sc = _strategic_cfg(cost_kind, c1, c2, dropout_p, seed, 0)
+    nbytes = c_size_t(0)
+    check(L.ac_head_train_strategic_workspace_bytes(n, ctypes.byref(hp), ctypes.byref(nbytes)), "ac_head_train_strategic_workspace_bytes")
+    ws = _workspace(nbytes.value, X.device)
+    batch = min(16, n)
+    stats = torch.zeros((epochs * ((n + batch - 1) // batch), 3), dtype=torch.float32, device=X.device)
+    targets = targets.to(device=X.device, dtype=torch.int64).contiguous()
+    perms = perms.to(device=X.device, dtype=torch.int64).contiguous()
+    check(L.ac_head_train_strategic(X.data_ptr(), targets.data_ptr(), perms.data_ptr(), n, epochs, ctypes.byref(hp), ctypes.byref(hm),
+                                    ctypes.byref(hv), ctypes.byref(cfg), ctypes.byref(sc), stats.data_ptr(), ws.data_ptr(), ws.numel(),
+                                    stream_ptr()), "ac_head_train_strategic")
+    return stats
 
 
 def ewc_penalty(p, fisher, star, lam: float, batch_size: Optional[int], C_old: int = 0) -> torch.Tensor:

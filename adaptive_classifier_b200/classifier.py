@@ -5,8 +5,10 @@ types, label-id rules, blending formulas and error behaviour (citations inline).
 the H100 through the C ABI: encoder (csrc/encoder.cu), prototype kNN (csrc/knn_*.cu), adaptive head +
 AdamW/EWC (csrc/head.cu).  HuggingFace is used for checkpoint/tokenizer IO only.
 
-Out of scope (SURVEY.md section 2): ONNX export/ORT inference (use_onnx is accepted and ignored), strategic mode,
-Hub push.  Persistence keeps the reference's on-disk format (persistence.py).
+Strategic mode (classifier.py:1573-1823, strategic.py) is supported: the best-response search runs in csrc/strategic.cu and the
+strategic training step in the training kernel (AC_LOSS_CE_STRATEGIC); the label blends stay host dicts.
+Out of scope (SURVEY.md section 2): ONNX export/ORT inference (use_onnx is accepted and ignored), Hub push.  Persistence keeps
+the reference's on-disk format (persistence.py).
 """
 from __future__ import annotations
 
@@ -24,6 +26,7 @@ from . import _cabi
 from .ewc import EWC
 from .memory import PrototypeMemory
 from .models import AdaptiveHead, Example, ModelConfig
+from .strategic import CostFunctionFactory, StrategicEvaluator, StrategicOptimizer
 
 logger = logging.getLogger(__name__)
 
@@ -82,11 +85,28 @@ class AdaptiveClassifier:
         self.strategic_optimizer = None
         self.strategic_evaluator = None
         if self.config.enable_strategic_mode:
-            raise _cabi.AdaptiveB200Error("strategic mode is out of scope of the GPU hot path (SURVEY.md section 2 #9)")
+            self._initialize_strategic_components()
+
+    def _initialize_strategic_components(self):
+        """classifier.py:1573-1592: an empty / missing coefficient set logs a warning and leaves strategic mode off; a failing
+        factory call (dict coefficients without feature names, an unknown cost type) is logged and disables it."""
+        try:
+            if self.config.cost_coefficients:
+                self.strategic_cost_function = CostFunctionFactory.create_cost_function(
+                    cost_type=self.config.cost_function_type, cost_coefficients=self.config.cost_coefficients)
+                self.strategic_optimizer = StrategicOptimizer(self.strategic_cost_function)
+                self.strategic_evaluator = StrategicEvaluator(self.strategic_cost_function)
+                logger.info(f"Initialized strategic mode with {self.config.cost_function_type} cost function")
+            else:
+                logger.warning("Strategic mode enabled but no cost coefficients provided")
+        except Exception as e:
+            logger.error(f"Failed to initialize strategic components: {e}")
+            self.config.enable_strategic_mode = False
 
     @property
     def strategic_mode(self) -> bool:
-        return False
+        """classifier.py:1594-1600."""
+        return self.config.enable_strategic_mode and self.strategic_cost_function is not None
 
     @property
     def _device_lock(self):
@@ -168,6 +188,8 @@ class AdaptiveClassifier:
                 self.adaptive_head.update_num_classes(len(self.label_to_id))
                 self.adaptive_head = self.adaptive_head.to(self.device)
             self._train_adaptive_head()
+            if self.strategic_mode and self.train_steps % self.config.strategic_training_frequency == 0:   # classifier.py:194-197
+                self._perform_strategic_training()
         self.memory._rebuild_index()                           # classifier.py:200
 
     def _initialize_adaptive_head(self):
@@ -316,7 +338,9 @@ class AdaptiveClassifier:
         """classifier.py:392-413."""
         if not text:
             raise ValueError("Empty input text")
-        return self._predict_regular(text, k)
+        if not self.strategic_mode:
+            return self._predict_regular(text, k)
+        return self._predict_dual(text, k)
 
     def _head_probs(self, emb: torch.Tensor) -> Optional[torch.Tensor]:
         if self.adaptive_head is None:
@@ -325,10 +349,12 @@ class AdaptiveClassifier:
             self.adaptive_head.eval()
             return _cabi.head_forward(emb.contiguous(), self.adaptive_head._param_dict(), _cabi.AC_ACT_SOFTMAX)
 
-    def _predict_regular(self, text: str, k: int = 5) -> List[Tuple[str, float]]:
+    def _predict_regular(self, text: str, k: int = 5, emb: Optional[torch.Tensor] = None) -> List[Tuple[str, float]]:
         """classifier.py:415-480: prototype scores over ALL classes, head softmax over all classes,
-        per-label weights from training_history (<10 -> 0.3/0.7 else 0.7/0.3), renormalise, top k."""
-        emb = self._embed_device([text])
+        per-label weights from training_history (<10 -> 0.3/0.7 else 0.7/0.3), renormalise, top k.
+        emb: the text's unit CLS row when the caller has it already."""
+        if emb is None:
+            emb = self._embed_device([text])
         max_classes = len(self.id_to_label) if self.id_to_label else k
         proto_preds = self.memory.get_nearest_prototypes_batch(emb, max_classes)[0]
         head_preds = []
@@ -349,6 +375,143 @@ class AdaptiveClassifier:
         if total > 0:
             predictions = [(label, score / total) for label, score in predictions]
         return predictions[:k]
+
+    # ------------------------------------------------------------------------------------------ strategic mode
+    def _perform_strategic_training(self):
+        """classifier.py:369-390: every stored example in memory order (label insertion order, then list order), embeddings as
+        stored (not re-normalised)."""
+        if not self.strategic_mode or not self.memory.examples:
+            return
+        all_embeddings, all_labels = [], []
+        for label in self.memory.examples:
+            for example in self.memory.examples[label]:
+                all_embeddings.append(example.embedding)
+                all_labels.append(self.label_to_id[label])
+        if all_embeddings:
+            X = torch.stack(all_embeddings).to(self.device, dtype=torch.float32)
+            Y = torch.tensor(all_labels, dtype=torch.long, device=self.device)
+            self._strategic_training_step(X, Y)
+
+    def _strategic_training_step(self, all_embeddings: torch.Tensor, all_labels: torch.Tensor):
+        """classifier.py:1602-1647: 5 epochs of DataLoader(batch min(16, N), shuffle, manual_seed(42)) batches, fresh
+        AdamW(lr = learning_rate / 2, wd 0.01), clip 1.0, loss = strategic_loss (strategic.py:200-242) with the best responses
+        searched in train mode.  All steps run in one library call (ac_head_train_strategic) with no host synchronisation;
+        the per-step (loss, 0, grad norm) stay on the device in `last_strategic_trace`."""
+        if not self.strategic_mode or self.adaptive_head is None:
+            return
+        cost = self.strategic_cost_function
+        n = all_embeddings.shape[0]
+        gen = torch.Generator().manual_seed(42)
+        perms = torch.cat([dataloader_epoch_permutation(gen, n) for _ in range(5)])
+        with self._device_lock:
+            X = all_embeddings.to(self.device, dtype=torch.float32).contiguous()
+            c1, c2 = cost.device_coefficients(X.shape[1], X.device)
+            p, m, v = self._head_blocks()
+            self.adaptive_head.train()
+            self.last_strategic_trace = _cabi.head_train_strategic(
+                X, all_labels, perms, p, m, v, cost_kind=cost.cost_kind, c1=c1, c2=c2, lr=self.config.learning_rate * 0.5,
+                strategic_lambda=self.config.strategic_lambda, dropout_p=self._dropout_p, seed=int(torch.initial_seed() & 0x7FFFFFFF))
+            self.adaptive_head.eval()
+
+    def _best_response(self, emb: torch.Tensor) -> torch.Tensor:
+        """Best responses of the rows of emb [B, D] (device) against the eval-mode head; with no head every candidate has
+        the same score (the reference's uniform 1/C) and the cost-free x itself wins."""
+        if self.adaptive_head is None:
+            return emb
+        with self._device_lock:
+            self.adaptive_head.eval()
+            _, _, br = self.strategic_cost_function.compute_best_response(emb.contiguous(), self.adaptive_head._param_dict())
+            return br
+
+    def _coefficients_usable(self, what: str) -> bool:
+        """The reference's torch.dot raises for coefficients of the wrong length or a non-floating dtype and its predict
+        methods fall back to regular prediction; here that is decided before anything is launched."""
+        try:
+            self.strategic_cost_function.device_coefficients(self.embedding_dim, self.device)
+            return True
+        except ValueError as e:
+            logger.warning(f"{what} prediction failed: {e}. Falling back to regular prediction.")
+            return False
+
+    def _predict_dual(self, text: str, k: int = 5) -> List[Tuple[str, float]]:
+        """classifier.py:482-522: 0.6 regular + 0.4 strategic over the union of labels.  The text is embedded once."""
+        emb = self._embed_device([text])
+        regular_preds = self._predict_regular(text, k, emb)
+        strategic_preds = self.predict_strategic(text, k, emb)
+        blended_scores = {}
+        regular_weight = self.config.strategic_blend_regular_weight
+        strategic_weight = self.config.strategic_blend_strategic_weight
+        for label, score in regular_preds:
+            blended_scores[label] = score * regular_weight
+        for label, score in strategic_preds:
+            blended_scores[label] = blended_scores.get(label, 0) + score * strategic_weight
+        blended_predictions = sorted(blended_scores.items(), key=lambda x: x[1], reverse=True)
+        total = sum(score for _, score in blended_predictions)
+        if total > 0:
+            blended_predictions = [(label, score / total) for label, score in blended_predictions]
+        return blended_predictions[:k]
+
+    def predict_strategic(self, text: str, k: int = 5, emb: Optional[torch.Tensor] = None) -> List[Tuple[str, float]]:
+        """classifier.py:1649-1694: predict on the best response of the text's embedding."""
+        if not self.strategic_mode:
+            return self._predict_regular(text, k, emb)
+        if emb is None:
+            emb = self._embed_device([text])
+        if not self._coefficients_usable("Strategic"):
+            return self._predict_regular(text, k, emb)
+        return self._predict_from_embedding(self._best_response(emb), k, strategic=True)
+
+    def predict_robust(self, text: str, k: int = 5) -> List[Tuple[str, float]]:
+        """classifier.py:1696-1721: prototype-heavy blend (0.8 / 0.2) on the unmodified embedding."""
+        if not self.strategic_mode:
+            return self._predict_regular(text, k)
+        emb = self._embed_device([text])
+        if not self._coefficients_usable("Robust"):
+            return self._predict_regular(text, k, emb)
+        return self._predict_from_embedding(emb, k, robust=True)
+
+    def _predict_from_embedding(self, embedding: torch.Tensor, k: int = 5, robust: bool = False,
+                                strategic: bool = False) -> List[Tuple[str, float]]:
+        """classifier.py:1723-1795: k nearest prototypes (softmax over the k returned), head softmax top min(k, C), fixed
+        weights of the mode, renormalise, top k.  embedding: [1, D] on the device."""
+        proto_preds = self.memory.get_nearest_prototypes(embedding, k=k)
+        head_preds = []
+        probs = self._head_probs(embedding)
+        if probs is not None:
+            values, indices = _cabi.topk_desc(probs[:1], min(k, len(self.id_to_label)))
+            values, indices = values[0].cpu().tolist(), indices[0].cpu().tolist()
+            head_preds = [(self.id_to_label[i], v) for v, i in zip(values, indices)]
+        combined_scores = {}
+        if self.strategic_mode and robust:
+            proto_weight = self.config.strategic_robust_proto_weight
+            head_weight = self.config.strategic_robust_head_weight
+        elif self.strategic_mode and strategic:
+            proto_weight = self.config.strategic_prediction_proto_weight
+            head_weight = self.config.strategic_prediction_head_weight
+        else:
+            proto_weight = self.config.prototype_weight
+            head_weight = self.config.neural_weight
+        for label, score in proto_preds:
+            combined_scores[label] = score * proto_weight
+        for label, score in head_preds:
+            combined_scores[label] = combined_scores.get(label, 0) + score * head_weight
+        predictions = sorted(combined_scores.items(), key=lambda x: x[1], reverse=True)
+        total = sum(score for _, score in predictions)
+        if total > 0:
+            predictions = [(label, score / total) for label, score in predictions]
+        return predictions[:k]
+
+    def evaluate_strategic_robustness(self, test_texts: List[str], test_labels: List[str],
+                                      gaming_levels: List[float] = [0.0, 0.5, 1.0]) -> Dict[str, float]:
+        """classifier.py:1797-1823."""
+        if not self.strategic_mode:
+            raise ValueError("Strategic mode not enabled")
+        test_embeddings = self._embed_device(test_texts)
+        test_label_indices = torch.tensor([self.label_to_id[label] for label in test_labels])
+        with self._device_lock:
+            self.adaptive_head.eval()
+            return self.strategic_evaluator.evaluate_robustness(self.adaptive_head, test_embeddings, test_label_indices,
+                                                                gaming_levels)
 
     def predict_batch(self, texts: List[str], k: int = 5, batch_size: int = 32) -> List[List[Tuple[str, float]]]:
         """classifier.py:1308-1388: top-k prototype search (softmax over the k returned), head top-k, fixed

@@ -394,7 +394,11 @@ static int launch_training(const TrainCall &c, void *workspace, size_t workspace
         a.dropout_p = cfg->dropout_p; a.seed = cfg->seed; a.mask0 = cfg->mask0; a.mask1 = cfg->mask1;
         if (cfg->dropout_p > 0.f && cfg->mask0 && cfg->mask1) a.dropout_p = cfg->dropout_p;      // injected masks carry their own scale
         a.use_ewc = ewc ? 1 : 0; a.ewc_lambda = cfg->ewc_lambda;
+        a.n_regular = cfg->n_regular; a.strategic_lambda = cfg->strategic_lambda;
     }
+    if (c.loss_kind == AC_LOSS_CE_STRATEGIC)
+        AC_REQUIRE(cfg && c.n_steps == 1 && cfg->n_regular >= 1 && c.n == 2 * cfg->n_regular,
+                   "%s: AC_LOSS_CE_STRATEGIC steps one batch of 2 * n_regular rows (n=%d, n_regular=%d)", who, c.n, cfg ? cfg->n_regular : 0);
     a.loss_kind = c.loss_kind;
     a.fisher_scale = c.fisher_scale;
     a.h0d = reinterpret_cast<float *>(w + pl.off_h0d); a.h1d = reinterpret_cast<float *>(w + pl.off_h1d);
@@ -409,15 +413,17 @@ static int launch_training(const TrainCall &c, void *workspace, size_t workspace
     if (g_head_timing_dev) {               // diagnostic: per-phase nanoseconds of CTA 0 (ac_head_phase_timing)
         a.timing = g_head_timing_dev;
     }
-    static bool attr_set[64] = {};
+    const bool strat = c.loss_kind == AC_LOSS_CE_STRATEGIC;
+    const void *kern = strat ? reinterpret_cast<const void *>(ht::head_train_kernel<true>) : reinterpret_cast<const void *>(ht::head_train_kernel<false>);
+    static bool attr_set[2][64] = {};
     int dev = 0;
     AC_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        AC_CUDA(cudaFuncSetAttribute(ht::head_train_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
+    if (dev < 0 || dev >= 64 || !attr_set[strat][dev]) {
+        AC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+        if (dev >= 0 && dev < 64) attr_set[strat][dev] = true;
     }
     void *args[] = {&a};
-    AC_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(ht::head_train_kernel), dim3(pl.G), dim3(ht::HT_THREADS), args,
+    AC_CUDA(cudaLaunchCooperativeKernel(kern, dim3(pl.G), dim3(ht::HT_THREADS), args,
                                         pl.smem_bytes, s));
     count_launch();
     return AC_OK;
@@ -526,6 +532,91 @@ extern "C" int ac_head_grad(const float *X, const void *targets, int B, const ac
     float *stats = nullptr;
     if ((rc = launch_training(c, workspace, workspace_bytes, s, "ac_head_grad", &stats))) return rc;
     AC_CUDA(cudaMemcpyAsync(out_loss, stats, sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return AC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// strategic training (classifier.py:1602-1647, strategic.py:200-242): per step gather the batch, search its best responses in
+// train mode (strategic.cu), one optimizer step on [x ; br]
+// ------------------------------------------------------------------------------------------------
+constexpr int ST_MAX_BATCH = 16;       // DataLoader(batch_size=min(16, N)) of the reference
+
+// rows [0, Bt) of Xa / ta: the batch's rows and targets through the permutation; targets [Bt, 2 Bt) repeat them
+__global__ void strategic_gather_kernel(const float *__restrict__ X, const int64_t *__restrict__ targets, const int64_t *__restrict__ perm,
+                                        int Bt, int D, float *__restrict__ Xa, int64_t *__restrict__ ta) {
+    const int r = blockIdx.x;
+    const int64_t src = perm[r];
+    for (int k = threadIdx.x; k < D; k += blockDim.x) Xa[static_cast<int64_t>(r) * D + k] = X[src * D + k];
+    if (threadIdx.x == 0) { ta[r] = targets[src]; ta[Bt + r] = targets[src]; }
+}
+
+struct StLayout { size_t xa, ta, choice, util, train, search, total; };
+static int st_layout(int n, const ac_head_params *p, StLayout &l, const char *who) {
+    const int batch = n < ST_MAX_BATCH ? n : ST_MAX_BATCH;
+    TrainPlan pl;
+    int rc = plan_training(2 * batch, p, 1, true, pl, who);
+    if (rc) return rc;
+    size_t search = 0;
+    if ((rc = ac_strategic_workspace_bytes(batch, p, &search))) return rc;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+    l.xa = take(sizeof(float) * 2 * batch * p->D);
+    l.ta = take(sizeof(int64_t) * 2 * batch);
+    l.choice = take(sizeof(int32_t) * batch);
+    l.util = take(sizeof(float) * batch);
+    l.train = take(pl.total + 512);
+    l.search = take(search);
+    l.total = off + 256;
+    return AC_OK;
+}
+
+extern "C" int ac_head_train_strategic_workspace_bytes(int n, const ac_head_params *p, size_t *bytes) {
+    int rc = check_params(p, "ac_head_train_strategic_workspace_bytes");
+    if (rc) return rc;
+    AC_REQUIRE(bytes && n > 0, "ac_head_train_strategic_workspace_bytes: bad arguments");
+    StLayout l;
+    if ((rc = st_layout(n, p, l, "ac_head_train_strategic_workspace_bytes"))) return rc;
+    *bytes = l.total;
+    return AC_OK;
+}
+
+extern "C" int ac_head_train_strategic(const float *X, const int64_t *targets, const int64_t *perms, int n, int n_epochs, ac_head_params *p,
+                                       ac_head_params *m, ac_head_params *v, const ac_train_cfg *cfg, const ac_strategic_cfg *scfg,
+                                       float *step_stats, void *workspace, size_t workspace_bytes, ac_stream_t stream) {
+    const char *who = "ac_head_train_strategic";
+    int rc = check_params(p, who);
+    if (rc) return rc;
+    AC_REQUIRE(X && targets && perms && n > 0 && n_epochs >= 0 && m && v && cfg && scfg && step_stats && workspace, "%s: bad arguments", who);
+    AC_REQUIRE(cfg->step >= 1 && !cfg->mask0 && !cfg->mask1 && !cfg->ewc_fisher, "%s: step >= 1, no injected masks, no EWC", who);
+    StLayout l;
+    if ((rc = st_layout(n, p, l, who))) return rc;
+    uint8_t *w = reinterpret_cast<uint8_t *>(align_up(reinterpret_cast<uintptr_t>(workspace), 256));
+    if (l.total + (w - static_cast<uint8_t *>(workspace)) > workspace_bytes) { set_error("%s: workspace needs %zu bytes", who, l.total); return AC_E_WORKSPACE; }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    float *Xa = reinterpret_cast<float *>(w + l.xa);
+    int64_t *ta = reinterpret_cast<int64_t *>(w + l.ta);
+    const int batch = n < ST_MAX_BATCH ? n : ST_MAX_BATCH;
+    const int steps_per_epoch = (n + batch - 1) / batch;
+    ac_train_cfg tc = *cfg;
+    ac_strategic_cfg sc = *scfg;
+    for (int e = 0; e < n_epochs; ++e) {
+        for (int t = 0; t < steps_per_epoch; ++t) {
+            const int off = t * batch;
+            const int Bt = n - off < batch ? n - off : batch;
+            const int gstep = e * steps_per_epoch + t;
+            strategic_gather_kernel<<<Bt, 128, 0, s>>>(X, targets, perms + static_cast<int64_t>(e) * n + off, Bt, p->D, Xa, ta);
+            AC_LAUNCH_CHECK();
+            sc.step = cfg->step + gstep;
+            if ((rc = ac_strategic_best_response(Xa, Bt, p, &sc, reinterpret_cast<int32_t *>(w + l.choice), reinterpret_cast<float *>(w + l.util),
+                                                 Xa + static_cast<int64_t>(Bt) * p->D, w + l.search, l.total - l.search, stream)))
+                return rc;
+            tc.step = cfg->step + gstep;
+            tc.n_regular = Bt;
+            TrainCall c{Xa, ta, nullptr, 2 * Bt, 2 * Bt, 1, tc.step, p, m, v, &tc, AC_LOSS_CE_STRATEGIC, nullptr, nullptr, 0.f,
+                        step_stats + 3 * static_cast<int64_t>(gstep), nullptr};
+            if ((rc = launch_training(c, w + l.train, l.search - l.train, s, who, nullptr))) return rc;
+        }
+    }
     return AC_OK;
 }
 

@@ -82,7 +82,7 @@ struct Args {
     int n, batch, n_steps, first_step;
     Layer L[3];
     float lr, beta1, beta2, eps, wd, max_norm, dropout_p;
-    int loss_kind;                // 0 CE, 1 BCE
+    int loss_kind;                // 0 CE, 1 BCE, 2 CE_STRATEGIC
     unsigned long long seed;
     const float *mask0, *mask1;   // injected dropout masks [B,H0], [B,H1] (single step) or NULL
     int use_ewc;
@@ -99,6 +99,10 @@ struct Args {
     int res_mv;                   // AdamW moments of the own rows stay in shared memory for the whole launch
     int nst;                      // stages of the streamed-operand ring (2..8)
     unsigned long long *timing;   // nullable, [3][HT_TROW]: nanoseconds per phase of three observed CTAs (one per layer), summed over the steps
+    // CE_STRATEGIC: rows [0, n_regular) are x, rows [n_regular, 2 n_regular) their best responses.  Row weights: 1 / n_regular for x,
+    // strategic_lambda / n_regular for a best response whose first argmax differs from its target, 0 otherwise
+    int n_regular;
+    float strategic_lambda;
 };
 
 // ownership for a grid of G CTAs (host and emulator call this before ht_smem_layout)
@@ -491,6 +495,8 @@ __device__ __forceinline__ void ht_adamw_block(float *th, const float *g, float 
 // ---------------------------------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------------------------------
+// STRAT: the AC_LOSS_CE_STRATEGIC instantiation (row weights of P3b); the other loss kinds run head_train_kernel<false>
+template <bool STRAT = false>
 __global__ void __launch_bounds__(HT_THREADS, 1) head_train_kernel(const Args a) {
 #if !defined(AC_CPU_SHIM)
     extern __shared__ __align__(16) float ht_smem[];
@@ -596,7 +602,7 @@ __global__ void __launch_bounds__(HT_THREADS, 1) head_train_kernel(const Args a)
         for (int b = cta + G * warp; b < Bt; b += G * HT_KPARTS) {
             const float *zr = a.z + static_cast<int64_t>(b) * C;
             float *dr = a.dz + static_cast<int64_t>(b) * ldz;
-            if (a.loss_kind == 0) {
+            if (STRAT || a.loss_kind == 0) {
                 const int64_t y = static_cast<const int64_t *>(a.targets)[ridx[b]];
                 // the first 128 logits of the row are fetched once (one L2 round trip), wider rows re-read the tail
                 float zc[4];
@@ -612,7 +618,30 @@ __global__ void __launch_bounds__(HT_THREADS, 1) head_train_kernel(const Args a)
                 for (int j = lane + 128; j < C; j += 32) sum += expf(HT_LDCG(zr + j) - mx);
                 for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
                 const float lse = mx + logf(sum);
-                const float invB = 1.f / static_cast<float>(Bt);
+                float invB = 1.f / static_cast<float>(Bt);          // the row's weight in the batch loss
+                if (STRAT) {
+                    const float invR = 1.f / static_cast<float>(a.n_regular);
+                    invB = invR;
+                    if (b >= a.n_regular) {
+                        // first argmax of the row's logits (the same dropout masks as its loss): lanes scan their columns in
+                        // ascending order, the shuffle tree keeps the smaller column on equal values
+                        float bv = zc[0];
+                        int bi = lane;
+#pragma unroll
+                        for (int u = 1; u < 4; ++u)
+                            if (lane + 32 * u < C && zc[u] > bv) { bv = zc[u]; bi = lane + 32 * u; }
+                        for (int j = lane + 128; j < C; j += 32) {
+                            const float zv = HT_LDCG(zr + j);
+                            if (zv > bv) { bv = zv; bi = j; }
+                        }
+                        for (int o = 16; o > 0; o >>= 1) {
+                            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+                            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+                        }
+                        invB = (bi != y) ? a.strategic_lambda * invR : 0.f;
+                    }
+                }
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     const int j = lane + 32 * u;
@@ -627,7 +656,7 @@ __global__ void __launch_bounds__(HT_THREADS, 1) head_train_kernel(const Args a)
                         dr[j] = 0.f;
                     }
                 }
-                if (lane == 0) a.rowloss[b] = (y >= 0 && y < C) ? (lse - zy) : 0.f;
+                if (lane == 0) a.rowloss[b] = (y >= 0 && y < C) ? (STRAT ? invB * (lse - zy) : (lse - zy)) : 0.f;
             } else {
                 const float *yr = static_cast<const float *>(a.targets) + ridx[b] * C;
                 const float inv = 1.f / (static_cast<float>(Bt) * static_cast<float>(C));
@@ -841,7 +870,7 @@ __global__ void __launch_bounds__(HT_THREADS, 1) head_train_kernel(const Args a)
             for (int b = 0; b < 32; ++b) ls += __shfl_sync(0xffffffffu, r0, b);
             for (int b = 0; b < 32; ++b) ls += __shfl_sync(0xffffffffu, r1, b);
             if (tid == 0) {
-                const float loss = ls / static_cast<float>(Bt);
+                const float loss = STRAT ? ls : ls / static_cast<float>(Bt);     // CE_STRATEGIC rows carry their weights
                 const float penalty = a.use_ewc ? a.ewc_lambda / static_cast<float>(Bt) * pt : 0.f;
                 if (a.stats) { a.stats[3 * t + 0] = loss; a.stats[3 * t + 1] = penalty; a.stats[3 * t + 2] = scal[3]; }
                 if (a.loss_accum) a.loss_accum[0] += loss + penalty;

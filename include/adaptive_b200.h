@@ -121,7 +121,7 @@ int ac_memory_append_prune(float *rows, int32_t *order, int32_t *count, int cap,
  * Weights in nn.Linear layout: W0[H0,D], W1[H1,H0], W2[C,H1]  (H0 = D, H1 = D/2 in the reference).
  * ------------------------------------------------------------------------------------------ */
 enum { AC_ACT_LOGITS = 0, AC_ACT_SOFTMAX = 1, AC_ACT_SIGMOID = 2 };
-enum { AC_LOSS_CE = 0, AC_LOSS_BCE = 1 };
+enum { AC_LOSS_CE = 0, AC_LOSS_BCE = 1, AC_LOSS_CE_STRATEGIC = 2 };
 
 typedef struct {
     int D, H0, H1, C;
@@ -146,6 +146,10 @@ typedef struct {
     const ac_head_params *ewc_star;
     float ewc_lambda;
     int ewc_C_old;
+    /* AC_LOSS_CE_STRATEGIC only (0 otherwise): the batch is [x_1..x_n ; br_1..br_n] with n = n_regular, and the step minimises
+       mean CE(x) + strategic_lambda / n * sum over the best-response rows whose first-argmax differs from y of CE(br) */
+    int n_regular;
+    float strategic_lambda;
 } ac_train_cfg;
 
 /* bytes of workspace for a training / gradient call with `batch` rows per step and n_steps steps (1 for a single step) */
@@ -190,6 +194,51 @@ int ac_head_grad(const float *X, const void *targets, int B, const ac_head_param
  * output layer) */
 int ac_ewc_penalty(const ac_head_params *p, const ac_head_params *fisher, const ac_head_params *star,
                    float lambda, float inv_batch, int C_old, float *out, ac_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Stage S -- strategic mode.  Replaces the per-sample Python loops of
+ *   strategic.py:74-123   SeparableCostFunction.compute_best_response / _generate_candidates (50 head forwards per sample)
+ *   strategic.py:200-242  StrategicOptimizer.strategic_loss
+ *   classifier.py:1602-1647 AdaptiveClassifier._strategic_training_step
+ * The candidate set of a row x (D >= 5) is fixed: candidate 0 is x, candidate 1 + 10 i + j (i = 0..3, j = 0..9) and
+ * 41 + j (i = 4, j = 0..8) is x with x_i replaced by fl(x_i + delta[j]), delta = torch.linspace(-2, 2, 10).  The utility of a
+ * candidate y is max softmax(head(y)) - cost(x, y); the first maximum wins (NaN never does; no winner -> candidate 0).
+ *   AC_COST_LINEAR     relu(c1 . (y - x)) = relu(fl(c1_i * fl(y_i - x_i)))       (LinearCostFunction, bit-exact)
+ *   AC_COST_SEPARABLE  relu(c2 . y - c1 . x), both dots in one fixed order       (SeparableCostFunction)
+ * ------------------------------------------------------------------------------------------ */
+enum { AC_COST_LINEAR = 0, AC_COST_SEPARABLE = 1 };
+#define AC_STRATEGIC_CANDIDATES 50
+
+typedef struct {
+    int cost_kind;           /* AC_COST_* */
+    const float *c1;         /* [D] device: alpha (linear) or c1 (separable) */
+    const float *c2;         /* [D] device: c2 (separable; ignored for linear) */
+    float delta[10];         /* torch.linspace(-2, 2, 10) in fp32, built on the host */
+    float dropout_p;         /* train-mode candidate forwards (0 = eval mode) */
+    uint64_t seed;           /* dropout key: (seed, step, row, candidate), a stream apart from the training kernel's masks */
+    int step;
+} ac_strategic_cfg;
+
+/* bytes of workspace for ac_strategic_best_response on B rows */
+int ac_strategic_workspace_bytes(int B, const ac_head_params *p, size_t *bytes);
+
+/* best response of every row of X[B,D] against the head p: out_choice[B] (candidate index 0..49), out_utility[B] (its utility),
+ * out_Y[B,D] (nullable: the chosen candidate, bit for bit).  D >= 5; D, H0, H1 multiples of 4. */
+int ac_strategic_best_response(const float *X, int B, const ac_head_params *p, const ac_strategic_cfg *cfg, int32_t *out_choice,
+                               float *out_utility, float *out_Y, void *workspace, size_t workspace_bytes, ac_stream_t stream);
+
+/* bytes of workspace for ac_head_train_strategic on n stored rows */
+int ac_head_train_strategic_workspace_bytes(int n, const ac_head_params *p, size_t *bytes);
+
+/* the whole _strategic_training_step on the device with no host synchronisation: for each of n_epochs epochs, batches of
+ * min(16, n) rows of X[n,D] / targets int64[n] are taken in the order perms[epoch * n ..] (what the reference's DataLoader with
+ * torch.Generator().manual_seed(42) yields), their best responses are searched in train mode (scfg->dropout_p, seed, step),
+ * and one AdamW step runs on the 2B rows [x ; br] with AC_LOSS_CE_STRATEGIC (cfg->strategic_lambda; cfg->step = first step,
+ * cfg->loss_kind and cfg->n_regular are ignored).  step_stats[n_steps, 3] (device) = (strategic loss, 0, grad norm before
+ * clipping) of every step. */
+int ac_head_train_strategic(const float *X, const int64_t *targets, const int64_t *perms, int n, int n_epochs, ac_head_params *p,
+                            ac_head_params *m, ac_head_params *v, const ac_train_cfg *cfg, const ac_strategic_cfg *scfg,
+                            float *step_stats, void *workspace, size_t workspace_bytes, ac_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Stage E -- encoder.  Replaces `self.model(**inputs).last_hidden_state[:,0,:]` + F.normalize at
