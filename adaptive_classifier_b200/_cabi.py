@@ -551,6 +551,17 @@ def distilbert_to_bert_state_dict(sd: dict, c):
     return out, dims
 
 
+def check_head_dim(hidden: int, heads: int, what: str = "encoder") -> None:
+    """The attention kernels of the BERT-family encoder take head_dim = hidden / heads of 64 (bert-base, RoBERTa, DistilBERT)
+    or 32 (all-MiniLM, BGE-small, E5-small, GTE-small); raises AdaptiveB200Error naming anything else (no device call)."""
+    if heads <= 0 or hidden % heads != 0:
+        raise AdaptiveB200Error(f"{what} hidden={hidden} is not divisible by heads={heads}: head_dim must be 64 or 32")
+    head_dim = hidden // heads
+    if head_dim not in (64, 32):
+        raise AdaptiveB200Error(f"{what} head_dim={head_dim} (hidden={hidden}, heads={heads}): only head_dim 64 and 32 are "
+                                "implemented")
+
+
 def modernbert_rope_table(theta: float, n_pos: int = AC_ENCODER_MAX_S, head_dim: int = 64) -> torch.Tensor:
     """[n_pos, head_dim] fp32 table the encoder's RoPE epilogue reads: row p = cos | sin of the head_dim / 2 frequencies at
     position p, computed with HF ModernBertRotaryEmbedding's own formula (default rope type, attention scaling 1)."""
@@ -657,21 +668,23 @@ class Encoder:
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
         """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel (post-LN blocks) or ModernBertModel (pre-LN,
-        RoPE, GeGLU, sliding-window layers); head_dim 64."""
+        RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for the post-LN family, 64 for ModernBERT."""
         c = model.config
         mt = getattr(c, "model_type", "bert")
         if mt == "modernbert":
             dims = modernbert_settings(c)
             return cls(dict(model.state_dict()), arch="modernbert", max_tokens=max_tokens, device=device, cls_only=cls_only,
                        **dims)
-        sd = {k: v for k, v in model.state_dict().items()}
         if mt == "distilbert":
-            sd, dims = distilbert_to_bert_state_dict(sd, c)
+            check_head_dim(c.dim, c.n_heads, "DistilBERT")
+            sd, dims = distilbert_to_bert_state_dict(dict(model.state_dict()), c)
             return cls(sd, arch="bert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
         if mt not in ("bert", "roberta", "xlm-roberta"):
             raise AdaptiveB200Error(f"encoder architecture '{mt}' is not implemented in the CUDA path yet")
         if getattr(c, "hidden_act", "gelu") != "gelu" or getattr(c, "position_embedding_type", "absolute") != "absolute":
             raise AdaptiveB200Error("only exact-erf GELU and absolute position embeddings are implemented")
+        check_head_dim(c.hidden_size, c.num_attention_heads, mt)
+        sd = {k: v for k, v in model.state_dict().items()}
         return cls(sd, arch="bert" if mt == "bert" else "roberta", layers=c.num_hidden_layers, hidden=c.hidden_size,
                    heads=c.num_attention_heads, intermediate=c.intermediate_size, vocab=c.vocab_size,
                    max_pos=c.max_position_embeddings, type_vocab=c.type_vocab_size, ln_eps=c.layer_norm_eps,

@@ -206,6 +206,19 @@ __device__ __forceinline__ void wgmma_m64n64_f16(float (&d)[32], uint64_t a_desc
           "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
+__device__ __forceinline__ void wgmma_m64n32_f16(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
 
 // Accumulator fragment of an m64nN wgmma -> rows of a row-major fp32 tile (ld floats per row).  Thread t of the warpgroup
 // holds, for every 8-column group j, rows 16 (t/32) + (t%32)/4 (+8) and columns 8 j + 2 (t%4) (+1).

@@ -13,7 +13,7 @@
 //   projections   wgmma GEMM of gemm_tc.cuh (.f16) with compile-time-specialised fused epilogues:
 //                 bias | bias+GELU(erf) | bias+residual, fp16 or fp32 output, V written TRANSPOSED per (sequence, head)
 //   attention     one CTA per (sequence, head): Q, K and V^T tiles by TMA, QK^T and PV as wgmma with the score tile
-//                 staged in shared memory, thread-per-query-row softmax in between (S <= 128, head_dim 64)
+//                 staged in shared memory, thread-per-query-row softmax in between (S <= 128; head_dim 64 or 32)
 //   LayerNorm     never materialised inside the layer stack: the residual epilogues keep the un-normalised sums y (fp32) and
 //                 per-row (sum, sumsq) partials, the consuming projections run on gamma-scaled weights and apply the
 //                 rank-1 correction r (acc - mu c1) + c0 in their epilogue ("deferred LayerNorm" below)
@@ -578,14 +578,19 @@ __global__ void to_half_kernel(const float *__restrict__ in, __half *__restrict_
 }
 
 // ------------------------------------------------------------------------------------------------
-// attention: one CTA (128 threads = one warpgroup) per (sequence b, head h); S <= 128, head_dim == 64, fp16 operands.
-//   scores[128x128] = Q K^T        2 x 4 wgmma m64n128k16 (query rows 0-63, 64-127), fp32 fragments -> smem score tile
+// attention: one CTA (128 threads = one warpgroup) per (sequence b, head h); S <= 128, head_dim DH (64 or 32), fp16 operands.
+//   scores[128x128] = Q K^T        2 x DH/16 wgmma m64n128k16 (query rows 0-63, 64-127), fp32 fragments -> smem score tile
 //   P = exp(scale*(s - max)) masked  thread = query row, reads its score row; P held in registers, then -> smem (swizzled fp16)
-//   out[128x64] = P V              2 x 8 wgmma m64n64k16, fragments -> smem
-//   ctx[row, h*64 + :] = out / rowsum  (fp16: the A operand of the output projection)
+//   out[128xDH] = P V              2 x 8 wgmma m64nDHk16, fragments -> smem
+//   ctx[row, h*DH + :] = out / rowsum  (fp16: the A operand of the output projection)
 // smem: one 68 KB region that holds, in turn, the Q and K tiles (16 KB each, TMA, 128B swizzle), the fp32 score tile, P
 // (2 slabs x 16 KB) and the output tile; then V^T (2 slabs x 8 KB by TMA from the transposed buffer the QKV epilogue wrote).
 // 85 KB per CTA: two CTAs share an SM, so one CTA's softmax overlaps the other's loads and MMAs.
+// DH = 32 (MiniLM, BGE-small, E5-small: hidden 384 = 12 x 32) keeps every layout and descriptor of DH = 64.  The Q and K
+// boxes still span 64 halves but start at column h*32, so they hold this head and its neighbour (TMA zero-fills past 2H for
+// the last head) and QK^T issues only k-steps 0-1.  The V^T box still spans 64 rows from row (b*heads + h)*32; PV reads
+// its first 32 rows (one 4 KB, 1 KB-aligned block of 8-row swizzle atoms per slab) as the N = 32 operand.  Attention is
+// ~5% of such an encoder's flops, so the unused half of each box costs less than a second descriptor type would add.
 // ------------------------------------------------------------------------------------------------
 constexpr int ATT_THREADS = 128;
 constexpr int ATT_S_LD = 128 + 4;                            // score tile row stride (floats): conflict-free row reads
@@ -596,6 +601,8 @@ static_assert(2 * (ATT_SMEM + 1024) <= 228 * 1024, "two attention CTAs must fit 
 
 // S[128 x 128] = Q K^T for the query tile sQ and key tile sK (both [128 rows x 128 B], 128B swizzle) -> sS (fp32, ld ATT_S_LD).
 // Issued by the whole warpgroup; returns once the products are in shared memory (the caller synchronises the CTA).
+// Only the first DH halves of every row are the head's: DH / 16 k-steps.
+template <int DH>
 __device__ __forceinline__ void att_scores(const uint8_t *sQ, const uint8_t *sK, float *sS) {
     const uint64_t bd = wgmma_desc_sw128(smem_u32(sK));
 #pragma unroll 1
@@ -604,14 +611,16 @@ __device__ __forceinline__ void att_scores(const uint8_t *sQ, const uint8_t *sK,
         const uint64_t a = wgmma_desc_sw128(smem_u32(sQ + half * 8192));
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(s, a + 2 * k, bd + 2 * k, k != 0);
+        for (int k = 0; k < DH / 16; ++k) wgmma_m64n128_f16(s, a + 2 * k, bd + 2 * k, k != 0);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_store_acc(s, sS + half * 64 * ATT_S_LD, ATT_S_LD);
     }
 }
-// O[128 x 64] (+)= P V with P = 2 slabs x [128 rows x 64 keys] and V^T = 2 slabs x [64 (d) x 64 keys] in shared memory
-__device__ __forceinline__ void att_pv(const uint8_t *sP, const uint8_t *sVt, float (&o)[2][32], bool accumulate) {
+// O[128 x DH] (+)= P V with P = 2 slabs x [128 rows x 64 keys] and V^T = 2 slabs x [64 (d) x 64 keys] in shared memory,
+// of which the first DH rows (d) are the head's
+template <int DH>
+__device__ __forceinline__ void att_pv(const uint8_t *sP, const uint8_t *sVt, float (&o)[2][DH / 2], bool accumulate) {
 #pragma unroll
     for (int half = 0; half < 2; ++half) {
         wgmma_fence();
@@ -620,7 +629,10 @@ __device__ __forceinline__ void att_pv(const uint8_t *sP, const uint8_t *sVt, fl
             const uint64_t a = wgmma_desc_sw128(smem_u32(sP + slab * 16384 + half * 8192));
             const uint64_t bd = wgmma_desc_sw128(smem_u32(sVt + slab * 8192));
 #pragma unroll
-            for (int k = 0; k < 4; ++k) wgmma_m64n64_f16(o[half], a + 2 * k, bd + 2 * k, accumulate || (slab | k) != 0);
+            for (int k = 0; k < 4; ++k) {
+                if constexpr (DH == 64) wgmma_m64n64_f16(o[half], a + 2 * k, bd + 2 * k, accumulate || (slab | k) != 0);
+                else wgmma_m64n32_f16(o[half], a + 2 * k, bd + 2 * k, accumulate || (slab | k) != 0);
+            }
         }
     }
     wgmma_commit();
@@ -637,10 +649,11 @@ __device__ __forceinline__ void att_store_p(uint32_t sp_base, int qrow, int c, c
                      : "memory");
     }
 }
-// ctx[dst row, 0..63] = fp16(out row * inv), out row read from the smem tile
+// ctx[dst row, 0..DH-1] = fp16(out row * inv), out row read from the smem tile
+template <int DH>
 __device__ __forceinline__ void att_write_row(const float *orow, float inv, __half *dst) {
 #pragma unroll
-    for (int c = 0; c < 64; c += 8) {
+    for (int c = 0; c < DH; c += 8) {
         const float4 a = *reinterpret_cast<const float4 *>(orow + c);
         const float4 b = *reinterpret_cast<const float4 *>(orow + c + 4);
         __half2 h0 = __floats2half2_rn(a.x * inv, a.y * inv), h1 = __floats2half2_rn(a.z * inv, a.w * inv);
@@ -663,6 +676,7 @@ __device__ __forceinline__ uint32_t band_bits(int q, int k0, int w) {
 }
 
 // window: ModernBERT sliding_attention half-window (keys |q - key| <= window), 0 = full attention
+template <int DH>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
                  const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
@@ -689,9 +703,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     if (tid == 0) {
         mbar_arrive_expect_tx(bar_load, 48 * 1024);
         const int r = static_cast<int>(row0);
-        tma_load_2d(sQ, &tmap_qk, bar_load, h * 64, r);
-        tma_load_2d(sK, &tmap_qk, bar_load, H + h * 64, r);
-        const int vrow = (b * heads + h) * 64;                 // rows (b, h, d) of the transposed V buffer
+        tma_load_2d(sQ, &tmap_qk, bar_load, h * DH, r);
+        tma_load_2d(sK, &tmap_qk, bar_load, H + h * DH, r);
+        const int vrow = (b * heads + h) * DH;                 // rows (b, h, d) of the transposed V buffer
         tma_load_2d(sVt, &tmap_vt, bar_load, 0, vrow);
         tma_load_2d(sVt + 8 * 1024, &tmap_vt, bar_load, 64, vrow);
     }
@@ -703,9 +717,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
         const uint64_t a0 = wgmma_desc_sw128(smem_u32(sQ)), a1 = wgmma_desc_sw128(smem_u32(sQ + 8192));
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(s0, a0 + 2 * k, bd + 2 * k, k != 0);
+        for (int k = 0; k < DH / 16; ++k) wgmma_m64n128_f16(s0, a0 + 2 * k, bd + 2 * k, k != 0);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(s1, a1 + 2 * k, bd + 2 * k, k != 0);
+        for (int k = 0; k < DH / 16; ++k) wgmma_m64n128_f16(s1, a1 + 2 * k, bd + 2 * k, k != 0);
         wgmma_commit();
         wgmma_wait<0>();
         __syncthreads();
@@ -726,7 +740,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
         const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
         kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(qrow, 32 * w4, window);
     }
-    const float scale_log2 = rsqrtf(64.f) * 1.44269504088896340736f;
+    const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
     float mx = -CUDART_INF_F;
 #pragma unroll 1
     for (int c = 0; c < 128; c += 32) {
@@ -763,14 +777,14 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     __syncthreads();
 
     // ---- O = P V, staged over P once every warp's MMAs have read it
-    float o[2][32];
-    att_pv(sP, sVt, o, false);
+    float o[2][DH / 2];
+    att_pv<DH>(sP, sVt, o, false);
     __syncthreads();
     wgmma_store_acc(o[0], sS, ATT_S_LD);
     wgmma_store_acc(o[1], sS + 64 * ATT_S_LD, ATT_S_LD);
     __syncthreads();
     const float inv = (sum > 0.f) ? 1.f / sum : 0.f;
-    if (qrow < S) att_write_row(srow, inv, ctx + (row0 + qrow) * H + h * 64);
+    if (qrow < S) att_write_row<DH>(srow, inv, ctx + (row0 + qrow) * H + h * DH);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -783,6 +797,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
 // ------------------------------------------------------------------------------------------------
 constexpr int ATTL_SMEM = 80 * 1024 + ATT_S_BYTES + 1024 + 64;
 
+template <int DH>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
                       const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
@@ -800,7 +815,7 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
     const int qb = blockIdx.y;                                   // query block
     const int nkb = (S + 127) / 128;
     const int64_t row0 = static_cast<int64_t>(b) * S;
-    const int vrow = (b * heads + h) * 64;
+    const int vrow = (b * heads + h) * DH;
 
     if (tid == 0) {
         tma_prefetch_desc(&tmap_qk);
@@ -812,11 +827,11 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
     const int qrow = warp * 32 + lane;                            // row inside the query block
     const int qglob = qb * 128 + qrow;                            // position inside the sequence
     const float *srow = sS + qrow * ATT_S_LD;
-    const float scale_log2 = rsqrtf(64.f) * 1.44269504088896340736f;
+    const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
 
     uint32_t ph_load = 0;
     float mx = -CUDART_INF_F, sum = 0.f;
-    float o[2][32];
+    float o[2][DH / 2];
 
     for (int pass = 0; pass < 2; ++pass) {
         for (int j = 0; j < nkb; ++j) {
@@ -825,8 +840,8 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
                 const bool first = (pass == 0 && j == 0);
                 const uint32_t bytes = (first ? 16 * 1024 : 0) + 16 * 1024 + (pass == 1 ? 16 * 1024 : 0);
                 mbar_arrive_expect_tx(bar_load, bytes);
-                if (first) tma_load_2d(sQ, &tmap_qk, bar_load, h * 64, static_cast<int>(row0) + qb * 128);
-                tma_load_2d(sK, &tmap_qk, bar_load, H + h * 64, static_cast<int>(row0) + key0);
+                if (first) tma_load_2d(sQ, &tmap_qk, bar_load, h * DH, static_cast<int>(row0) + qb * 128);
+                tma_load_2d(sK, &tmap_qk, bar_load, H + h * DH, static_cast<int>(row0) + key0);
                 if (pass == 1) {
                     tma_load_2d(sVt, &tmap_vt, bar_load, key0, vrow);
                     tma_load_2d(sVt + 8 * 1024, &tmap_vt, bar_load, key0 + 64, vrow);
@@ -834,7 +849,7 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
             }
             mbar_wait_guarded(bar_load, ph_load);
             ph_load ^= 1;
-            att_scores(sQ, sK, sS);
+            att_scores<DH>(sQ, sK, sS);
             __syncthreads();
 
             // key validity bits of this block
@@ -878,7 +893,7 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
                 }
                 fence_proxy_async_smem();
                 __syncthreads();
-                att_pv(sP, sVt, o, j != 0);
+                att_pv<DH>(sP, sVt, o, j != 0);
                 __syncthreads();                                  // sK / sVt / sP / the score tile are free again
             }
         }
@@ -888,7 +903,7 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
     wgmma_store_acc(o[1], sS + 64 * ATT_S_LD, ATT_S_LD);
     __syncthreads();
     const float inv = (sum > 0.f) ? 1.f / sum : 0.f;
-    if (qglob < S) att_write_row(srow, inv, ctx + (row0 + qglob) * H + h * 64);
+    if (qglob < S) att_write_row<DH>(srow, inv, ctx + (row0 + qglob) * H + h * DH);
 }
 
 // last layer, deferred flow: CLS rows of the attention context and of LN_pending(y) (two-pass statistics from the fp32 sums)
@@ -961,27 +976,32 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
     return AC_OK;
 }
 
-// softmax(Q K^T / 8 + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention
+// softmax(Q K^T / sqrt(head_dim) + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention
 static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, cudaStream_t s) {
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden;
+    const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create)
     // per-device: the attribute is a property of the (function, device) pair
     static bool att_attr[64] = {};
     int dev = 0;
     AC_CUDA(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !att_attr[dev]) {
-        AC_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTL_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_long_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTL_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_long_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTL_SMEM));
         if (dev >= 0 && dev < 64) att_attr[dev] = true;
     }
     // algorithmic flops of softmax(QK^T)V at the true sequence length (the 128-wide tile does more)
-    const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * static_cast<double>(S) * S * 64, 0.0, s);
-    if (S <= 128)
-        attention_kernel<<<B * c.heads, ATT_THREADS, ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window,
-                                                                    e->ctx);
-    else
-        attention_long_kernel<<<dim3(B * c.heads, (S + 127) / 128), ATT_THREADS, ATTL_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S,
-                                                                                                c.heads, H, window, e->ctx);
+    const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * static_cast<double>(S) * S * dh, 0.0, s);
+    if (S <= 128) {
+        auto kern = dh == 32 ? attention_kernel<32> : attention_kernel<64>;
+        kern<<<B * c.heads, ATT_THREADS, ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx);
+    } else {
+        auto kern = dh == 32 ? attention_long_kernel<32> : attention_long_kernel<64>;
+        kern<<<dim3(B * c.heads, (S + 127) / 128), ATT_THREADS, ATTL_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H,
+                                                                               window, e->ctx);
+    }
     prof_end(slot, s);
     AC_LAUNCH_CHECK();
     return AC_OK;
@@ -1074,8 +1094,11 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
                "wqkv, wi, final_norm_w and attn_norm_w", AC_ENCODER_MAX_S);
     AC_REQUIRE(cfg->precision == AC_PREC_F16, "ac_encoder_create: only AC_PREC_F16 (fp16 operands, fp32 accumulate) is implemented");
     AC_REQUIRE(cfg->hidden % 128 == 0 && cfg->hidden <= 1024, "ac_encoder_create: hidden=%d must be a multiple of 128, <= 1024", cfg->hidden);
-    AC_REQUIRE(cfg->heads > 0 && cfg->hidden / cfg->heads == 64 && cfg->hidden % cfg->heads == 0,
-               "ac_encoder_create: head_dim must be 64 (hidden=%d heads=%d)", cfg->hidden, cfg->heads);
+    // the attention kernels take head_dim 64 or 32; ModernBERT's RoPE epilogue pairs (d, d + 32) inside a 64-column head
+    AC_REQUIRE(cfg->heads > 0 && cfg->hidden % cfg->heads == 0 &&
+                   (cfg->hidden / cfg->heads == 64 || (!mb && cfg->hidden / cfg->heads == 32)),
+               "ac_encoder_create: head_dim must be %s (hidden=%d heads=%d)", mb ? "64 for ModernBERT" : "64 or 32", cfg->hidden,
+               cfg->heads);
     AC_REQUIRE(cfg->intermediate % 64 == 0 && cfg->layers > 0 && cfg->max_tokens > 0, "ac_encoder_create: bad dims");
     int rc = ac_device_check();
     if (rc) return rc;
@@ -1292,7 +1315,8 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
                "ac_encoder_forward_cls: B=%d sequences of S=%d exceed the transposed-V workspace; split the batch", B, S);
     int rc;
     if (e->vt_B != B || e->vt_S != S) {
-        // V^T view of this call: rows (b, h, d), S_pad keys per row; box = 64 keys x 64 head dims
+        // V^T view of this call: rows (b, h, d), S_pad keys per row; box = 64 keys x 64 rows (one head of 64, or a head of
+        // 32 and its neighbour; rows past B*H read as zeros)
         if ((rc = make_tmap_2d(&e->m_vt_att, e->vT, 2, static_cast<uint64_t>(B) * H, S_pad, static_cast<uint64_t>(S_pad) * 2, 64, 64)))
             return rc;
         e->vt_B = B; e->vt_S = S;

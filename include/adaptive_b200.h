@@ -254,7 +254,8 @@ enum {
 
 typedef struct {
     int arch;            /* AC_ARCH_* */
-    int layers, hidden, heads, intermediate;
+    int layers, hidden, heads, intermediate;   /* hidden % 128 == 0; head_dim = hidden / heads is 64 or 32
+                                                  (64 only for AC_ARCH_MODERNBERT) */
     int vocab, max_pos, type_vocab;
     int pad_idx;         /* roberta: position ids start at pad_idx+1 */
     float ln_eps;
