@@ -3,7 +3,8 @@
 // Replaces `self.model(**inputs).last_hidden_state[:, 0, :]` + F.normalize at
 // /root/reference/src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel.forward:
 // embeddings modeling_bert.py:53-113, self-attention :143-207, output+LN :287-298, FFN :330-356;
-// HF ModernBertModel.forward in models/modernbert/modeling_modernbert.py: see forward_modernbert).
+// HF ModernBertModel.forward in models/modernbert/modeling_modernbert.py).  One layer loop (forward_layers) runs both
+// block kinds; they differ in the LayerNorm left pending on the residual path and in compile-time epilogue choices.
 //
 // Precision: every tensor-core operand is fp16 (RNE from fp32), accumulation fp32 (wgmma), residual stream, LayerNorm,
 // softmax and GELU in fp32.  fp16 carries the same 10-bit mantissa as tf32, so the measured error is the tf32 one
@@ -931,16 +932,31 @@ __global__ void gather_cls_ln_kernel(const __half *__restrict__ ctx, const float
 // ================================================================================================
 using namespace ac;
 
+// One encoder layer, fields by role; where BERT-family (post-LN) and ModernBERT (pre-LN) layers differ, the comment says so.
+struct Layer {
+    // fp16 GEMM operands with their GEMM_BLOCK_N-row-box maps: QKV [3H, H] and FFN1 (BERT W1 [I, H], ModernBERT Wi [2I, H]
+    // interleaved for GeGLU) consume un-normalised residual sums and are packed as fp16(gamma * W) by pack_consumer
+    __half *wqkv = nullptr, *wo = nullptr, *w1 = nullptr, *w2 = nullptr;
+    CUtensorMap m_wqkv, m_wo, m_w1, m_w2;
+    // rank-1 corrections of the deferred-LayerNorm consumers: c1 (row sums of the packed weight), c0 (W beta + bias)
+    float *c1qkv = nullptr, *c0qkv = nullptr, *c1f = nullptr, *c0f = nullptr;
+    float *bo = nullptr, *b2 = nullptr;   // residual biases of Wo / W2 (ModernBERT: zeros)
+    // LayerNorm FFN1 consumes: BERT attention.output.LayerNorm (left pending on the residual sums), ModernBERT mlp_norm
+    // (beta zeros; the residual sums stay raw)
+    float *ln_ffn_w = nullptr, *ln_ffn_b = nullptr;
+    // LayerNorm of the layer output: BERT output.LayerNorm (left pending on the residual sums), ModernBERT final_norm (beta
+    // zeros) in the last layer only (the next layer's attn_norm is folded into its Wqkv)
+    float *ln_out_w = nullptr, *ln_out_b = nullptr;
+    int window = 0;                       // sliding-attention half-window, 0 = full attention (always 0 for BERT)
+};
+
 struct ac_encoder {
     ac_encoder_config cfg;
-    // packed weights (device): fp16 GEMM operands, fp32 everything else
+    // packed weights (device): fp16 GEMM operands, fp32 everything else.  ModernBERT: no pos / type, emb_ln_b = zeros
     float *word = nullptr, *pos = nullptr, *type = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
-    // QKV / FFN1 consume un-normalised residual sums: their weights are packed as fp16(gamma * W) with the rank-1 correction
-    // vectors c1 (row sums of the packed weight) and c0 (W beta + bias), see pack_defer_kernel
-    std::vector<__half *> wqkv_d, wo, w1_d, w2;
-    std::vector<float *> c1qkv, c0qkv, c1f, c0f, bo, ln1w, ln1b, b2, ln2w, ln2b;
+    std::vector<Layer> layers;
     __half *w1_last = nullptr;            // plain fp16 FFN1 weight of the last layer (CLS-only tail runs on materialised LayerNorm rows)
-    float *b1_last = nullptr;
+    float *b1_last = nullptr;             // its bias (ModernBERT: zeros)
     // activations: fp32 residual sums x (+ tmp for a materialised final LayerNorm); fp16 GEMM operands xh, qk, vT, ctx, ffn
     float *x = nullptr, *tmp = nullptr;
     __half *xh = nullptr, *qk = nullptr, *vT = nullptr, *ctx = nullptr, *ffn = nullptr;
@@ -954,19 +970,14 @@ struct ac_encoder {
     // cached TMA descriptors: A operands (128-row boxes) and weights (128-row boxes = the B half one CTA of a pair stages)
     CUtensorMap m_xh, m_ctx, m_ffn, m_qk_att, m_vt_att;
     int vt_B = -1, vt_S = -1;
-    std::vector<CUtensorMap> p_wqkv_d, p_wo, p_w1_d, p_w2;
     CUtensorMap p_w1_last;
     // row statistics (ping-pong) and the per-GEMM_EPI_COLS-column partials the residual epilogues write
     float2 *stats_a = nullptr, *stats_b = nullptr, *stats_id = nullptr, *parts = nullptr;
     float *ones = nullptr, *zeros = nullptr;   // ones [H]; zeros [max(3H, 2I)]: beta / bias of the bias-free ModernBERT
-    // ModernBERT: per-layer half-window (0 = full attention), RoPE tables [AC_ENCODER_MAX_S, 64] (full, sliding), final_norm.
-    // Wqkv packs into wqkv_d / c1qkv / c0qkv, Wi (interleaved, 2I rows) into w1_d / c1f / c0f, mlp_norm into ln1w.
-    std::vector<int> window;
-    float *rope[2] = {nullptr, nullptr}, *final_norm = nullptr;
+    float *rope[2] = {nullptr, nullptr};       // ModernBERT RoPE tables [AC_ENCODER_MAX_S, 64] (full, sliding layers)
     std::vector<void *> allocs;
-    int last_B = 0, last_S = 0;
+    int last_B = 0, last_S = 0;           // shape of the previous forward; its full hidden state (cls_only = 0) is in tmp
     bool last_cls_only = false;
-    const float *last_hidden = nullptr;   // where the previous full forward left the last hidden state
 };
 
 static int launch_cls_normalize(const float *x, int B, int S, int H, float *out, cudaStream_t s) {
@@ -1038,50 +1049,21 @@ extern "C" int ac_encoder_destroy(ac_encoder *enc) {
     return AC_OK;
 }
 
-// ModernBERT weights (modeling_modernbert.py).  Wqkv consumes the un-normalised residual sums pending attn_norm (identity
-// for layer 0), Wi the sums pending mlp_norm: both packed as deferred-LayerNorm consumers with beta = bias = 0.
-static int pack_modernbert(ac_encoder *e, const ac_encoder_config *cfg, const ac_encoder_weights *w) {
-    const int H = cfg->hidden, I = cfg->intermediate, L = cfg->layers;
-    const size_t HH = static_cast<size_t>(H) * H;
+// Packs a deferred-LayerNorm consumer of sums pending LayerNorm (gamma, beta), NULL = identity: the n weights W[j] [N, K]
+// with biases bias[j] (bias NULL: none) stacked into one operand *wp [n N, K] and its vectors *c1, *c0 [n N].
+// glu != 0: W is a GeGLU weight (input rows, then gate rows), see pack_defer_kernel.
+static int pack_consumer(ac_encoder *e, int n, const float *const *W, const float *const *bias, const float *gamma,
+                         const float *beta, int N, int K, int glu, __half **wp, float **c1, float **c0) {
+    const size_t NK = static_cast<size_t>(N) * K;
     int rc;
-#define CHK(x) do { if ((rc = (x))) return rc; } while (0)
-    CHK(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
-    CHK(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
-    CHK(pack_f32(e, &e->final_norm, w->final_norm_w, H));
-    CHK(pack_f32(e, &e->rope[0], cfg->rope_full, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
-    CHK(pack_f32(e, &e->rope[1], cfg->rope_sliding, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
-    e->window.assign(L, 0);
-    e->wqkv_d.assign(L, nullptr); e->c1qkv.assign(L, nullptr); e->c0qkv.assign(L, nullptr); e->wo.assign(L, nullptr);
-    e->ln1w.assign(L, nullptr); e->w1_d.assign(L, nullptr); e->c1f.assign(L, nullptr); e->c0f.assign(L, nullptr);
-    e->w2.assign(L, nullptr);
-    for (int l = 0; l < L; ++l) {
-        e->window[l] = cfg->layer_sliding[l] ? cfg->sliding_window : 0;
-        CHK(dev_alloc(e, &e->wqkv_d[l], 3 * HH));
-        CHK(dev_alloc(e, &e->c1qkv[l], 3 * static_cast<size_t>(H)));
-        CHK(dev_alloc(e, &e->c0qkv[l], 3 * static_cast<size_t>(H)));
-        pack_defer_kernel<<<(3 * H + 7) / 8, 256>>>(w->wqkv[l], nullptr, l ? w->attn_norm_w[l] : nullptr, nullptr, 3 * H, H,
-                                                    e->wqkv_d[l], e->c1qkv[l], e->c0qkv[l]);
-        CHK(check_cuda(cudaGetLastError(), "pack_defer_kernel Wqkv"));
-        CHK(pack_f16(e, &e->wo[l], w->ao_w[l], HH));
-        CHK(pack_f32(e, &e->ln1w[l], w->ao_ln_w[l], H));
-        CHK(dev_alloc(e, &e->w1_d[l], 2 * static_cast<size_t>(I) * H));
-        CHK(dev_alloc(e, &e->c1f[l], 2 * static_cast<size_t>(I)));
-        CHK(dev_alloc(e, &e->c0f[l], 2 * static_cast<size_t>(I)));
-        pack_defer_kernel<<<(2 * I + 7) / 8, 256>>>(w->wi[l], nullptr, w->ao_ln_w[l], nullptr, 2 * I, H, e->w1_d[l], e->c1f[l],
-                                                    e->c0f[l], 1);
-        CHK(check_cuda(cudaGetLastError(), "pack_defer_kernel Wi"));
-        CHK(pack_f16(e, &e->w2[l], w->ff2_w[l], static_cast<size_t>(H) * I));
+    if ((rc = dev_alloc(e, wp, n * NK)) || (rc = dev_alloc(e, c1, static_cast<size_t>(n) * N)) ||
+        (rc = dev_alloc(e, c0, static_cast<size_t>(n) * N)))
+        return rc;
+    for (int j = 0; j < n; ++j) {
+        pack_defer_kernel<<<(N + 7) / 8, 256>>>(W[j], bias ? bias[j] : nullptr, gamma, beta, N, K, *wp + j * NK, *c1 + j * N,
+                                                *c0 + j * N, glu);
+        if ((rc = check_cuda(cudaGetLastError(), "pack_defer_kernel"))) return rc;
     }
-    if (cfg->cls_only) {
-        // plain interleaved Wi of the last layer: the CLS-only tail materialises mlp_norm (c1 / c0 are not used)
-        float *c1 = nullptr, *c0 = nullptr;
-        CHK(dev_alloc(e, &e->w1_last, 2 * static_cast<size_t>(I) * H));
-        CHK(dev_alloc(e, &c1, 2 * static_cast<size_t>(I)));
-        CHK(dev_alloc(e, &c0, 2 * static_cast<size_t>(I)));
-        pack_defer_kernel<<<(2 * I + 7) / 8, 256>>>(w->wi[L - 1], nullptr, nullptr, nullptr, 2 * I, H, e->w1_last, c1, c0, 1);
-        CHK(check_cuda(cudaGetLastError(), "pack_defer_kernel Wi (last layer)"));
-    }
-#undef CHK
     return AC_OK;
 }
 
@@ -1108,63 +1090,74 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     const size_t T = static_cast<size_t>((cfg->max_tokens + 127) / 128 * 128);
     e->T = T;
 #define TRY(x) do { rc = (x); if (rc) { ac_encoder_destroy(e); return rc; } } while (0)
-    e->cfg.layer_sliding = nullptr;   // copied into e->window / e->rope by pack_modernbert
+    e->cfg.layer_sliding = nullptr;   // copied into e->layers / e->rope below
     e->cfg.rope_full = e->cfg.rope_sliding = nullptr;
+    // ones / zeros are filled with the other constants after packing; the bias-free ModernBERT roles point at zeros
+    const int nzeros = std::max(3 * H, 2 * I);
+    TRY(dev_alloc(e, &e->ones, H));
+    TRY(dev_alloc(e, &e->zeros, nzeros));
+    e->layers.resize(L);
+    const size_t HH = static_cast<size_t>(H) * H, HI = static_cast<size_t>(H) * I;
     if (mb) {
-        TRY(pack_modernbert(e, cfg, w));
+        // ModernBERT (modeling_modernbert.py): no biases or LayerNorm betas.  Wqkv consumes the sums pending attn_norm
+        // (Identity in layer 0), Wi the sums pending mlp_norm
+        Layer &last = e->layers[L - 1];
+        TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
+        TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
+        TRY(pack_f32(e, &last.ln_out_w, w->final_norm_w, H));
+        TRY(pack_f32(e, &e->rope[0], cfg->rope_full, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
+        TRY(pack_f32(e, &e->rope[1], cfg->rope_sliding, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
+        e->emb_ln_b = e->b1_last = last.ln_out_b = e->zeros;
+        for (int l = 0; l < L; ++l) {
+            Layer &ly = e->layers[l];
+            ly.window = cfg->layer_sliding[l] ? cfg->sliding_window : 0;
+            ly.bo = ly.b2 = ly.ln_ffn_b = e->zeros;
+            TRY(pack_consumer(e, 1, &w->wqkv[l], nullptr, l ? w->attn_norm_w[l] : nullptr, nullptr, 3 * H, H, 0, &ly.wqkv,
+                              &ly.c1qkv, &ly.c0qkv));
+            TRY(pack_f16(e, &ly.wo, w->ao_w[l], HH));
+            TRY(pack_f32(e, &ly.ln_ffn_w, w->ao_ln_w[l], H));
+            TRY(pack_consumer(e, 1, &w->wi[l], nullptr, w->ao_ln_w[l], nullptr, 2 * I, H, 1, &ly.w1, &ly.c1f, &ly.c0f));
+            TRY(pack_f16(e, &ly.w2, w->ff2_w[l], HI));
+        }
+        if (cfg->cls_only) {
+            // plain interleaved Wi of the last layer: the CLS-only tail materialises mlp_norm (c1 / c0 are not used)
+            float *c1, *c0;
+            TRY(pack_consumer(e, 1, &w->wi[L - 1], nullptr, nullptr, nullptr, 2 * I, H, 1, &e->w1_last, &c1, &c0));
+        }
     } else {
         TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
         TRY(pack_f32(e, &e->pos, w->pos_emb, static_cast<size_t>(cfg->max_pos) * H));
         TRY(pack_f32(e, &e->type, w->type_emb, static_cast<size_t>(cfg->type_vocab) * H));
         TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
         TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, H));
-        e->wqkv_d.assign(L, nullptr); e->wo.assign(L, nullptr); e->w1_d.assign(L, nullptr); e->w2.assign(L, nullptr);
-        e->c1qkv.assign(L, nullptr); e->c0qkv.assign(L, nullptr); e->c1f.assign(L, nullptr); e->c0f.assign(L, nullptr);
-        e->bo.assign(L, nullptr); e->ln1w.assign(L, nullptr); e->ln1b.assign(L, nullptr);
-        e->b2.assign(L, nullptr); e->ln2w.assign(L, nullptr); e->ln2b.assign(L, nullptr);
-        const size_t HH = static_cast<size_t>(H) * H;
         for (int l = 0; l < L; ++l) {
-            // fused QKV operand [3H, H]: the projection of layer l consumes the sums whose pending LayerNorm is the output
-            // LayerNorm of layer l-1 (identity for layer 0: the embeddings arrive normalised)
-            TRY(dev_alloc(e, &e->wqkv_d[l], 3 * HH));
-            TRY(dev_alloc(e, &e->c1qkv[l], 3 * static_cast<size_t>(H)));
-            TRY(dev_alloc(e, &e->c0qkv[l], 3 * static_cast<size_t>(H)));
+            Layer &ly = e->layers[l];
+            // the fused QKV [3H, H] of layer l consumes the sums pending the output LayerNorm of layer l-1 (identity for
+            // layer 0: the embeddings arrive normalised), FFN1 the sums pending the attention-output LayerNorm of layer l
             const float *ws[3] = {w->q_w[l], w->k_w[l], w->v_w[l]};
             const float *bs[3] = {w->q_b[l], w->k_b[l], w->v_b[l]};
-            const float *pg = l ? w->out_ln_w[l - 1] : nullptr, *pb = l ? w->out_ln_b[l - 1] : nullptr;
-            for (int j = 0; j < 3; ++j) {
-                pack_defer_kernel<<<(H + 7) / 8, 256>>>(ws[j], bs[j], pg, pb, H, H, e->wqkv_d[l] + j * HH, e->c1qkv[l] + j * H,
-                                                        e->c0qkv[l] + j * H);
-                TRY(check_cuda(cudaGetLastError(), "pack_defer_kernel qkv"));
-            }
-            TRY(pack_f16(e, &e->wo[l], w->ao_w[l], HH));
-            TRY(pack_f32(e, &e->bo[l], w->ao_b[l], H));
-            TRY(pack_f32(e, &e->ln1w[l], w->ao_ln_w[l], H));
-            TRY(pack_f32(e, &e->ln1b[l], w->ao_ln_b[l], H));
-            // FFN1 of layer l consumes the sums pending the attention-output LayerNorm of layer l
-            TRY(dev_alloc(e, &e->w1_d[l], static_cast<size_t>(I) * H));
-            TRY(dev_alloc(e, &e->c1f[l], I));
-            TRY(dev_alloc(e, &e->c0f[l], I));
-            pack_defer_kernel<<<(I + 7) / 8, 256>>>(w->ff1_w[l], w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], I, H, e->w1_d[l], e->c1f[l],
-                                                    e->c0f[l]);
-            TRY(check_cuda(cudaGetLastError(), "pack_defer_kernel ffn1"));
-            TRY(pack_f16(e, &e->w2[l], w->ff2_w[l], static_cast<size_t>(H) * I));
-            TRY(pack_f32(e, &e->b2[l], w->ff2_b[l], H));
-            TRY(pack_f32(e, &e->ln2w[l], w->out_ln_w[l], H));
-            TRY(pack_f32(e, &e->ln2b[l], w->out_ln_b[l], H));
+            TRY(pack_consumer(e, 3, ws, bs, l ? w->out_ln_w[l - 1] : nullptr, l ? w->out_ln_b[l - 1] : nullptr, H, H, 0,
+                              &ly.wqkv, &ly.c1qkv, &ly.c0qkv));
+            TRY(pack_f16(e, &ly.wo, w->ao_w[l], HH));
+            TRY(pack_f32(e, &ly.bo, w->ao_b[l], H));
+            TRY(pack_f32(e, &ly.ln_ffn_w, w->ao_ln_w[l], H));
+            TRY(pack_f32(e, &ly.ln_ffn_b, w->ao_ln_b[l], H));
+            TRY(pack_consumer(e, 1, &w->ff1_w[l], &w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], I, H, 0, &ly.w1, &ly.c1f,
+                              &ly.c0f));
+            TRY(pack_f16(e, &ly.w2, w->ff2_w[l], HI));
+            TRY(pack_f32(e, &ly.b2, w->ff2_b[l], H));
+            TRY(pack_f32(e, &ly.ln_out_w, w->out_ln_w[l], H));
+            TRY(pack_f32(e, &ly.ln_out_b, w->out_ln_b[l], H));
         }
         if (cfg->cls_only) {
-            TRY(pack_f16(e, &e->w1_last, w->ff1_w[L - 1], static_cast<size_t>(I) * H));
+            TRY(pack_f16(e, &e->w1_last, w->ff1_w[L - 1], HI));
             TRY(pack_f32(e, &e->b1_last, w->ff1_b[L - 1], I));
         }
     }
-    const int nzeros = std::max(3 * H, 2 * I);
     TRY(dev_alloc(e, &e->stats_a, T));
     TRY(dev_alloc(e, &e->stats_b, T));
     TRY(dev_alloc(e, &e->stats_id, T));
     TRY(dev_alloc(e, &e->parts, static_cast<size_t>(H / GEMM_EPI_COLS) * T));
-    TRY(dev_alloc(e, &e->ones, H));
-    TRY(dev_alloc(e, &e->zeros, nzeros));
     fill_stats_identity_kernel<<<static_cast<unsigned>((T + 255) / 256), 256>>>(e->stats_id, static_cast<int64_t>(T));
     fill_value_kernel<<<(H + 255) / 256, 256>>>(e->ones, H, 1.f);
     fill_value_kernel<<<(nzeros + 255) / 256, 256>>>(e->zeros, nzeros, 0.f);
@@ -1199,13 +1192,12 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     TRY(make_tmap_2d(&e->m_xh_cls, e->xh_cls, 2, e->Bc, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_M, 64));
     TRY(make_tmap_2d(&e->m_ctx_cls, e->ctx_cls, 2, e->Bc, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_M, 64));
     TRY(make_tmap_2d(&e->m_ffn_cls, e->ffn_cls, 2, e->Bc, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_M, 64));
-    e->p_wqkv_d.resize(L); e->p_wo.resize(L); e->p_w1_d.resize(L); e->p_w2.resize(L);
     const int n1 = mb ? 2 * I : I;    // rows of the first FFN weight (ModernBERT: GeGLU input + gate)
-    for (int l = 0; l < L; ++l) {
-        TRY(make_tmap_2d(&e->p_wqkv_d[l], e->wqkv_d[l], 2, 3 * H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
-        TRY(make_tmap_2d(&e->p_wo[l], e->wo[l], 2, H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
-        TRY(make_tmap_2d(&e->p_w1_d[l], e->w1_d[l], 2, n1, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
-        TRY(make_tmap_2d(&e->p_w2[l], e->w2[l], 2, H, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_N, 64));
+    for (Layer &ly : e->layers) {
+        TRY(make_tmap_2d(&ly.m_wqkv, ly.wqkv, 2, 3 * H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+        TRY(make_tmap_2d(&ly.m_wo, ly.wo, 2, H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+        TRY(make_tmap_2d(&ly.m_w1, ly.w1, 2, n1, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
+        TRY(make_tmap_2d(&ly.m_w2, ly.w2, 2, H, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_N, 64));
     }
     if (cfg->cls_only) TRY(make_tmap_2d(&e->p_w1_last, e->w1_last, 2, n1, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
     TRY(check_cuda(cudaDeviceSynchronize(), "encoder_create sync"));
@@ -1214,85 +1206,100 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     return AC_OK;
 }
 
-using EpiGelu = EpiLinear<1, true, false>;                  // bias + GELU, fp16 out                       (CLS-only tail)
-using EpiResid = EpiLinear<2, false, false>;                // bias + residual, fp32 out (pre-LayerNorm sum, CLS-only tail)
-using EpiQKVDefer = EpiLinear<0, true, true, true>;         // r (acc - mu c1) + c0, fp16 out, V third transposed
-using EpiGeluDefer = EpiLinear<1, true, false, true>;       // GELU(r (acc - mu c1) + c0), fp16 out
-
-using EpiQKVRopeDefer = EpiLinear<0, true, true, true, true>;   // deferred LN + RoPE on q, k; V third transposed
-using EpiGegluDefer = EpiLinear<3, true, false, true>;        // GELU(input) * gate of the deferred-LN Wi, fp16 out
-using EpiGeglu = EpiLinear<3, true, false>;                   // the same on materialised LayerNorm rows (CLS-only tail)
-
 // One encoder projection = one GEMM (gemm_tc.cuh).  tb is the weight's GEMM_BLOCK_N-row-box map.
 template <class Epi>
 static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, int N, int K, const Epi &epi, cudaStream_t s) {
     return launch_gemm_tc<Epi, false, GEMM_KIND_F16>(ta, tb, M, N, K, epi, s);
 }
 
-// ModernBERT (modeling_modernbert.py ModernBertModel.forward): pre-LN blocks
-//     y += Wo attn(rope(Wqkv attn_norm(y)))        y += mlp.Wo GeGLU(Wi mlp_norm(y))        out = final_norm(y)
-// No LayerNorm is pending on the residual path, so the residual epilogues add the raw old sums (EpiResidDefer with the
-// identity LayerNorm: stats (0, 1), gamma 1, beta 0) and only the consuming projections apply attn_norm / mlp_norm deferred.
-static int forward_modernbert(ac_encoder *e, const int32_t *ids, const int32_t *mask, int B, int S, float *out_unit_cls,
-                              cudaStream_t s) {
+// The layer stack, for post-LN (BERT / RoBERTa / DistilBERT, modeling_bert.py) or pre-LN (ModernBERT,
+// modeling_modernbert.py ModernBertModel.forward) blocks:
+//     post-LN   y = LN1(y + attn(y))               y = LN2(y + GELU-FFN(y))               out = y
+//     pre-LN    y = y + attn(attn_norm(y))         y = y + GeGLU-FFN(mlp_norm(y))         out = final_norm(y)
+// e->x holds the un-normalised residual sums y, e->xh their fp16 copy.  QKV and FFN1 apply the LayerNorm they consume
+// deferred; the residual epilogues add LN_pending(y), carried as (row statistics, gamma, beta).  That pending LayerNorm is
+// the one decision the block kinds differ in: post-LN blocks leave LN1 / LN2 pending, pre-LN blocks keep the identity
+// (stats (0, 1), gamma 1, beta 0) pending throughout.  The rest is the epilogue type (RoPE, GeGLU) and data in e->layers.
+template <bool PRE_LN>
+static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids, int B, int S,
+                          float *out_unit_cls, cudaStream_t s) {
+    using EpiQKV = EpiLinear<0, true, true, true, PRE_LN>;          // r (acc - mu c1) + c0 (+ RoPE on q, k), V third transposed
+    using EpiFfn1 = EpiLinear<PRE_LN ? 3 : 1, true, false, true>;   // GELU, or GeGLU input * gate, of r (acc - mu c1) + c0
+    using EpiFfn1Rows = EpiLinear<PRE_LN ? 3 : 1, true, false>;     // the same on materialised LayerNorm rows (CLS-only tail)
+    using EpiResid = EpiLinear<2, false, false>;                    // bias + residual, fp32 out (CLS-only tail)
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden, I = c.intermediate, M = B * S;
+    const int N1 = PRE_LN ? 2 * I : I;                              // FFN1 accumulator columns (GeGLU: input + gate)
     const int S_pad = (S + 7) / 8 * 8;
     const int wpb = 8;
     const int row_blocks = (M + wpb - 1) / wpb;
     const int nparts = H / GEMM_EPI_COLS;
     const int64_t pstride = static_cast<int64_t>(e->T);
+    const bool cls_tail = c.cls_only && static_cast<size_t>(B) <= e->Bc;
     int rc;
-    embed_ln_kernel<<<row_blocks, wpb * 32, 0, s>>>(ids, nullptr, e->word, nullptr, nullptr, e->emb_ln_w, e->zeros, c.ln_eps, B, S,
-                                                    H, c.arch, c.pad_idx, c.vocab, c.max_pos, c.type_vocab, e->x, e->xh);
+    embed_ln_kernel<<<row_blocks, wpb * 32, 0, s>>>(ids, PRE_LN ? nullptr : type_ids, e->word, e->pos, e->type, e->emb_ln_w,
+                                                    e->emb_ln_b, c.ln_eps, B, S, H, c.arch, c.pad_idx, c.vocab, c.max_pos,
+                                                    c.type_vocab, e->x, e->xh);
     AC_LAUNCH_CHECK();
-    const float2 *st_in = e->stats_id;     // layer 0: attn_norm is Identity
+    // the embeddings arrive normalised: identity LayerNorm pending, and identity statistics for layer 0's QKV
+    const float2 *pst = e->stats_id, *st_qkv = e->stats_id;
+    const float *pg = e->ones, *pb = e->zeros;
     for (int l = 0; l < c.layers; ++l) {
-        const float *rope = e->rope[e->window[l] ? 1 : 0];
-        EpiQKVRopeDefer eq{e->c0qkv[l], nullptr, e->qk, M, 3 * H, 2 * H, 0, e->vT, 2 * H, S, S_pad, H, e->c1qkv[l], st_in, rope};
-        if ((rc = launch_linear(e->m_xh, e->p_wqkv_d[l], M, 3 * H, H, eq, s))) return rc;
-        if ((rc = launch_attention(e, mask, B, S, e->window[l], s))) return rc;
-        if (l == c.layers - 1 && c.cls_only && static_cast<size_t>(B) <= e->Bc) {
-            // CLS-only tail: y_cls += Wo ctx_cls; mlp_norm materialised; GeGLU; y_cls += mlp.Wo h; final_norm; normalise
-            const int cb = (B + wpb - 1) / wpb;
-            gather_cls_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, e->ctx_cls, e->x_cls);
-            AC_LAUNCH_CHECK();
-            EpiResid eo{e->zeros, e->x_cls, e->tmp_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
-            if ((rc = launch_linear(e->m_ctx_cls, e->p_wo[l], B, H, H, eo, s))) return rc;
-            layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->tmp_cls, e->ln1w[l], e->zeros, c.ln_eps, B, H, nullptr, e->xh_cls);
-            AC_LAUNCH_CHECK();
-            EpiGeglu e1{e->zeros, nullptr, e->ffn_cls, B, 2 * I, I, 0, nullptr, 0, 0, 0, 0};
-            if ((rc = launch_linear(e->m_xh_cls, e->p_w1_last, B, 2 * I, H, e1, s))) return rc;
-            EpiResid e2{e->zeros, e->tmp_cls, e->x_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
-            if ((rc = launch_linear(e->m_ffn_cls, e->p_w2[l], B, H, I, e2, s))) return rc;
-            layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->x_cls, e->final_norm, e->zeros, c.ln_eps, B, H, e->tmp_cls, nullptr);
-            AC_LAUNCH_CHECK();
-            if ((rc = launch_cls_normalize(e->tmp_cls, B, 1, H, out_unit_cls, s))) return rc;
-            e->last_B = B;
-            e->last_S = S;
-            e->last_cls_only = true;
-            return AC_OK;
-        }
-        EpiResidDefer eo{e->zeros, e->x, e->xh, e->stats_id, e->ones, e->zeros, e->parts, pstride, M, H, H};
-        if ((rc = launch_linear(e->m_ctx, e->p_wo[l], M, H, H, eo, s))) return rc;
+        const Layer &ly = e->layers[l];
+        EpiQKV eq{ly.c0qkv, nullptr, e->qk, M, 3 * H, 2 * H, 0, e->vT, 2 * H, S, S_pad, H, ly.c1qkv, st_qkv,
+                  e->rope[ly.window ? 1 : 0]};
+        if ((rc = launch_linear(e->m_xh, ly.m_wqkv, M, 3 * H, H, eq, s))) return rc;
+        if ((rc = launch_attention(e, mask, B, S, ly.window, s))) return rc;
+        if (l == c.layers - 1 && cls_tail) break;
+        // attention output projection + residual: y <- ctx Wo^T + bo + LN_pending(y); statistics of the new sums
+        EpiResidDefer eo{ly.bo, e->x, e->xh, pst, pg, pb, e->parts, pstride, M, H, H};
+        if ((rc = launch_linear(e->m_ctx, ly.m_wo, M, H, H, eo, s))) return rc;
         ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
         AC_LAUNCH_CHECK();
-        EpiGegluDefer e1{e->c0f[l], nullptr, e->ffn, M, 2 * I, I, 0, nullptr, 0, 0, 0, 0, e->c1f[l], e->stats_b};
-        if ((rc = launch_linear(e->m_xh, e->p_w1_d[l], M, 2 * I, H, e1, s))) return rc;
-        EpiResidDefer e2{e->zeros, e->x, e->xh, e->stats_id, e->ones, e->zeros, e->parts, pstride, M, H, H};
-        if ((rc = launch_linear(e->m_ffn, e->p_w2[l], M, H, I, e2, s))) return rc;
+        EpiFfn1 e1{ly.c0f, nullptr, e->ffn, M, N1, I, 0, nullptr, 0, 0, 0, 0, ly.c1f, e->stats_b};
+        if ((rc = launch_linear(e->m_xh, ly.m_w1, M, N1, H, e1, s))) return rc;
+        if constexpr (!PRE_LN) { pst = e->stats_b; pg = ly.ln_ffn_w; pb = ly.ln_ffn_b; }
+        // FFN output projection + residual: y <- ffn W2^T + b2 + LN_pending(y)
+        EpiResidDefer e2{ly.b2, e->x, e->xh, pst, pg, pb, e->parts, pstride, M, H, H};
+        if ((rc = launch_linear(e->m_ffn, ly.m_w2, M, H, I, e2, s))) return rc;
         ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_a);
         AC_LAUNCH_CHECK();
-        st_in = e->stats_a;
+        st_qkv = e->stats_a;
+        if constexpr (!PRE_LN) { pst = e->stats_a; pg = ly.ln_out_w; pb = ly.ln_out_b; }
     }
-    // full hidden state requested (cls_only = 0): final_norm on every row
-    layernorm_kernel<<<row_blocks, wpb * 32, 0, s>>>(e->x, e->final_norm, e->zeros, c.ln_eps, M, H, e->tmp, nullptr);
-    AC_LAUNCH_CHECK();
-    if ((rc = launch_cls_normalize(e->tmp, B, S, H, out_unit_cls, s))) return rc;
+    const Layer &last = e->layers.back();
+    if (cls_tail) {
+        // ---- CLS-only tail of the last layer (classifier.py:1272 pools row 0): M = B rows.  The LayerNorms are materialised
+        // on the CLS rows and FFN1 runs on the plain (not gamma-scaled) weight.  The W2 residual adds `res`: post-LN the
+        // LN1-normalised rows, pre-LN the raw sums; the output LayerNorm reads the new sums from `sum` and writes `res`.
+        float *res = PRE_LN ? e->tmp_cls : e->x_cls, *sum = PRE_LN ? e->x_cls : e->tmp_cls;
+        const int cb = (B + wpb - 1) / wpb;
+        if (pst == e->stats_id)   // identity pending: pre-LN, or the embeddings of a single-layer encoder
+            gather_cls_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, e->ctx_cls, e->x_cls);
+        else
+            gather_cls_ln_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, pg, pb, c.ln_eps, e->ctx_cls, e->x_cls);
+        AC_LAUNCH_CHECK();
+        EpiResid eo{last.bo, e->x_cls, e->tmp_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
+        if ((rc = launch_linear(e->m_ctx_cls, last.m_wo, B, H, H, eo, s))) return rc;
+        layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->tmp_cls, last.ln_ffn_w, last.ln_ffn_b, c.ln_eps, B, H, PRE_LN ? nullptr : res,
+                                                 e->xh_cls);
+        AC_LAUNCH_CHECK();
+        EpiFfn1Rows e1{e->b1_last, nullptr, e->ffn_cls, B, N1, I, 0, nullptr, 0, 0, 0, 0};
+        if ((rc = launch_linear(e->m_xh_cls, e->p_w1_last, B, N1, H, e1, s))) return rc;
+        EpiResid e2{last.b2, res, sum, B, H, H, 0, nullptr, 0, 0, 0, 0};
+        if ((rc = launch_linear(e->m_ffn_cls, last.m_w2, B, H, I, e2, s))) return rc;
+        layernorm_kernel<<<cb, wpb * 32, 0, s>>>(sum, last.ln_out_w, last.ln_out_b, c.ln_eps, B, H, res, nullptr);
+        AC_LAUNCH_CHECK();
+        if ((rc = launch_cls_normalize(res, B, 1, H, out_unit_cls, s))) return rc;
+    } else {
+        // full hidden state requested (cls_only = 0, or B > Bc): materialise the output LayerNorm for every row
+        layernorm_kernel<<<row_blocks, wpb * 32, 0, s>>>(e->x, last.ln_out_w, last.ln_out_b, c.ln_eps, M, H, e->tmp, nullptr);
+        AC_LAUNCH_CHECK();
+        if ((rc = launch_cls_normalize(e->tmp, B, S, H, out_unit_cls, s))) return rc;
+    }
     e->last_B = B;
     e->last_S = S;
-    e->last_cls_only = false;
-    e->last_hidden = e->tmp;
+    e->last_cls_only = cls_tail;
     return AC_OK;
 }
 
@@ -1309,7 +1316,7 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
     AC_REQUIRE(S <= e->cfg.max_pos, "ac_encoder_forward_cls: S exceeds max_position_embeddings");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const ac_encoder_config &c = e->cfg;
-    const int H = c.hidden, I = c.intermediate, M = B * S;
+    const int H = c.hidden;
     const int S_pad = (S + 7) / 8 * 8;
     AC_REQUIRE(static_cast<size_t>(B) * H * S_pad <= e->vt_elems,
                "ac_encoder_forward_cls: B=%d sequences of S=%d exceed the transposed-V workspace; split the batch", B, S);
@@ -1321,74 +1328,8 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
             return rc;
         e->vt_B = B; e->vt_S = S;
     }
-    if (c.arch == AC_ARCH_MODERNBERT) return forward_modernbert(e, ids, mask, B, S, out_unit_cls, s);
-    const int wpb = 8;
-    const int row_blocks = (M + wpb - 1) / wpb;
-    const int nparts = H / GEMM_EPI_COLS;
-    const int64_t pstride = static_cast<int64_t>(e->T);
-
-    // e->x holds the un-normalised residual sums y, e->xh their fp16 copy; the LayerNorm still pending on y is carried as
-    // (gamma, beta, row statistics).  The embeddings arrive normalised: identity LayerNorm pending.
-    embed_ln_kernel<<<row_blocks, wpb * 32, 0, s>>>(ids, type_ids, e->word, e->pos, e->type, e->emb_ln_w, e->emb_ln_b,
-                                                    c.ln_eps, B, S, H, c.arch, c.pad_idx, c.vocab, c.max_pos,
-                                                    c.type_vocab, e->x, e->xh);
-    AC_LAUNCH_CHECK();
-    const float *pg = e->ones, *pb = e->zeros;
-    const float2 *st_in = e->stats_id;
-    for (int l = 0; l < c.layers; ++l) {
-        EpiQKVDefer eq{e->c0qkv[l], nullptr, e->qk, M, 3 * H, 2 * H, 0, e->vT, 2 * H, S, S_pad, H, e->c1qkv[l], st_in};
-        if ((rc = launch_linear(e->m_xh, e->p_wqkv_d[l], M, 3 * H, H, eq, s))) return rc;
-        if ((rc = launch_attention(e, mask, B, S, 0, s))) return rc;
-        if (l == c.layers - 1 && c.cls_only && static_cast<size_t>(B) <= e->Bc) {
-            // ---- CLS-only tail of the last layer (classifier.py:1272 pools row 0): M = B rows.  LN_pending is materialised on
-            // the CLS rows and the tail runs on ordinary LayerNorm kernels and the plain (not gamma-scaled) FFN1 weight
-            const int cb = (B + wpb - 1) / wpb;
-            if (l == 0)   // single-layer encoder: nothing is pending on the (already normalised) embeddings
-                gather_cls_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, e->ctx_cls, e->x_cls);
-            else
-                gather_cls_ln_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, pg, pb, c.ln_eps, e->ctx_cls, e->x_cls);
-            AC_LAUNCH_CHECK();
-            EpiResid eo{e->bo[l], e->x_cls, e->tmp_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
-            if ((rc = launch_linear(e->m_ctx_cls, e->p_wo[l], B, H, H, eo, s))) return rc;
-            layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->tmp_cls, e->ln1w[l], e->ln1b[l], c.ln_eps, B, H, e->x_cls, e->xh_cls);
-            AC_LAUNCH_CHECK();
-            EpiGelu e1{e->b1_last, nullptr, e->ffn_cls, B, I, I, 0, nullptr, 0, 0, 0, 0};
-            if ((rc = launch_linear(e->m_xh_cls, e->p_w1_last, B, I, H, e1, s))) return rc;
-            EpiResid e2{e->b2[l], e->x_cls, e->tmp_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
-            if ((rc = launch_linear(e->m_ffn_cls, e->p_w2[l], B, H, I, e2, s))) return rc;
-            layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->tmp_cls, e->ln2w[l], e->ln2b[l], c.ln_eps, B, H, e->x_cls, nullptr);
-            AC_LAUNCH_CHECK();
-            if ((rc = launch_cls_normalize(e->x_cls, B, 1, H, out_unit_cls, s))) return rc;
-            e->last_B = B;
-            e->last_S = S;
-            e->last_cls_only = true;
-            return AC_OK;
-        }
-        // attention output projection + residual: y <- ctx Wo^T + bo + LN_pending(y); statistics of the new sums
-        EpiResidDefer eo{e->bo[l], e->x, e->xh, st_in, pg, pb, e->parts, pstride, M, H, H};
-        if ((rc = launch_linear(e->m_ctx, e->p_wo[l], M, H, H, eo, s))) return rc;
-        ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
-        AC_LAUNCH_CHECK();
-        EpiGeluDefer e1{e->c0f[l], nullptr, e->ffn, M, I, I, 0, nullptr, 0, 0, 0, 0, e->c1f[l], e->stats_b};
-        if ((rc = launch_linear(e->m_xh, e->p_w1_d[l], M, I, H, e1, s))) return rc;
-        // FFN output projection + residual: y <- ffn W2^T + b2 + LN_attention_output(y)
-        EpiResidDefer e2{e->b2[l], e->x, e->xh, e->stats_b, e->ln1w[l], e->ln1b[l], e->parts, pstride, M, H, H};
-        if ((rc = launch_linear(e->m_ffn, e->p_w2[l], M, H, I, e2, s))) return rc;
-        ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_a);
-        AC_LAUNCH_CHECK();
-        pg = e->ln2w[l];
-        pb = e->ln2b[l];
-        st_in = e->stats_a;
-    }
-    // full hidden state requested (cls_only = 0): materialise the last LayerNorm for every row
-    layernorm_kernel<<<row_blocks, wpb * 32, 0, s>>>(e->x, pg, pb, c.ln_eps, M, H, e->tmp, nullptr);
-    AC_LAUNCH_CHECK();
-    if ((rc = launch_cls_normalize(e->tmp, B, S, H, out_unit_cls, s))) return rc;
-    e->last_B = B;
-    e->last_S = S;
-    e->last_cls_only = false;
-    e->last_hidden = e->tmp;
-    return AC_OK;
+    return c.arch == AC_ARCH_MODERNBERT ? forward_layers<true>(e, ids, mask, type_ids, B, S, out_unit_cls, s)
+                                        : forward_layers<false>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
 }
 
 extern "C" int ac_encoder_last_hidden(ac_encoder *e, float *out, int64_t n_floats, ac_stream_t stream) {
@@ -1397,7 +1338,7 @@ extern "C" int ac_encoder_last_hidden(ac_encoder *e, float *out, int64_t n_float
                                   "(create the encoder with cls_only = 0 to keep the full hidden state)");
     const int64_t have = static_cast<int64_t>(e->last_B) * e->last_S * e->cfg.hidden;
     AC_REQUIRE(n_floats <= have, "ac_encoder_last_hidden: asked %lld floats, have %lld", (long long)n_floats, (long long)have);
-    AC_CUDA(cudaMemcpyAsync(out, e->last_hidden ? e->last_hidden : e->x, n_floats * sizeof(float), cudaMemcpyDeviceToDevice,
+    AC_CUDA(cudaMemcpyAsync(out, e->tmp, n_floats * sizeof(float), cudaMemcpyDeviceToDevice,
                             static_cast<cudaStream_t>(stream)));
     return AC_OK;
 }
