@@ -27,6 +27,7 @@ AC_COST_LINEAR, AC_COST_SEPARABLE = 0, 1
 AC_STRATEGIC_CANDIDATES = 50
 AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT = 0, 1, 2
 AC_ENCODER_MAX_S = 512
+AC_MODERNBERT_MAX_S = 8192
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
 
 EXPORTS = [
@@ -595,8 +596,14 @@ def modernbert_settings(c) -> dict:
     window = int(c.sliding_window)
     if "sliding_attention" in types and window < 1:
         raise AdaptiveB200Error(f"ModernBERT sliding_window={window}: the half-window must be >= 1")
+    # the longest sequence the encoder accepts and the rows of its RoPE tables; never fewer than the BERT-family limit
+    max_pos = max(AC_ENCODER_MAX_S, int(c.max_position_embeddings))
+    if max_pos > AC_MODERNBERT_MAX_S:
+        raise AdaptiveB200Error(f"ModernBERT max_position_embeddings={c.max_position_embeddings}: at most "
+                                f"{AC_MODERNBERT_MAX_S} is implemented")
     return dict(layers=c.num_hidden_layers, hidden=c.hidden_size, heads=heads, intermediate=c.intermediate_size,
-                vocab=c.vocab_size, ln_eps=c.norm_eps, pad_idx=(c.pad_token_id if c.pad_token_id is not None else 0),
+                vocab=c.vocab_size, max_pos=max_pos, ln_eps=c.norm_eps,
+                pad_idx=(c.pad_token_id if c.pad_token_id is not None else 0),
                 sliding_window=window, layer_sliding=[1 if t == "sliding_attention" else 0 for t in types],
                 rope_theta=(theta["full_attention"], theta["sliding_attention"]))
 
@@ -636,10 +643,10 @@ class Encoder:
             w.wqkv, w.wi = arr(p + "attn.Wqkv.weight"), arr(p + "mlp.Wi.weight")
             an = (c_void_p * layers)(None, *[g(f"layers.{l}.attn_norm.weight") for l in range(1, layers)])  # layer 0: Identity
             ls = (ctypes.c_int32 * layers)(*layer_sliding)
-            rope = [modernbert_rope_table(t).to(dev) for t in rope_theta]
+            rope = [modernbert_rope_table(t, max_pos).to(dev) for t in rope_theta]
             keep.update(an=an, ls=ls, rope=rope)
             w.attn_norm_w = ctypes.cast(an, _PP)
-            cfg = EncoderConfig(AC_ARCH_MODERNBERT, layers, hidden, heads, intermediate, vocab, AC_ENCODER_MAX_S, 1, pad_idx,
+            cfg = EncoderConfig(AC_ARCH_MODERNBERT, layers, hidden, heads, intermediate, vocab, max_pos, 1, pad_idx,
                                 ln_eps, AC_PREC_F16, max_tokens, 1 if cls_only else 0, sliding_window,
                                 ctypes.cast(ls, POINTER(ctypes.c_int32)), rope[0].data_ptr(), rope[1].data_ptr())
         else:
@@ -668,7 +675,8 @@ class Encoder:
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
         """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel (post-LN blocks) or ModernBertModel (pre-LN,
-        RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for the post-LN family, 64 for ModernBERT."""
+        RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for the post-LN family, 64 for ModernBERT.  Sequences up to 512
+        tokens, or for ModernBERT up to max(512, max_position_embeddings) <= AC_MODERNBERT_MAX_S."""
         c = model.config
         mt = getattr(c, "model_type", "bert")
         if mt == "modernbert":

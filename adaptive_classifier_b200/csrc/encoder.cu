@@ -14,7 +14,9 @@
 //   projections   wgmma GEMM of gemm_tc.cuh (.f16) with compile-time-specialised fused epilogues:
 //                 bias | bias+GELU(erf) | bias+residual, fp16 or fp32 output, V written TRANSPOSED per (sequence, head)
 //   attention     one CTA per (sequence, head): Q, K and V^T tiles by TMA, QK^T and PV as wgmma with the score tile
-//                 staged in shared memory, thread-per-query-row softmax in between (S <= 128; head_dim 64 or 32)
+//                 staged in shared memory, thread-per-query-row softmax in between (S <= 128; head_dim 64 or 32); 128-query
+//                 blocks over streamed key blocks for S <= 512, and for ModernBERT up to S = 8192 one pass with an online
+//                 softmax that visits only the key blocks inside a sliding layer's band (attention_stream_kernel)
 //   LayerNorm     never materialised inside the layer stack: the residual epilogues keep the un-normalised sums y (fp32) and
 //                 per-row (sum, sumsq) partials, the consuming projections run on gamma-scaled weights and apply the
 //                 rank-1 correction r (acc - mu c1) + c0 in their epilogue ("deferred LayerNorm" below)
@@ -907,6 +909,159 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
     if (qglob < S) att_write_row<DH>(srow, inv, ctx + (row0 + qglob) * H + h * DH);
 }
 
+// ------------------------------------------------------------------------------------------------
+// attention for AC_ENCODER_MAX_S < S <= AC_MODERNBERT_MAX_S (ModernBERT, head_dim 64): one CTA per (sequence, head,
+// 128-query block), ONE pass over the key blocks with an online softmax.
+//   key blocks    full layers visit all ceil(S / 128); sliding layers only those intersecting [q0 - w, q0 + 127 + w]
+//                 (band_bits masks inside them), so a sliding layer costs O(S w) instead of O(S^2)
+//   ring          K and V^T blocks come through two TMA stages: block i + 1 loads while block i runs its MMAs and softmax
+//   softmax       thread = query row on the shared score tile: running row max m and row sum l; when m grows, the fp32
+//                 O accumulator (wgmma registers) is scaled by exp(m_old - m_new), handed to the fragment rows
+//                 16 warp + lane / 4 (+ 8, + 64) through shared memory.  A row that has seen no valid key yet (the ends of
+//                 a sliding query block, holes in the mask) keeps m = -inf, P = 0 and a zero accumulator: the factor is
+//                 0 there rather than exp((-inf) - (-inf))
+//   P fp16, every accumulator fp32, as in the kernels above.  q_blocks = 1 (CLS-only tail next) computes rows 0..127 only.
+// smem: Q 16 KB | K 2 x 16 KB | V^T 2 x 16 KB | P 32 KB | score tile 66 KB | factors 512 B | 2 barriers: one CTA per SM.
+// ------------------------------------------------------------------------------------------------
+constexpr int ATTS_STAGE_BYTES = 16 * 1024;
+constexpr int ATTS_OFF_K = 16 * 1024, ATTS_OFF_VT = 48 * 1024, ATTS_OFF_P = 80 * 1024, ATTS_OFF_S = 112 * 1024;
+constexpr int ATTS_SMEM = ATTS_OFF_S + ATT_S_BYTES + 128 * 4 + 2 * 8 + 1024 /*align*/;
+static_assert(ATTS_SMEM <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
+
+template <int DH>
+__global__ void __launch_bounds__(ATT_THREADS)
+attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
+                        const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
+    static_assert(DH == 64, "S > 512 runs ModernBERT only (head_dim 64)");
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *sQ = smem;                              // [128 x 128 B]
+    uint8_t *sK = smem + ATTS_OFF_K;                 // stage st: [128 keys x 128 B]
+    uint8_t *sVt = smem + ATTS_OFF_VT;               // stage st: 2 slabs x [64 (d) x 128 B (64 keys)]
+    uint8_t *sP = smem + ATTS_OFF_P;                 // 2 slabs x [128 x 128 B (64 keys)]
+    float *sS = reinterpret_cast<float *>(smem + ATTS_OFF_S);
+    float *sAlpha = sS + 128 * ATT_S_LD;             // [128] rescale factor of each query row
+    uint64_t *bar = reinterpret_cast<uint64_t *>(sAlpha + 128);
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+    const int q0 = blockIdx.y * 128;
+    const int64_t row0 = static_cast<int64_t>(b) * S;
+    const int vrow = (b * heads + h) * DH;
+    int kb0 = 0, kb1 = (S + 127) / 128;              // key blocks [kb0, kb1) of this query block
+    if (window > 0) {
+        kb0 = max(q0 - window, 0) / 128;
+        kb1 = min(q0 + 127 + window, S - 1) / 128 + 1;
+    }
+    const int nblk = kb1 - kb0;
+
+    // visit i -> stage i & 1; the first visit also brings Q
+    auto issue = [&](int i) {
+        const int st = i & 1, key0 = (kb0 + i) * 128;
+        mbar_arrive_expect_tx(bar + st, (i == 0 ? 3 : 2) * ATTS_STAGE_BYTES);
+        if (i == 0) tma_load_2d(sQ, &tmap_qk, bar, h * DH, static_cast<int>(row0) + q0);
+        tma_load_2d(sK + st * ATTS_STAGE_BYTES, &tmap_qk, bar + st, H + h * DH, static_cast<int>(row0) + key0);
+        tma_load_2d(sVt + st * ATTS_STAGE_BYTES, &tmap_vt, bar + st, key0, vrow);
+        tma_load_2d(sVt + st * ATTS_STAGE_BYTES + 8192, &tmap_vt, bar + st, key0 + 64, vrow);
+    };
+    if (tid == 0) {
+        tma_prefetch_desc(&tmap_qk);
+        tma_prefetch_desc(&tmap_vt);
+        mbar_init(bar, 1);
+        mbar_init(bar + 1, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    if (tid == 0) {
+        issue(0);
+        if (nblk > 1) issue(1);
+    }
+
+    const int qrow = warp * 32 + lane;                            // row inside the query block
+    const int qglob = q0 + qrow;                                  // position inside the sequence
+    const float *srow = sS + qrow * ATT_S_LD;
+    const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
+    const int frow = 16 * warp + (lane >> 2);                     // accumulator fragment rows frow, frow + 8 (+ 64)
+    const uint32_t sp_base = smem_u32(sP);
+    float mx = -CUDART_INF_F, sum = 0.f;
+    float o[2][DH / 2];
+#pragma unroll
+    for (int half = 0; half < 2; ++half)
+#pragma unroll
+        for (int j = 0; j < DH / 2; ++j) o[half][j] = 0.f;
+
+#pragma unroll 1
+    for (int i = 0; i < nblk; ++i) {
+        const int st = i & 1, key0 = (kb0 + i) * 128;
+        mbar_wait_guarded(bar + st, (i >> 1) & 1);
+        att_scores<DH>(sQ, sK + st * ATTS_STAGE_BYTES, sS);
+        __syncthreads();
+
+        uint32_t kmask[4];
+#pragma unroll
+        for (int w4 = 0; w4 < 4; ++w4) {
+            const int key = key0 + 32 * w4 + lane;
+            const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
+            kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(qglob, key0 + 32 * w4, window);
+        }
+        float bmx = -CUDART_INF_F;
+#pragma unroll
+        for (int ci = 0; ci < 4; ++ci) {
+            float r[32];
+            acc_row_ld32(srow + 32 * ci, r);
+#pragma unroll
+            for (int jj = 0; jj < 32; ++jj)
+                if ((kmask[ci] >> jj) & 1u) bmx = fmaxf(bmx, r[jj]);
+        }
+        const float mnew = fmaxf(mx, bmx);
+        const float alpha = (mx == -CUDART_INF_F) ? 0.f : ex2_approx((mx - mnew) * scale_log2);
+        const float mxs = (mnew == -CUDART_INF_F) ? 0.f : mnew * scale_log2;   // no valid key yet: every P below is 0
+        float bsum = 0.f;
+#pragma unroll
+        for (int ci = 0; ci < 4; ++ci) {
+            float r[32];
+            acc_row_ld32(srow + 32 * ci, r);
+            const uint32_t km = kmask[ci];
+            uint32_t pk[16];
+#pragma unroll
+            for (int jj = 0; jj < 32; jj += 2) {
+                const float e0 = ((km >> jj) & 1u) ? ex2_approx(fmaf(r[jj], scale_log2, -mxs)) : 0.f;
+                const float e1 = ((km >> (jj + 1)) & 1u) ? ex2_approx(fmaf(r[jj + 1], scale_log2, -mxs)) : 0.f;
+                bsum += e0 + e1;
+                __half2 hh = __floats2half2_rn(e0, e1);
+                pk[jj >> 1] = *reinterpret_cast<uint32_t *>(&hh);
+            }
+            att_store_p(sp_base, qrow, 32 * ci, pk);
+        }
+        sum = fmaf(sum, alpha, bsum);
+        mx = mnew;
+        sAlpha[qrow] = alpha;
+        fence_proxy_async_smem();
+        __syncthreads();                                          // P and the factors are complete
+
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const float a0 = sAlpha[64 * half + frow], a1 = sAlpha[64 * half + frow + 8];
+#pragma unroll
+            for (int j = 0; j < DH / 8; ++j) {
+                o[half][4 * j] *= a0;
+                o[half][4 * j + 1] *= a0;
+                o[half][4 * j + 2] *= a1;
+                o[half][4 * j + 3] *= a1;
+            }
+        }
+        att_pv<DH>(sP, sVt + st * ATTS_STAGE_BYTES, o, true);
+        __syncthreads();                                          // stage st, P, the score tile and the factors are free
+        if (tid == 0 && i + 2 < nblk) issue(i + 2);
+    }
+
+    wgmma_store_acc(o[0], sS, ATT_S_LD);
+    wgmma_store_acc(o[1], sS + 64 * ATT_S_LD, ATT_S_LD);
+    __syncthreads();
+    const float inv = (sum > 0.f) ? 1.f / sum : 0.f;
+    if (qglob < S) att_write_row<DH>(srow, inv, ctx + (row0 + qglob) * H + h * DH);
+}
+
 // last layer, deferred flow: CLS rows of the attention context and of LN_pending(y) (two-pass statistics from the fp32 sums)
 __global__ void gather_cls_ln_kernel(const __half *__restrict__ ctx, const float *__restrict__ y, int B, int S, int H,
                                      const float *__restrict__ g, const float *__restrict__ b, float eps,
@@ -974,7 +1129,7 @@ struct ac_encoder {
     // row statistics (ping-pong) and the per-GEMM_EPI_COLS-column partials the residual epilogues write
     float2 *stats_a = nullptr, *stats_b = nullptr, *stats_id = nullptr, *parts = nullptr;
     float *ones = nullptr, *zeros = nullptr;   // ones [H]; zeros [max(3H, 2I)]: beta / bias of the bias-free ModernBERT
-    float *rope[2] = {nullptr, nullptr};       // ModernBERT RoPE tables [AC_ENCODER_MAX_S, 64] (full, sliding layers)
+    float *rope[2] = {nullptr, nullptr};       // ModernBERT RoPE tables [max_pos, 64] (full, sliding layers)
     std::vector<void *> allocs;
     int last_B = 0, last_S = 0;           // shape of the previous forward; its full hidden state (cls_only = 0) is in tmp
     bool last_cls_only = false;
@@ -987,8 +1142,39 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
     return AC_OK;
 }
 
-// softmax(Q K^T / sqrt(head_dim) + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention
-static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, cudaStream_t s) {
+// S > AC_ENCODER_MAX_S (attention_stream_kernel): the queries of q_blocks 128-row blocks, each attending to the keys of its band
+static int launch_attention_stream(ac_encoder *e, const int32_t *mask, int B, int S, int window, int q_blocks, cudaStream_t s) {
+    const ac_encoder_config &c = e->cfg;
+    const int H = c.hidden, dh = H / c.heads;
+    AC_REQUIRE(dh == 64, "attention: S=%d > %d needs head_dim 64 (ModernBERT)", S, AC_ENCODER_MAX_S);
+    static bool att_attr[64] = {};
+    int dev = 0;
+    AC_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= 64 || !att_attr[dev]) {
+        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
+        if (dev >= 0 && dev < 64) att_attr[dev] = true;
+    }
+    // algorithmic flops over the keys each computed query attends to: (2w + 1) clipped to [0, S) in sliding layers
+    const int nq = std::min(S, 128 * q_blocks);
+    double keys = 0.0;
+    if (window > 0) {
+        for (int q = 0; q < nq; ++q) keys += std::min(S - 1, q + window) - std::max(0, q - window) + 1;
+    } else {
+        keys = static_cast<double>(nq) * S;
+    }
+    const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * keys * dh, 0.0, s);
+    attention_stream_kernel<64><<<dim3(B * c.heads, q_blocks), ATT_THREADS, ATTS_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S,
+                                                                                          c.heads, H, window, e->ctx);
+    prof_end(slot, s);
+    AC_LAUNCH_CHECK();
+    return AC_OK;
+}
+
+// softmax(Q K^T / sqrt(head_dim) + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention.
+// cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail); S > AC_ENCODER_MAX_S then computes the first
+// query block only.
+static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, cudaStream_t s) {
+    if (S > AC_ENCODER_MAX_S) return launch_attention_stream(e, mask, B, S, window, cls_rows ? 1 : (S + 127) / 128, s);
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden;
     const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create)
@@ -1070,10 +1256,11 @@ static int pack_consumer(ac_encoder *e, int n, const float *const *W, const floa
 extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_weights *w, ac_encoder **out) {
     AC_REQUIRE(cfg && w && out, "ac_encoder_create: null argument");
     const bool mb = cfg->arch == AC_ARCH_MODERNBERT;
-    AC_REQUIRE(!mb || (cfg->max_pos == AC_ENCODER_MAX_S && cfg->layer_sliding && cfg->sliding_window > 0 && cfg->rope_full &&
-                       cfg->rope_sliding && w->wqkv && w->wi && w->final_norm_w && (cfg->layers == 1 || w->attn_norm_w)),
-               "ac_encoder_create: ModernBERT needs max_pos = %d, layer_sliding, sliding_window > 0, both RoPE tables, "
-               "wqkv, wi, final_norm_w and attn_norm_w", AC_ENCODER_MAX_S);
+    AC_REQUIRE(!mb || (cfg->max_pos >= AC_ENCODER_MAX_S && cfg->max_pos <= AC_MODERNBERT_MAX_S && cfg->layer_sliding &&
+                       cfg->sliding_window > 0 && cfg->rope_full && cfg->rope_sliding && w->wqkv && w->wi && w->final_norm_w &&
+                       (cfg->layers == 1 || w->attn_norm_w)),
+               "ac_encoder_create: ModernBERT needs %d <= max_pos <= %d (max_pos=%d), layer_sliding, sliding_window > 0, both "
+               "RoPE tables, wqkv, wi, final_norm_w and attn_norm_w", AC_ENCODER_MAX_S, AC_MODERNBERT_MAX_S, cfg->max_pos);
     AC_REQUIRE(cfg->precision == AC_PREC_F16, "ac_encoder_create: only AC_PREC_F16 (fp16 operands, fp32 accumulate) is implemented");
     AC_REQUIRE(cfg->hidden % 128 == 0 && cfg->hidden <= 1024, "ac_encoder_create: hidden=%d must be a multiple of 128, <= 1024", cfg->hidden);
     // the attention kernels take head_dim 64 or 32; ModernBERT's RoPE epilogue pairs (d, d + 32) inside a 64-column head
@@ -1105,8 +1292,8 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
         TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
         TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
         TRY(pack_f32(e, &last.ln_out_w, w->final_norm_w, H));
-        TRY(pack_f32(e, &e->rope[0], cfg->rope_full, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
-        TRY(pack_f32(e, &e->rope[1], cfg->rope_sliding, static_cast<size_t>(AC_ENCODER_MAX_S) * 64));
+        TRY(pack_f32(e, &e->rope[0], cfg->rope_full, static_cast<size_t>(cfg->max_pos) * 64));
+        TRY(pack_f32(e, &e->rope[1], cfg->rope_sliding, static_cast<size_t>(cfg->max_pos) * 64));
         e->emb_ln_b = e->b1_last = last.ln_out_b = e->zeros;
         for (int l = 0; l < L; ++l) {
             Layer &ly = e->layers[l];
@@ -1249,7 +1436,7 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
         EpiQKV eq{ly.c0qkv, nullptr, e->qk, M, 3 * H, 2 * H, 0, e->vT, 2 * H, S, S_pad, H, ly.c1qkv, st_qkv,
                   e->rope[ly.window ? 1 : 0]};
         if ((rc = launch_linear(e->m_xh, ly.m_wqkv, M, 3 * H, H, eq, s))) return rc;
-        if ((rc = launch_attention(e, mask, B, S, ly.window, s))) return rc;
+        if ((rc = launch_attention(e, mask, B, S, ly.window, l == c.layers - 1 && cls_tail, s))) return rc;
         if (l == c.layers - 1 && cls_tail) break;
         // attention output projection + residual: y <- ctx Wo^T + bo + LN_pending(y); statistics of the new sums
         EpiResidDefer eo{ly.bo, e->x, e->xh, pst, pg, pb, e->parts, pstride, M, H, H};
@@ -1307,7 +1494,11 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
                                       int B, int S, float *out_unit_cls, ac_stream_t stream) {
     AC_REQUIRE(e && ids && out_unit_cls, "ac_encoder_forward_cls: null argument");
     AC_REQUIRE(B > 0 && S > 0, "ac_encoder_forward_cls: B=%d S=%d", B, S);
-    if (S > 512) {
+    if (e->cfg.arch == AC_ARCH_MODERNBERT) {
+        // RoPE has no position table: any S up to the encoder's max_pos (<= AC_MODERNBERT_MAX_S) runs
+        AC_REQUIRE(S <= e->cfg.max_pos, "ac_encoder_forward_cls: S=%d exceeds this ModernBERT encoder's max_pos=%d "
+                   "(max_position_embeddings)", S, e->cfg.max_pos);
+    } else if (S > 512) {
         set_error("ac_encoder_forward_cls: S=%d > 512 is not supported (the reference truncates at max_length = 512)", S);
         return AC_E_UNSUPPORTED;
     }

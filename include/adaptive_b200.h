@@ -245,7 +245,10 @@ int ac_head_train_strategic(const float *X, const int64_t *targets, const int64_
  *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel / ModernBertModel forward).
  * ------------------------------------------------------------------------------------------ */
 enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2 };
-#define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts (the reference truncates at 512) */
+#define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts for BERT / RoBERTa / DistilBERT (their
+                                  position tables stop at 512) */
+#define AC_MODERNBERT_MAX_S 8192   /* largest max_pos of an AC_ARCH_MODERNBERT encoder (max_position_embeddings of the
+                                      published checkpoints); S > AC_ENCODER_MAX_S runs the streamed attention kernel */
 enum {
     AC_PREC_TF32 = 0,   /* wgmma .tf32 on fp32 storage (kNN coarse pass, ac_linear_tc tests) */
     AC_PREC_F16 = 1     /* wgmma .f16 with fp16 operands (RNE from fp32; same 10-bit mantissa as tf32),
@@ -263,10 +266,11 @@ typedef struct {
     int max_tokens;      /* workspace is sized for B*S <= max_tokens */
     int cls_only;        /* != 0: the last layer's output projection / FFN / LayerNorms run on the CLS rows only
                             (classifier.py:1272 uses nothing else); 0 keeps the full last hidden state */
-    /* AC_ARCH_MODERNBERT only (ignored otherwise).  max_pos must be AC_ENCODER_MAX_S (RoPE has no position table). */
+    /* AC_ARCH_MODERNBERT only (ignored otherwise).  AC_ENCODER_MAX_S <= max_pos <= AC_MODERNBERT_MAX_S: the longest
+       sequence the encoder accepts and the rows of both RoPE tables (RoPE has no position parameters). */
     int sliding_window;          /* half-window w = local_attention / 2: a sliding layer's query i sees keys |i - j| <= w */
     const int32_t *layer_sliding;  /* HOST array [layers]: 1 = sliding_attention, 0 = full_attention (config.layer_types) */
-    const float *rope_full;      /* DEVICE [AC_ENCODER_MAX_S, 64] fp32 RoPE table of the full-attention layers:      */
+    const float *rope_full;      /* DEVICE [max_pos, 64] fp32 RoPE table of the full-attention layers:              */
     const float *rope_sliding;   /*   row = position, [0, 32) cos, [32, 64) sin of the 32 frequencies (HF
                                        ModernBertRotaryEmbedding's formula, built by the caller); the sliding layers' table */
 } ac_encoder_config;
@@ -298,7 +302,8 @@ int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_weights *w,
 int ac_encoder_destroy(ac_encoder *enc);
 
 /* ids[B,S] int32 token ids, mask[B,S] int32 (1 keep / 0 pad; NULL = all ones), type_ids nullable (ignored by
- * AC_ARCH_MODERNBERT, whose RoPE positions are 0..S-1 for every sequence, padded or not).  S <= AC_ENCODER_MAX_S.
+ * AC_ARCH_MODERNBERT, whose RoPE positions are 0..S-1 for every sequence, padded or not).  S <= AC_ENCODER_MAX_S, or
+ * S <= max_pos for AC_ARCH_MODERNBERT.
  * out_unit_cls[B,H] = L2-normalised (eps 1e-12) CLS row of the last hidden state. */
 int ac_encoder_forward_cls(ac_encoder *enc, const int32_t *ids, const int32_t *mask,
                            const int32_t *type_ids, int B, int S, float *out_unit_cls,
