@@ -127,6 +127,13 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// per-thread register budget of the calling warpgroup (warpgroup-collective; N a multiple of 8 in [24, 256]).  inc blocks
+// until the CTA's pool has the registers, which other warpgroups return with dec.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // Shared-memory matrix descriptor, K-major operand in the canonical 128-byte-swizzled layout that TMA writes with
 // CU_TENSOR_MAP_SWIZZLE_128B (rows of 128 B, 8-row groups of 1024 B): start>>4 | LBO 1 (unused) | SBO 1024>>4 | SWIZZLE_128B.

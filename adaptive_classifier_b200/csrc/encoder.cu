@@ -87,11 +87,14 @@ struct EpiLinear {
     const float *__restrict__ rope;       // ROPE only: [S, 64] cos | sin per position
 
     static constexpr int kUnrollChunks = 4;   // `buf` must be a compile-time constant (register double buffer)
-    static constexpr int kPrefetchDist = 1;
+    // MODE 2 (linear_tc's residual, the CLS-only tail) requests each chunk's residual just before it is used: one residual
+    // buffer instead of two keeps the epilogue within its 160 registers
+    // MODE 2 (linear_tc's residual, the CLS-only tail) requests each chunk's residual right before the chunk: one buffer of
+    // 32 registers instead of two keeps its epilogue within the GEMM's 160 registers per thread
+    static constexpr int kPrefetchDist = (MODE == 2) ? 0 : 1;
     struct State {
-        // residual (MODE 2) of one 32-column chunk in the layout of the transposed phase: [column half][row pass],
-        // double-buffered so chunk c+1 is in flight while chunk c is processed
-        float4 res[(MODE == 2) ? 2 : 1][(MODE == 2) ? 8 : 1];
+        // residual (MODE 2) of one 32-column chunk in the layout of the transposed phase: [column half][row pass]
+        float4 res[1][(MODE == 2) ? 8 : 1];
         float mu, r;                      // DEFER: statistics of this thread's accumulator row
     };
     // accumulator + bias, or the deferred-LayerNorm form r (acc - mu c1) + c0
@@ -291,7 +294,6 @@ struct EpiResidDefer {
     static constexpr int kPrefetchDist = AC_RESID_PREFETCH;
     struct State {
         float4 res[kPrefetchDist + 1][8];  // old sums of 32-column chunks (transposed-phase layout), one buffer more than the distance
-        float2 ms[4];                      // (mu, r) of this lane's 4 rows (r8 + 8 i)
         float sum[4], sq[4];               // running partials of the new sums over this warp's GEMM_EPI_COLS columns
     };
     __device__ __forceinline__ bool skip_kernel() const { return false; }
@@ -304,8 +306,6 @@ struct EpiResidDefer {
         if (((col0 - ti.n0) & (GEMM_EPI_COLS - 1)) == 0) {              // first chunk of this warp's column half
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                const int grow = row_base + r8 + 8 * i;
-                st.ms[i] = (grow < M) ? __ldg(stats_prev + grow) : make_float2(0.f, 0.f);
                 st.sum[i] = 0.f;
                 st.sq[i] = 0.f;
             }
@@ -348,7 +348,8 @@ struct EpiResidDefer {
                 if (grow < M && col_ok) {
                     const float4 a = *reinterpret_cast<const float4 *>(stage + rr * GEMM_EPI_STAGE_ROW_BYTES + 16 * c);
                     const float4 rs = st.res[buf][half * 4 + i];             // old sums, requested one chunk ago
-                    const float mu = st.ms[i].x, r = st.ms[i].y;
+                    const float2 ms = __ldg(stats_prev + grow);             // (mu, r): re-read, not held across chunks
+                    const float mu = ms.x, r = ms.y;
                     float4 o;
                     o.x = (a.x + b4.x) + fmaf((rs.x - mu) * r, g4.x, e4.x);
                     o.y = (a.y + b4.y) + fmaf((rs.y - mu) * r, g4.y, e4.y);

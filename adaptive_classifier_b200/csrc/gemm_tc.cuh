@@ -5,14 +5,18 @@
 //       kKind = GEMM_KIND_F16  : fp16 values                         (wgmma .f16,  64 elements per 128-byte k-block)
 //   (same bytes per stage, same descriptors; fp16 has tf32's 10-bit mantissa at twice the tensor rate)
 //
-//   warpgroup 2 : TMA producer (one thread: cp.async.bulk.tensor.2d, 128B swizzle, 4-stage mbarrier ring)
-//   warpgroups 0, 1 : consumers.  Warpgroup g issues the wgmma m64n128 chain of tile rows [64 g, 64 g + 64) with the fp32
-//                 accumulator in registers, stores it into its half of a shared-memory accumulator tile, and then runs the
-//                 fused epilogue functor on it: warp w of the warpgroup drains rows 32 (2 g + w % 2) .. + 32 and the column
-//                 half w / 2 (64 columns = two chunks of 32), thread = one accumulator row.
+//   warpgroup 3 : TMA producer (one thread: cp.async.bulk.tensor.2d, 128B swizzle, 4-stage mbarrier ring)
+//   warpgroup 2 : MMA.  Issues both wgmma m64n128 chains of a 128 x 128 tile (rows 0-63 and 64-127, 2 x 64 fp32
+//                 accumulator registers per thread) and stores the finished accumulators into a shared-memory tile.
+//   warpgroups 0, 1 : epilogue.  Warpgroup g runs the fused epilogue functor on tile rows [64 g, 64 g + 64): warp w of the
+//                 warpgroup drains rows 32 (2 g + w % 2) .. + 32 and the column half w / 2 (64 columns = two chunks of
+//                 32), thread = one accumulator row.
 //
-// The two consumer warpgroups run independently (each waits only on its own rows), so one warpgroup's epilogue overlaps
-// the other's mainloop, and the producer keeps loading the next tile's stages during both.  This one kernel serves the
+// Hand-off through the single accumulator tile: the MMA warpgroup runs the mainloop of tile i, waits on acc_empty (the
+// epilogue of tile i-1 has read the tile for the last time), stores, arrives on acc_full and goes on with the mainloop of
+// tile i+1, so tile i's epilogue runs under tile i+1's mainloop.  The producer keeps loading stages throughout.  Registers:
+// 128 per thread at launch (512 threads); setmaxnreg moves them from the producer (24) to the MMA warpgroup (160: the 128
+// accumulators plus addressing; at 152 ptxas spills the accumulators) and the epilogue (160).  This one kernel serves the
 // encoder linears and the kNN scans (running per-query top-k' lists / threshold collection over prototype tiles).
 #pragma once
 #include "common.cuh"
@@ -26,9 +30,13 @@ constexpr int GEMM_KIND_TF32 = 0, GEMM_KIND_F16 = 1;
 __host__ __device__ constexpr int gemm_block_k(int kind) { return kind == GEMM_KIND_F16 ? 64 : 32; }
 constexpr int GEMM_STAGES = 4;
 constexpr int GEMM_EPI_COLS = GEMM_BLOCK_N / 2;     // accumulator columns one epilogue warp drains per tile
-constexpr int GEMM_EPI_WARPS = 8;                   // the consumer warps
-constexpr int GEMM_PRODUCER_THREAD = 32 * GEMM_EPI_WARPS;
-constexpr int GEMM_THREADS = 32 * GEMM_EPI_WARPS + 128; // 384: two consumer warpgroups + the producer warpgroup
+constexpr int GEMM_EPI_WARPS = 8;                   // the epilogue warps (threads 0-255)
+constexpr int GEMM_MMA_THREAD0 = 32 * GEMM_EPI_WARPS;   // first thread of the MMA warpgroup
+constexpr int GEMM_PRODUCER_THREAD = GEMM_MMA_THREAD0 + 128;
+constexpr int GEMM_THREADS = GEMM_PRODUCER_THREAD + 128; // 512: two epilogue warpgroups + MMA + producer
+// per-thread registers of each role after setmaxnreg: 128 * 24 + 128 * 160 + 256 * 160 = 64512 of 65536
+constexpr int GEMM_EPI_REGS = 160, GEMM_MMA_REGS = 160, GEMM_PRODUCER_REGS = 24;
+static_assert(128 * GEMM_PRODUCER_REGS + 128 * GEMM_MMA_REGS + 256 * GEMM_EPI_REGS <= 65536, "register split exceeds the file");
 constexpr int GEMM_A_STAGE_BYTES = GEMM_BLOCK_M * 128;  // 16 KB
 constexpr int GEMM_B_STAGE_BYTES = GEMM_BLOCK_N * 128;  // 16 KB
 constexpr int GEMM_STAGE_BYTES = GEMM_A_STAGE_BYTES + GEMM_B_STAGE_BYTES;
@@ -102,6 +110,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     uint64_t *bars = reinterpret_cast<uint64_t *>(epi_stage + GEMM_EPI_WARPS * GEMM_EPI_STAGE_BYTES);
     uint64_t *full_bar = bars;                        // [STAGES]
     uint64_t *empty_bar = bars + GEMM_STAGES;         // [STAGES]
+    uint64_t *acc_full = bars + 2 * GEMM_STAGES;      // accumulator tile stored (MMA -> epilogue)
+    uint64_t *acc_empty = acc_full + 1;               // accumulator tile read for the last time (epilogue -> MMA)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -110,20 +120,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const int num_tiles = tiles_m * tiles_n;
     constexpr int BK = gemm_block_k(kKind);            // elements per 128-byte k-block
     const int num_kb = (K + BK - 1) / BK;
+    // tiles blockIdx.x, blockIdx.x + gridDim.x, ... : the MMA and epilogue loops count them instead of carrying tile ids
+    const int my_tiles = (num_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
 
     if (threadIdx.x == GEMM_PRODUCER_THREAD) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_b);
         for (int s = 0; s < GEMM_STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], GEMM_EPI_WARPS);   // one arrival per consumer warp
+            mbar_init(&empty_bar[s], 4);                // one arrival per MMA warp
         }
+        mbar_init(acc_full, 128);                       // every MMA thread, after its own accumulator stores
+        mbar_init(acc_empty, 32 * GEMM_EPI_WARPS);      // every epilogue thread, after its last read of the tile
         fence_mbar_init();
     }
     __syncthreads();
 
     if (threadIdx.x >= GEMM_PRODUCER_THREAD) {
         // ---------------- TMA producer ----------------
+        setmaxnreg_dec<GEMM_PRODUCER_REGS>();          // the whole warpgroup, idle threads included
         if (threadIdx.x == GEMM_PRODUCER_THREAD) {
             int stage = 0;
             uint32_t phase = 0;
@@ -139,20 +154,71 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 }
             }
         }
-        return;     // no CTA-wide barrier follows: the consumers synchronise per warpgroup
+        return;     // no CTA-wide barrier follows: the other roles synchronise through mbarriers
     }
 
-    // ---------------- consumer warpgroups: wgmma mainloop, then the epilogue of their own 64 rows ----------------
+    if (threadIdx.x >= GEMM_MMA_THREAD0) {
+        // ---------------- MMA warpgroup: both 64-row wgmma chains of every tile, then the accumulator store ----------------
+        setmaxnreg_inc<GEMM_MMA_REGS>();
+        // the 128 accumulators leave 32 registers: keep the loop state small (a tile count instead of tile ids, stage
+        // descriptors as base + offset)
+        const uint64_t a_desc0 = wgmma_desc_sw128(smem_u32(smem_a));
+        const uint64_t b_desc0 = wgmma_desc_sw128(smem_u32(smem_b));
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int it = 0; it < my_tiles; ++it) {
+            float acc0[64], acc1[64];                // tile rows 0-63 and 64-127
+#pragma unroll
+            for (int j = 0; j < 64; ++j) { acc0[j] = 0.f; acc1[j] = 0.f; }
+            // one wgmma group stays in flight: the stage of k-block kb-1 is released once the group of kb has been issued
+            // and the group of kb-1 has retired
+            int prev_stage = -1;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait_guarded(&full_bar[stage], phase);
+                const uint64_t a_desc = a_desc0 + stage * (GEMM_A_STAGE_BYTES >> 4);
+                const uint64_t b_desc = b_desc0 + stage * (GEMM_B_STAGE_BYTES >> 4);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    // advance 32 bytes inside the 128B swizzle row: +2 in the (addr >> 4) field; rows 64-127 of the A
+                    // stage start 8192 B further: +512
+                    if (kKind == GEMM_KIND_F16) {
+                        wgmma_m64n128_f16(acc0, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                        wgmma_m64n128_f16(acc1, a_desc + 512 + 2 * k, b_desc + 2 * k, 1u);
+                    } else {
+                        wgmma_m64n128_tf32(acc0, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                        wgmma_m64n128_tf32(acc1, a_desc + 512 + 2 * k, b_desc + 2 * k, 1u);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                __syncwarp();
+                if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // this warp's share has been consumed
+                prev_stage = stage;
+                if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+            mbar_wait_guarded(acc_empty, (it & 1) ^ 1);  // the epilogue of tile it-1 is done with the accumulator tile
+            wgmma_store_acc(acc0, acc_tile, GEMM_ACC_LD);
+            wgmma_store_acc(acc1, acc_tile + 64 * GEMM_ACC_LD, GEMM_ACC_LD);
+            mbar_arrive(acc_full);                       // releases this thread's stores
+        }
+        return;
+    }
+
+    // ---------------- epilogue warpgroups: the fused epilogue of rows [64 wg, 64 wg + 64) of every tile ----------------
+    setmaxnreg_inc<GEMM_EPI_REGS>();
     const int wg = warp >> 2;                        // 0 or 1: tile rows [64 wg, 64 wg + 64)
     const int q = 2 * wg + (warp & 1);               // 32-row quarter of the tile this warp drains
     const int chalf = gemm_epi_chalf();
     typename Epi::State est;
     epi.begin_cta(est, q, lane);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
     const float *acc_row = acc_tile + (q * 32 + lane) * GEMM_ACC_LD;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+    for (int it = 0; it < my_tiles; ++it) {
+        const int tile = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
         GemmTileInfo ti;
         ti.m0 = (kMFastest ? tile % tiles_m : tile / tiles_n) * GEMM_BLOCK_M;
         ti.n0 = (kMFastest ? tile / tiles_m : tile % tiles_n) * GEMM_BLOCK_N;
@@ -160,43 +226,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         const int row = ti.m0 + q * 32 + lane;
         const int c_lo = chalf * GEMM_EPI_COLS;
         // operands the epilogue needs from global memory (residual rows) are requested kDist chunks ahead into kDist + 1
-        // register buffers; the first requests go out before the mainloop
+        // register buffers; the first requests go out while the tile's mainloop still runs
         constexpr int kDist = Epi::kPrefetchDist, kBufs = kDist + 1, kChunks = GEMM_EPI_COLS / 32;
 #pragma unroll
         for (int d = 0; d < kDist; ++d)
             if (d < kChunks) epi.prefetch(est, ti, row, ti.n0 + c_lo + 32 * d, lane, d % kBufs);
 
-        float acc[64];
-#pragma unroll
-        for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-        // one wgmma group stays in flight: the stage of k-block kb-1 is released once the group of kb has been issued and
-        // the group of kb-1 has retired
-        int prev_stage = -1;
-        for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait_guarded(&full_bar[stage], phase);
-            const uint64_t a_desc = wgmma_desc_sw128(smem_u32(smem_a + stage * GEMM_A_STAGE_BYTES + wg * 64 * 128));
-            const uint64_t b_desc = wgmma_desc_sw128(smem_u32(smem_b + stage * GEMM_B_STAGE_BYTES));
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                // advance 32 bytes inside the 128B swizzle row: +2 in the (addr >> 4) field
-                if (kKind == GEMM_KIND_F16) wgmma_m64n128_f16(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
-                else wgmma_m64n128_tf32(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait<1>();
-            __syncwarp();
-            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // this warp's share has been consumed
-            prev_stage = stage;
-            if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1; }
-        }
-        wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-
-        named_bar_sync(1 + wg, 128);                 // this warpgroup's epilogue of the previous tile is done reading
-        wgmma_store_acc(acc, acc_tile + wg * 64 * GEMM_ACC_LD, GEMM_ACC_LD);
-        named_bar_sync(1 + wg, 128);
+        mbar_wait_guarded(acc_full, it & 1);
 #pragma unroll (Epi::kUnrollChunks)
         for (int ci = 0; ci < kChunks; ++ci) {
             const int c = c_lo + 32 * ci;
@@ -205,6 +241,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
             acc_row_ld32(acc_row + c, v);
             epi.tile(est, ti, row, ti.n0 + c, v, epi_stage + warp * GEMM_EPI_STAGE_BYTES, lane, ci % kBufs, acc_row + c);
         }
+        mbar_arrive(acc_empty);                      // tile() re-reads acc (RoPE / GeGLU partners, kNN hits): only now done
     }
     epi.end_cta(est, q, lane);
 }
