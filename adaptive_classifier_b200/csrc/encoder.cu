@@ -14,9 +14,9 @@
 //   projections   wgmma GEMM of gemm_tc.cuh (.f16) with compile-time-specialised fused epilogues:
 //                 bias | bias+GELU(erf) | bias+residual, fp16 or fp32 output, V written TRANSPOSED per (sequence, head)
 //   attention     one CTA per (sequence, head): Q, K and V^T tiles by TMA, QK^T and PV as wgmma with the score tile
-//                 staged in shared memory, thread-per-query-row softmax in between (S <= 128; head_dim 64 or 32); 128-query
-//                 blocks over streamed key blocks for S <= 512, and for ModernBERT up to S = 8192 one pass with an online
-//                 softmax that visits only the key blocks inside a sliding layer's band (attention_stream_kernel)
+//                 staged in shared memory, thread-per-query-row softmax in between (S <= 128; head_dim 64 or 32); longer
+//                 sequences (up to 512, ModernBERT up to 8192) run 128-query blocks over streamed key blocks in one pass with
+//                 an online softmax that visits only the key blocks inside a sliding layer's band (attention_stream_kernel)
 //   LayerNorm     never materialised inside the layer stack: the residual epilogues keep the un-normalised sums y (fp32) and
 //                 per-row (sum, sumsq) partials, the consuming projections run on gamma-scaled weights and apply the
 //                 rank-1 correction r (acc - mu c1) + c0 in their epilogue ("deferred LayerNorm" below)
@@ -679,6 +679,30 @@ __device__ __forceinline__ uint32_t band_bits(int q, int k0, int w) {
     return up & dn;
 }
 
+// validity of keys [key0, key0 + 128) for query q (key < S, not padded, inside the band) as four 32-bit words held by
+// every thread: lane l of a warp tests key key0 + 32 w + l once and ballots; the softmax loops only test bits
+__device__ __forceinline__ void att_key_bits(const int32_t *mask, int64_t row0, int S, int key0, int q, int window, int lane,
+                                             uint32_t (&kmask)[4]) {
+#pragma unroll
+    for (int w4 = 0; w4 < 4; ++w4) {
+        const int key = key0 + 32 * w4 + lane;
+        const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
+        kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(q, key0 + 32 * w4, window);
+    }
+}
+// P = exp2(r scale_log2 - mxs) of 32 scores (0 where the key bit is clear) as 16 fp16 pairs into pk; sum += their total
+__device__ __forceinline__ void att_exp_pack(const float (&r)[32], uint32_t km, float scale_log2, float mxs, float &sum,
+                                             uint32_t *pk) {
+#pragma unroll
+    for (int j = 0; j < 32; j += 2) {
+        const float e0 = ((km >> j) & 1u) ? ex2_approx(fmaf(r[j], scale_log2, -mxs)) : 0.f;
+        const float e1 = ((km >> (j + 1)) & 1u) ? ex2_approx(fmaf(r[j + 1], scale_log2, -mxs)) : 0.f;
+        sum += e0 + e1;
+        __half2 hh = __floats2half2_rn(e0, e1);
+        pk[j >> 1] = *reinterpret_cast<uint32_t *>(&hh);
+    }
+}
+
 // window: ModernBERT sliding_attention half-window (keys |q - key| <= window), 0 = full attention
 template <int DH>
 __global__ void __launch_bounds__(ATT_THREADS)
@@ -735,15 +759,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     // ---- softmax: thread = query row, two passes over the 128 score columns
     const int qrow = warp * 32 + lane;
     const float *srow = sS + qrow * ATT_S_LD;
-    // key validity (key < S and not padded) as four 32-bit words held by every thread: lane l of a warp tests key
-    // 32*w + l once, ballots, and the loops below only test bits; the sliding-window band is per query row
     uint32_t kmask[4];
-#pragma unroll
-    for (int w4 = 0; w4 < 4; ++w4) {
-        const int key = 32 * w4 + lane;
-        const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
-        kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(qrow, 32 * w4, window);
-    }
+    att_key_bits(mask, row0, S, 0, qrow, window, lane, kmask);
     const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
     float mx = -CUDART_INF_F;
 #pragma unroll 1
@@ -761,16 +778,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     for (int ci = 0; ci < 4; ++ci) {
         float r[32];
         acc_row_ld32(srow + 32 * ci, r);
-        const uint32_t km = kmask[ci];
-        const float mxs = mx * scale_log2;
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-            const float e0 = ((km >> j) & 1u) ? ex2_approx(fmaf(r[j], scale_log2, -mxs)) : 0.f;
-            const float e1 = ((km >> (j + 1)) & 1u) ? ex2_approx(fmaf(r[j + 1], scale_log2, -mxs)) : 0.f;
-            sum += e0 + e1;
-            __half2 hh = __floats2half2_rn(e0, e1);
-            pk[16 * ci + (j >> 1)] = *reinterpret_cast<uint32_t *>(&hh);
-        }
+        att_exp_pack(r, kmask[ci], scale_log2, mx * scale_log2, sum, pk + 16 * ci);
     }
     __syncthreads();                       // every score row has been read
     const uint32_t sp_base = smem_u32(sP);
@@ -792,127 +800,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
 }
 
 // ------------------------------------------------------------------------------------------------
-// attention for 128 < S <= 512: one CTA per (sequence, head, 128-query block), key blocks of 128 streamed twice.
-//   pass A  row max over all key blocks        (QK^T only)
-//   pass B  P = exp(scale*(s - max)) per block, O += P V_block accumulated in the wgmma registers, row sums in registers
-// Using the final max in pass B means the accumulator never has to be rescaled; the price is computing QK^T
-// twice (QK^T is half of the attention flops, attention is a few % of the encoder).  Serial per block (TMA -> MMA ->
-// softmax -> MMA); the S <= 128 kernel above is the tuned path of the benchmark configurations.
-// ------------------------------------------------------------------------------------------------
-constexpr int ATTL_SMEM = 80 * 1024 + ATT_S_BYTES + 1024 + 64;
-
-template <int DH>
-__global__ void __launch_bounds__(ATT_THREADS)
-attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
-                      const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t *sQ = smem;                    // [128 x 128 B]
-    uint8_t *sK = smem + 16 * 1024;        // [128 x 128 B] current key block
-    uint8_t *sVt = smem + 32 * 1024;       // 2 slabs x [64 (d) x 128 B (64 keys)]
-    uint8_t *sP = smem + 48 * 1024;        // 2 slabs x [128 x 128 B (64 keys)]
-    float *sS = reinterpret_cast<float *>(smem + 80 * 1024);
-    uint64_t *bar_load = reinterpret_cast<uint64_t *>(smem + 80 * 1024 + ATT_S_BYTES);
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int b = blockIdx.x / heads, h = blockIdx.x % heads;
-    const int qb = blockIdx.y;                                   // query block
-    const int nkb = (S + 127) / 128;
-    const int64_t row0 = static_cast<int64_t>(b) * S;
-    const int vrow = (b * heads + h) * DH;
-
-    if (tid == 0) {
-        tma_prefetch_desc(&tmap_qk);
-        tma_prefetch_desc(&tmap_vt);
-        mbar_init(bar_load, 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
-    const int qrow = warp * 32 + lane;                            // row inside the query block
-    const int qglob = qb * 128 + qrow;                            // position inside the sequence
-    const float *srow = sS + qrow * ATT_S_LD;
-    const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
-
-    uint32_t ph_load = 0;
-    float mx = -CUDART_INF_F, sum = 0.f;
-    float o[2][DH / 2];
-
-    for (int pass = 0; pass < 2; ++pass) {
-        for (int j = 0; j < nkb; ++j) {
-            const int key0 = j * 128;
-            if (tid == 0) {
-                const bool first = (pass == 0 && j == 0);
-                const uint32_t bytes = (first ? 16 * 1024 : 0) + 16 * 1024 + (pass == 1 ? 16 * 1024 : 0);
-                mbar_arrive_expect_tx(bar_load, bytes);
-                if (first) tma_load_2d(sQ, &tmap_qk, bar_load, h * DH, static_cast<int>(row0) + qb * 128);
-                tma_load_2d(sK, &tmap_qk, bar_load, H + h * DH, static_cast<int>(row0) + key0);
-                if (pass == 1) {
-                    tma_load_2d(sVt, &tmap_vt, bar_load, key0, vrow);
-                    tma_load_2d(sVt + 8 * 1024, &tmap_vt, bar_load, key0 + 64, vrow);
-                }
-            }
-            mbar_wait_guarded(bar_load, ph_load);
-            ph_load ^= 1;
-            att_scores<DH>(sQ, sK, sS);
-            __syncthreads();
-
-            // key validity bits of this block
-            uint32_t kmask[4];
-#pragma unroll
-            for (int w4 = 0; w4 < 4; ++w4) {
-                const int key = key0 + 32 * w4 + lane;
-                const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
-                kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(qglob, key0 + 32 * w4, window);
-            }
-            if (pass == 0) {
-#pragma unroll
-                for (int ci = 0; ci < 4; ++ci) {
-                    float r[32];
-                    acc_row_ld32(srow + 32 * ci, r);
-                    const uint32_t km = kmask[ci];
-#pragma unroll
-                    for (int jj = 0; jj < 32; ++jj)
-                        if ((km >> jj) & 1u) mx = fmaxf(mx, r[jj]);
-                }
-                __syncthreads();                                  // the score tile and sK may be overwritten now
-            } else {
-                const uint32_t sp_base = smem_u32(sP);
-                const float mxs = mx * scale_log2;
-#pragma unroll
-                for (int ci = 0; ci < 4; ++ci) {
-                    const int c = 32 * ci;
-                    float r[32];
-                    acc_row_ld32(srow + c, r);
-                    const uint32_t km = kmask[ci];
-                    uint32_t pk[16];
-#pragma unroll
-                    for (int jj = 0; jj < 32; jj += 2) {
-                        const float e0 = ((km >> jj) & 1u) ? ex2_approx(fmaf(r[jj], scale_log2, -mxs)) : 0.f;
-                        const float e1 = ((km >> (jj + 1)) & 1u) ? ex2_approx(fmaf(r[jj + 1], scale_log2, -mxs)) : 0.f;
-                        sum += e0 + e1;
-                        __half2 hh = __floats2half2_rn(e0, e1);
-                        pk[jj >> 1] = *reinterpret_cast<uint32_t *>(&hh);
-                    }
-                    att_store_p(sp_base, qrow, c, pk);
-                }
-                fence_proxy_async_smem();
-                __syncthreads();
-                att_pv<DH>(sP, sVt, o, j != 0);
-                __syncthreads();                                  // sK / sVt / sP / the score tile are free again
-            }
-        }
-    }
-
-    wgmma_store_acc(o[0], sS, ATT_S_LD);
-    wgmma_store_acc(o[1], sS + 64 * ATT_S_LD, ATT_S_LD);
-    __syncthreads();
-    const float inv = (sum > 0.f) ? 1.f / sum : 0.f;
-    if (qglob < S) att_write_row<DH>(srow, inv, ctx + (row0 + qglob) * H + h * DH);
-}
-
-// ------------------------------------------------------------------------------------------------
-// attention for AC_ENCODER_MAX_S < S <= AC_MODERNBERT_MAX_S (ModernBERT, head_dim 64): one CTA per (sequence, head,
-// 128-query block), ONE pass over the key blocks with an online softmax.
+// attention for 128 < S <= AC_MODERNBERT_MAX_S, head_dim 64 or 32: one CTA per (sequence, head, 128-query block), ONE
+// pass over the key blocks with an online softmax.  BERT-family encoders pass window 0 and visit every key block.
 //   key blocks    full layers visit all ceil(S / 128); sliding layers only those intersecting [q0 - w, q0 + 127 + w]
 //                 (band_bits masks inside them), so a sliding layer costs O(S w) instead of O(S^2)
 //   ring          K and V^T blocks come through two TMA stages: block i + 1 loads while block i runs its MMAs and softmax
@@ -921,7 +810,7 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_
 //                 16 warp + lane / 4 (+ 8, + 64) through shared memory.  A row that has seen no valid key yet (the ends of
 //                 a sliding query block, holes in the mask) keeps m = -inf, P = 0 and a zero accumulator: the factor is
 //                 0 there rather than exp((-inf) - (-inf))
-//   P fp16, every accumulator fp32, as in the kernels above.  q_blocks = 1 (CLS-only tail next) computes rows 0..127 only.
+//   P fp16, every accumulator fp32, as in the kernel above.  q_blocks = 1 (CLS-only tail next) computes rows 0..127 only.
 // smem: Q 16 KB | K 2 x 16 KB | V^T 2 x 16 KB | P 32 KB | score tile 66 KB | factors 512 B | 2 barriers: one CTA per SM.
 // ------------------------------------------------------------------------------------------------
 constexpr int ATTS_STAGE_BYTES = 16 * 1024;
@@ -933,7 +822,6 @@ template <int DH>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
                         const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
-    static_assert(DH == 64, "S > 512 runs ModernBERT only (head_dim 64)");
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                              // [128 x 128 B]
@@ -999,12 +887,7 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         __syncthreads();
 
         uint32_t kmask[4];
-#pragma unroll
-        for (int w4 = 0; w4 < 4; ++w4) {
-            const int key = key0 + 32 * w4 + lane;
-            const bool ok = (key < S) && (!mask || mask[row0 + key] != 0);
-            kmask[w4] = __ballot_sync(0xffffffffu, ok) & band_bits(qglob, key0 + 32 * w4, window);
-        }
+        att_key_bits(mask, row0, S, key0, qglob, window, lane, kmask);
         float bmx = -CUDART_INF_F;
 #pragma unroll
         for (int ci = 0; ci < 4; ++ci) {
@@ -1022,16 +905,8 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         for (int ci = 0; ci < 4; ++ci) {
             float r[32];
             acc_row_ld32(srow + 32 * ci, r);
-            const uint32_t km = kmask[ci];
             uint32_t pk[16];
-#pragma unroll
-            for (int jj = 0; jj < 32; jj += 2) {
-                const float e0 = ((km >> jj) & 1u) ? ex2_approx(fmaf(r[jj], scale_log2, -mxs)) : 0.f;
-                const float e1 = ((km >> (jj + 1)) & 1u) ? ex2_approx(fmaf(r[jj + 1], scale_log2, -mxs)) : 0.f;
-                bsum += e0 + e1;
-                __half2 hh = __floats2half2_rn(e0, e1);
-                pk[jj >> 1] = *reinterpret_cast<uint32_t *>(&hh);
-            }
+            att_exp_pack(r, kmask[ci], scale_log2, mxs, bsum, pk);
             att_store_p(sp_base, qrow, 32 * ci, pk);
         }
         sum = fmaf(sum, alpha, bsum);
@@ -1143,19 +1018,28 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
     return AC_OK;
 }
 
-// S > AC_ENCODER_MAX_S (attention_stream_kernel): the queries of q_blocks 128-row blocks, each attending to the keys of its band
-static int launch_attention_stream(ac_encoder *e, const int32_t *mask, int B, int S, int window, int q_blocks, cudaStream_t s) {
+// softmax(Q K^T / sqrt(head_dim) + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention.
+// S <= 128 runs attention_kernel, longer sequences attention_stream_kernel over 128-query blocks.  cls_rows: only row 0 of
+// every sequence is read afterwards (the CLS-only tail), so only the first query block is computed.
+static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, cudaStream_t s) {
     const ac_encoder_config &c = e->cfg;
-    const int H = c.hidden, dh = H / c.heads;
-    AC_REQUIRE(dh == 64, "attention: S=%d > %d needs head_dim 64 (ModernBERT)", S, AC_ENCODER_MAX_S);
+    const int H = c.hidden;
+    const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create)
+    AC_REQUIRE(S <= AC_ENCODER_MAX_S || dh == 64, "attention: S=%d > %d needs head_dim 64 (ModernBERT)", S, AC_ENCODER_MAX_S);
+    // per-device: the attribute is a property of the (function, device) pair
     static bool att_attr[64] = {};
     int dev = 0;
     AC_CUDA(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !att_attr[dev]) {
+        AC_CUDA(cudaFuncSetAttribute(attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
         AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
         if (dev >= 0 && dev < 64) att_attr[dev] = true;
     }
-    // algorithmic flops over the keys each computed query attends to: (2w + 1) clipped to [0, S) in sliding layers
+    // algorithmic flops over the keys each computed query attends to at the true sequence length (the 128-wide tiles do
+    // more): (2w + 1) clipped to [0, S) in sliding layers
+    const int q_blocks = cls_rows ? 1 : (S + 127) / 128;
     const int nq = std::min(S, 128 * q_blocks);
     double keys = 0.0;
     if (window > 0) {
@@ -1164,41 +1048,13 @@ static int launch_attention_stream(ac_encoder *e, const int32_t *mask, int B, in
         keys = static_cast<double>(nq) * S;
     }
     const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * keys * dh, 0.0, s);
-    attention_stream_kernel<64><<<dim3(B * c.heads, q_blocks), ATT_THREADS, ATTS_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S,
-                                                                                          c.heads, H, window, e->ctx);
-    prof_end(slot, s);
-    AC_LAUNCH_CHECK();
-    return AC_OK;
-}
-
-// softmax(Q K^T / sqrt(head_dim) + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention.
-// cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail); S > AC_ENCODER_MAX_S then computes the first
-// query block only.
-static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, cudaStream_t s) {
-    if (S > AC_ENCODER_MAX_S) return launch_attention_stream(e, mask, B, S, window, cls_rows ? 1 : (S + 127) / 128, s);
-    const ac_encoder_config &c = e->cfg;
-    const int H = c.hidden;
-    const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create)
-    // per-device: the attribute is a property of the (function, device) pair
-    static bool att_attr[64] = {};
-    int dev = 0;
-    AC_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !att_attr[dev]) {
-        AC_CUDA(cudaFuncSetAttribute(attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_long_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTL_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_long_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTL_SMEM));
-        if (dev >= 0 && dev < 64) att_attr[dev] = true;
-    }
-    // algorithmic flops of softmax(QK^T)V at the true sequence length (the 128-wide tile does more)
-    const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * static_cast<double>(S) * S * dh, 0.0, s);
     if (S <= 128) {
         auto kern = dh == 32 ? attention_kernel<32> : attention_kernel<64>;
         kern<<<B * c.heads, ATT_THREADS, ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx);
     } else {
-        auto kern = dh == 32 ? attention_long_kernel<32> : attention_long_kernel<64>;
-        kern<<<dim3(B * c.heads, (S + 127) / 128), ATT_THREADS, ATTL_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H,
-                                                                               window, e->ctx);
+        auto kern = dh == 32 ? attention_stream_kernel<32> : attention_stream_kernel<64>;
+        kern<<<dim3(B * c.heads, q_blocks), ATT_THREADS, ATTS_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window,
+                                                                          e->ctx);
     }
     prof_end(slot, s);
     AC_LAUNCH_CHECK();

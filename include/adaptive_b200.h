@@ -248,7 +248,7 @@ enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2 };
 #define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts for BERT / RoBERTa / DistilBERT (their
                                   position tables stop at 512) */
 #define AC_MODERNBERT_MAX_S 8192   /* largest max_pos of an AC_ARCH_MODERNBERT encoder (max_position_embeddings of the
-                                      published checkpoints); S > AC_ENCODER_MAX_S runs the streamed attention kernel */
+                                      published checkpoints) */
 enum {
     AC_PREC_TF32 = 0,   /* wgmma .tf32 on fp32 storage (kNN coarse pass, ac_linear_tc tests) */
     AC_PREC_F16 = 1     /* wgmma .f16 with fp16 operands (RNE from fp32; same 10-bit mantissa as tf32),

@@ -63,7 +63,8 @@ def _check(out, ref):
 @pytest.mark.parametrize("cls_only", [True, False])
 def test_modernbert_tiny_matches_oracle(cabi, B, S, pad, cls_only):
     """hidden 128 / 2 heads, 4 layers (full, sliding, sliding, full), half-window 8: the band edge falls inside every
-    sequence; non-unit norm gammas; S <= 128 and 128 < S <= 512 attention kernels; padded batches"""
+    sequence; non-unit norm gammas; attention_kernel at S <= 128, attention_stream_kernel at 128 < S <= 512 (sliding layers
+    skip the key blocks outside the band); padded batches"""
     m = _model(7)
     ids, mask = _ids(B, S, 300, S + B, pad)
     ref, ref_hidden = _oracle(m, ids, mask)

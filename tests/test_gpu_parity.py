@@ -424,15 +424,18 @@ def _encoder(cabi, sd, cfg, max_tokens, cls_only=True, arch="bert"):
                         cls_only=cls_only)
 
 
-@pytest.mark.parametrize("B,S,pad", [(2, 300, True), (3, 129, False), (1, 512, False), (2, 384, True)])
+@pytest.mark.parametrize("B,S,pad", [(2, 300, True), (3, 129, False), (1, 512, False), (2, 384, True),
+                                     pytest.param(2, 384, (384, 90), id="2-384-masked_key_blocks")])
 def test_encoder_long_sequences(cabi, B, S, pad):
-    """128 < S <= 512 (the reference truncates at max_length = 512, classifier.py:1261): two-pass key-block attention"""
+    """128 < S <= 512 (the reference truncates at max_length = 512, classifier.py:1261): streamed key-block attention with
+    an online softmax.  pad True: sequence b ends 37 (b + 1) tokens early; a tuple gives the lengths, (384, 90) leaves key
+    blocks 1 and 2 of sequence 1 without a valid key"""
     sd, cfg = _small_bert(2)
     ids = eo.synthetic_ids(B, S)
     mask = torch.ones_like(ids)
     if pad:
         for b in range(B):
-            n = S - 37 * (b + 1)
+            n = pad[b] if isinstance(pad, tuple) else S - 37 * (b + 1)
             mask[b, n:] = 0
             ids[b, n:] = 0
     ref = eo.encoder_forward_cls(sd, ids, mask)
