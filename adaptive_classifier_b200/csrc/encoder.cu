@@ -24,6 +24,7 @@
 #include <cuda_fp16.h>
 #include <math_constants.h>
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 namespace ac {
@@ -56,71 +57,42 @@ __device__ __forceinline__ float gelu_erf(float y) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// fused epilogue of the encoder linears (compile-time specialised)
-//   MODE 0 bias, 1 bias + exact-erf GELU, 2 bias + fp32 residual;  OUT_HALF: fp16 output (next GEMM operand) or fp32
-//   VT: columns >= vt_col0 (the V third of the fused QKV projection) are written transposed to
-//       vT[(b*H + feature) * S_pad + key] so that attention can TMA-load V^T as a K-major B operand.
-// ------------------------------------------------------------------------------------------------
-//   DEFER: the A operand was the UN-normalised residual sum y (fp16) and the weights were packed as fp16(gamma * W):
-//       LayerNorm(y) W^T + b = r (acc - mu c1) + c0  with the row statistics (mu, r) of y, c1 = rowsum(W'), and
-//       `bias` holding c0 = W beta + b  (see "deferred LayerNorm" below)
-//   MODE 3 (GeGLU, ModernBERT's mlp.Wi): the weight rows were interleaved in 32-row groups by pack_defer_kernel, so a
-//       warp's 64-column slice holds [input cols 32 g .. 32 g + 31 | gate cols 32 g .. 32 g + 31]; the gate chunk re-reads
-//       the input chunk from the shared accumulator tile and writes fp16(GELU_erf(input) * gate) to columns 32 g.. of Y
-//       (N = 2 I accumulator columns, I output columns, ldy = I)
-//   ROPE (ModernBERT's Wqkv): columns < vt_col0 (the q and k thirds) are rotated in fp32 before the fp16 rounding,
-//       pairs (d, d + 32) of a head = the two 32-column chunks of one warp's slice; the partner is re-read from the
-//       accumulator tile.  Position = token index inside its sequence (row % S), table row = [cos(32) | sin(32)].
-template <int MODE, bool OUT_HALF, bool VT, bool DEFER = false, bool ROPE = false>
-struct EpiLinear {
-    static_assert(!DEFER || (OUT_HALF && MODE != 2), "the deferred-LayerNorm consumer epilogues write fp16 operands");
-    static_assert((MODE != 3 && !ROPE) || OUT_HALF, "the GeGLU / RoPE epilogues write fp16 operands");
-    const float *__restrict__ bias;       // [N]   (DEFER: c0)
-    const float *__restrict__ residual;   // [M, ldy] (MODE 2)
-    void *Y;                              // [M, ldy] fp16 or fp32
-    int M, N, ldy;
-    int round_out;                        // fp32 output only: round to tf32 (tests of the tf32 path)
-    __half *vT;                           // VT only
-    int vt_col0, S, S_pad, H;
-    const float *__restrict__ c1;         // DEFER only: [N] row sums of the packed weight
-    const float2 *__restrict__ row_stats; // DEFER only: [M] (mu, 1/sqrt(var + eps)) of the A rows
-    const float *__restrict__ rope;       // ROPE only: [S, 64] cos | sin per position
-
-    static constexpr int kUnrollChunks = 4;   // `buf` must be a compile-time constant (register double buffer)
-    // MODE 2 (linear_tc's residual, the CLS-only tail) requests each chunk's residual just before it is used: one residual
-    // buffer instead of two keeps the epilogue within its 160 registers
-    // MODE 2 (linear_tc's residual, the CLS-only tail) requests each chunk's residual right before the chunk: one buffer of
-    // 32 registers instead of two keeps its epilogue within the GEMM's 160 registers per thread
-    static constexpr int kPrefetchDist = (MODE == 2) ? 0 : 1;
-    struct State {
-        // residual (MODE 2) of one 32-column chunk in the layout of the transposed phase: [column half][row pass]
-        float4 res[1][(MODE == 2) ? 8 : 1];
-        float mu, r;                      // DEFER: statistics of this thread's accumulator row
-    };
-    // accumulator + bias, or the deferred-LayerNorm form r (acc - mu c1) + c0
-    __device__ __forceinline__ float pre(const State &st, float acc, float b, float c1v) const {
-        return DEFER ? fmaf(st.r, fmaf(-st.mu, c1v, acc), b) : acc + b;
-    }
+// fused epilogues of the encoder linears (gemm_tc.cuh's epilogue concept), one type per projection role.  A thread holds
+// one accumulator row; a warp's 32 rows leave through its staging tile as coalesced rows.  What they all share: the
+// whole grid runs, no per-CTA state, both chunks of a tile unrolled (`buf` must be a compile-time constant).
+struct EpiBase {
+    static constexpr int kUnrollChunks = 4;
     __device__ __forceinline__ bool skip_kernel() const { return false; }
-    __device__ __forceinline__ void begin_cta(State &, int, int) const {}
-    __device__ __forceinline__ void end_cta(State &, int, int) const {}
+    template <class State> __device__ __forceinline__ void begin_cta(State &, int, int) const {}
+    template <class State> __device__ __forceinline__ void end_cta(State &, int, int) const {}
+};
 
-    __device__ __forceinline__ float act(float y) const {
-        if (MODE == 1) y = gelu_erf(y);
-        return y;
-    }
+// one 16-column half of this thread's 32 accumulators into row `lane` of the warp's staging tile; afterwards lane
+// (r8 = lane / 4, c = lane % 4) reads the float4 of rows r8 + 8 i (i < 4) at byte 16 c
+__device__ __forceinline__ void stage_f32_half(const float (&v)[32], int half, uint8_t *stage, int lane) {
+    float4 *srow = reinterpret_cast<float4 *>(stage + lane * GEMM_EPI_STAGE_ROW_BYTES);
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+        srow[j] = make_float4(v[16 * half + 4 * j], v[16 * half + 4 * j + 1], v[16 * half + 4 * j + 2], v[16 * half + 4 * j + 3]);
+    __syncwarp();
+}
 
-    // transposed phase mapping (fp32 staging holds 16 columns at a time): lane = (r8 = lane / 4, c = lane % 4) handles
-    // rows r8 + 8*i (i < 4) and the 16-byte column group c of each 16-column half.
-    __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &ti, int row, int col0, int lane, int buf) const {
-        if (DEFER) {
-            if (((col0 - ti.n0) & (GEMM_EPI_COLS - 1)) == 0) {         // first chunk of this warp's column slice
-                const float2 ms = (row < M) ? __ldg(row_stats + row) : make_float2(0.f, 0.f);
-                st.mu = ms.x;
-                st.r = ms.y;
-            }
-        }
-        if (MODE != 2) return;
+__device__ __forceinline__ float gelu_if(bool on, float y) { return on ? gelu_erf(y) : y; }
+
+// fp32 output: bias, then GELU (exact erf) or + fp32 residual; round_out rounds to tf32 (tests of the tf32 path)
+template <bool GELU, bool RESID>
+struct EpiF32 : EpiBase {
+    const float *__restrict__ bias;       // [N]
+    const float *__restrict__ residual;   // RESID: [M, ldy]
+    float *Y;                             // [M, ldy]
+    int M, N, ldy;
+    int round_out = 0;
+    // RESID requests each chunk's residual right before the chunk: one buffer of 32 registers instead of two keeps the
+    // epilogue within the GEMM's 160 registers per thread
+    static constexpr int kPrefetchDist = 0;
+    struct State { float4 res[8]; };      // residual of one chunk: [column half][row pass], the staged layout
+    __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &, int row, int col0, int lane, int) const {
+        if (!RESID) return;
         const int row_base = row - lane;
         const int r8 = lane >> 2, c = lane & 3;
 #pragma unroll
@@ -129,135 +101,179 @@ struct EpiLinear {
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int grow = row_base + r8 + 8 * i;
-                st.res[buf][half * 4 + i] =
+                st.res[half * 4 + i] =
                     (grow < M && col + 4 <= N)
                         ? __ldg(reinterpret_cast<const float4 *>(residual + static_cast<int64_t>(grow) * ldy + col))
                         : make_float4(0, 0, 0, 0);
             }
         }
     }
-
-    __device__ __forceinline__ void tile(State &st, const GemmTileInfo &ti, int row, int col0, const float (&v)[32],
-                                         uint8_t *stage, int lane, int buf, const float *acc) const {
+    __device__ __forceinline__ void tile(State &st, const GemmTileInfo &, int row, int col0, const float (&v)[32], uint8_t *stage,
+                                         int lane, int, const float *) const {
         const int row_base = row - lane;                                     // first row of this warp's quarter
         if (row_base >= M || col0 >= N) return;                              // warp-uniform
-        if (VT && col0 >= vt_col0) {
-            // thread = token row: lanes hold 32 consecutive keys of (mostly) one sequence -> 64-byte coalesced stores
-            if (row < M) {
-                const int b = row / S, key = row - b * S;
-                __half *dst = vT + (static_cast<int64_t>(b) * H + (col0 - vt_col0)) * S_pad + key;
+        const int r8 = lane >> 2, c = lane & 3;
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 b4 = __ldg(reinterpret_cast<const float4 *>(bias + col0 + j));
-                    const float4 c4 = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + col0 + j)) : make_float4(0, 0, 0, 0);
-                    dst[static_cast<int64_t>(j) * S_pad] = __float2half_rn(pre(st, v[j], b4.x, c4.x));
-                    dst[static_cast<int64_t>(j + 1) * S_pad] = __float2half_rn(pre(st, v[j + 1], b4.y, c4.y));
-                    dst[static_cast<int64_t>(j + 2) * S_pad] = __float2half_rn(pre(st, v[j + 2], b4.z, c4.z));
-                    dst[static_cast<int64_t>(j + 3) * S_pad] = __float2half_rn(pre(st, v[j + 3], b4.w, c4.w));
-                }
-            }
-            return;
-        }
-        if (OUT_HALF) {
-            if (MODE == 3 && (col0 & 32) == 0) return;                      // input chunk: consumed by its gate chunk
-            const int ocol0 = MODE == 3 ? (col0 - 32) / 2 : col0, oN = MODE == 3 ? N / 2 : N;
-            const bool rot = ROPE && col0 < vt_col0;
-            const int pofs = (col0 & 32) ? -32 : 32;                         // partner chunk (RoPE half / GeGLU input)
-            const float *rrow = ROPE ? rope + static_cast<int64_t>(row < M ? row % S : 0) * 64 : nullptr;
-            // stage 32 rows x 32 halves (64 B payload per 80-byte row), then lane (r4 = lane/4 .. 8 rows per pass, c8 = lane%4)
-            uint4 *srow = reinterpret_cast<uint4 *>(stage + lane * GEMM_EPI_STAGE_ROW_BYTES);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float4 ba = __ldg(reinterpret_cast<const float4 *>(bias + col0 + 8 * j));
-                const float4 bb = __ldg(reinterpret_cast<const float4 *>(bias + col0 + 8 * j + 4));
-                const float4 ca = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + col0 + 8 * j)) : make_float4(0, 0, 0, 0);
-                const float4 cb = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + col0 + 8 * j + 4)) : make_float4(0, 0, 0, 0);
-                float y[8];
-                y[0] = act(pre(st, v[8 * j], ba.x, ca.x)); y[1] = act(pre(st, v[8 * j + 1], ba.y, ca.y));
-                y[2] = act(pre(st, v[8 * j + 2], ba.z, ca.z)); y[3] = act(pre(st, v[8 * j + 3], ba.w, ca.w));
-                y[4] = act(pre(st, v[8 * j + 4], bb.x, cb.x)); y[5] = act(pre(st, v[8 * j + 5], bb.y, cb.y));
-                y[6] = act(pre(st, v[8 * j + 6], bb.z, cb.z)); y[7] = act(pre(st, v[8 * j + 7], bb.w, cb.w));
-                if (MODE == 3 || rot) {
-                    const int pc = col0 + pofs + 8 * j;
-                    const float4 a0 = *reinterpret_cast<const float4 *>(acc + pofs + 8 * j);
-                    const float4 a1 = *reinterpret_cast<const float4 *>(acc + pofs + 8 * j + 4);
-                    const float4 pba = __ldg(reinterpret_cast<const float4 *>(bias + pc));
-                    const float4 pbb = __ldg(reinterpret_cast<const float4 *>(bias + pc + 4));
-                    const float4 pca = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + pc)) : make_float4(0, 0, 0, 0);
-                    const float4 pcb = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + pc + 4)) : make_float4(0, 0, 0, 0);
-                    float p[8];
-                    p[0] = pre(st, a0.x, pba.x, pca.x); p[1] = pre(st, a0.y, pba.y, pca.y);
-                    p[2] = pre(st, a0.z, pba.z, pca.z); p[3] = pre(st, a0.w, pba.w, pca.w);
-                    p[4] = pre(st, a1.x, pbb.x, pcb.x); p[5] = pre(st, a1.y, pbb.y, pcb.y);
-                    p[6] = pre(st, a1.z, pbb.z, pcb.z); p[7] = pre(st, a1.w, pbb.w, pcb.w);
-                    if (MODE == 3) {
-#pragma unroll
-                        for (int k = 0; k < 8; ++k) y[k] = gelu_erf(p[k]) * y[k];          // y = gate, p = input
-                    } else {
-                        // HF apply_rotary_pos_emb: x cos + rotate_half(x) sin, rotate_half = (-x[32:], x[:32])
-                        const float4 c0v = __ldg(reinterpret_cast<const float4 *>(rrow + 8 * j));
-                        const float4 c1v = __ldg(reinterpret_cast<const float4 *>(rrow + 8 * j + 4));
-                        const float4 s0v = __ldg(reinterpret_cast<const float4 *>(rrow + 32 + 8 * j));
-                        const float4 s1v = __ldg(reinterpret_cast<const float4 *>(rrow + 32 + 8 * j + 4));
-                        const float cs[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
-                        const float sn[8] = {s0v.x, s0v.y, s0v.z, s0v.w, s1v.x, s1v.y, s1v.z, s1v.w};
-                        const float sg = (col0 & 32) ? 1.f : -1.f;
-#pragma unroll
-                        for (int k = 0; k < 8; ++k) y[k] = __fadd_rn(__fmul_rn(y[k], cs[k]), __fmul_rn(sg * p[k], sn[k]));
-                    }
-                }
-                uint4 pk;
-                __half2 h0 = __floats2half2_rn(y[0], y[1]), h1 = __floats2half2_rn(y[2], y[3]);
-                __half2 h2 = __floats2half2_rn(y[4], y[5]), h3 = __floats2half2_rn(y[6], y[7]);
-                pk.x = *reinterpret_cast<uint32_t *>(&h0); pk.y = *reinterpret_cast<uint32_t *>(&h1);
-                pk.z = *reinterpret_cast<uint32_t *>(&h2); pk.w = *reinterpret_cast<uint32_t *>(&h3);
-                srow[j] = pk;
-            }
-            __syncwarp();
-            const int r8 = lane >> 2, c = lane & 3;                           // 8 rows x 4 x 16 B per pass
-            __half *Yh = static_cast<__half *>(Y);
+        for (int half = 0; half < 2; ++half) {
+            const int col = col0 + 16 * half + 4 * c;
+            stage_f32_half(v, half, stage, lane);
+            const float4 b4 = (col + 4 <= N) ? __ldg(reinterpret_cast<const float4 *>(bias + col)) : make_float4(0, 0, 0, 0);
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int rr = r8 + 8 * i;
                 const int grow = row_base + rr;
-                const int col = ocol0 + 8 * c;
-                if (grow < M && col + 8 <= oN) {
-                    const uint4 pk = *reinterpret_cast<const uint4 *>(stage + rr * GEMM_EPI_STAGE_ROW_BYTES + 16 * c);
-                    *reinterpret_cast<uint4 *>(Yh + static_cast<int64_t>(grow) * ldy + col) = pk;
+                if (grow < M && col + 4 <= N) {
+                    const float4 a = *reinterpret_cast<const float4 *>(stage + rr * GEMM_EPI_STAGE_ROW_BYTES + 16 * c);
+                    float4 o;
+                    o.x = gelu_if(GELU, a.x + b4.x); o.y = gelu_if(GELU, a.y + b4.y);
+                    o.z = gelu_if(GELU, a.z + b4.z); o.w = gelu_if(GELU, a.w + b4.w);
+                    if (RESID) {
+                        const float4 rs = st.res[half * 4 + i];                 // requested before the chunk
+                        o.x += rs.x; o.y += rs.y; o.z += rs.z; o.w += rs.w;
+                    }
+                    if (round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
+                    *reinterpret_cast<float4 *>(Y + static_cast<int64_t>(grow) * ldy + col) = o;
                 }
             }
             __syncwarp();
-        } else {
-            // fp32 output (pre-LayerNorm sums): two passes of 16 columns through the staging tile
-            float *Yf = static_cast<float *>(Y);
-            const int r8 = lane >> 2, c = lane & 3;
+        }
+    }
+};
+
+// fp16 output, the next GEMM's A operand: pre-activation acc + bias, or with DEFER the deferred-LayerNorm form below, then
+//   Act::Gelu   exact-erf GELU
+//   Act::GeGLU  (ModernBERT's mlp.Wi) pack_defer_kernel interleaved the weight rows in 32-row groups, so a warp's slice
+//               holds [input cols 32 g .. + 31 | gate cols 32 g .. + 31]; the gate chunk re-reads the input chunk from the
+//               accumulator tile and writes fp16(GELU_erf(input) * gate) to columns 32 g.. of Y (N = 2 I, ldy = I)
+//   Act::Rope   (q and k of ModernBERT's Wqkv) rotated in fp32 before the fp16 rounding: the pair (d, d + 32) of a head is
+//               the two chunks of a warp's slice, the partner re-read from the accumulator tile; position = row % S
+// DEFER: the A operand was the UN-normalised residual sum y (fp16) and the weights were packed as fp16(gamma * W):
+//   LayerNorm(y) W^T + b = r (acc - mu c1) + c0  with the row statistics (mu, r) of y, c1 = rowsum(W'), and `bias`
+//   holding c0 = W beta + b  (producer side: EpiResidDefer)
+enum class Act { None, Gelu, GeGLU, Rope };
+template <Act ACT, bool DEFER>
+struct EpiF16 : EpiBase {
+    const float *__restrict__ bias;       // [N]   (DEFER: c0)
+    const float *__restrict__ c1;         // DEFER: [N] row sums of the packed weight
+    const float2 *__restrict__ row_stats; // DEFER: [M] (mu, 1/sqrt(var + eps)) of the A rows
+    __half *Y;                            // [M, ldy]
+    int M, N, ldy;
+    int S;                                // Act::Rope, EpiQKV: tokens per sequence
+    const float *__restrict__ rope;       // Act::Rope: [S, 64] cos | sin per position
+    static constexpr int kPrefetchDist = 1;   // DEFER: the row statistics are requested before the accumulators arrive
+    struct State { float mu, r; };            // DEFER: statistics of this thread's accumulator row
+    __device__ __forceinline__ float pre(const State &st, float acc, float b, float c1v) const {
+        return DEFER ? fmaf(st.r, fmaf(-st.mu, c1v, acc), b) : acc + b;
+    }
+    __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &ti, int row, int col0, int, int) const {
+        if (DEFER && ((col0 - ti.n0) & (GEMM_EPI_COLS - 1)) == 0) {    // first chunk of this warp's column slice
+            const float2 ms = (row < M) ? __ldg(row_stats + row) : make_float2(0.f, 0.f);
+            st.mu = ms.x, st.r = ms.y;
+        }
+    }
+    __device__ __forceinline__ void tile(State &st, const GemmTileInfo &, int row, int col0, const float (&v)[32], uint8_t *stage,
+                                         int lane, int, const float *acc) const {
+        const int row_base = row - lane;                                     // first row of this warp's quarter
+        if (row_base >= M || col0 >= N) return;                              // warp-uniform
+        constexpr bool GLU = ACT == Act::GeGLU, ROT = ACT == Act::Rope;
+        if (GLU && (col0 & 32) == 0) return;                                 // input chunk: consumed by its gate chunk
+        const int ocol0 = GLU ? (col0 - 32) / 2 : col0, oN = GLU ? N / 2 : N;
+        const int pofs = (col0 & 32) ? -32 : 32;                             // partner chunk (RoPE half / GeGLU input)
+        const float *rrow = ROT ? rope + static_cast<int64_t>(row < M ? row % S : 0) * 64 : nullptr;
+        // stage 32 rows x 32 halves (64 B payload per 80-byte row), then lane (r4 = lane/4 .. 8 rows per pass, c8 = lane%4)
+        uint4 *srow = reinterpret_cast<uint4 *>(stage + lane * GEMM_EPI_STAGE_ROW_BYTES);
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                const int col = col0 + 16 * half + 4 * c;
-                float4 *srow = reinterpret_cast<float4 *>(stage + lane * GEMM_EPI_STAGE_ROW_BYTES);
+        for (int j = 0; j < 4; ++j) {
+            const float4 ba = __ldg(reinterpret_cast<const float4 *>(bias + col0 + 8 * j));
+            const float4 bb = __ldg(reinterpret_cast<const float4 *>(bias + col0 + 8 * j + 4));
+            const float4 ca = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + col0 + 8 * j)) : make_float4(0, 0, 0, 0);
+            const float4 cb = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + col0 + 8 * j + 4)) : make_float4(0, 0, 0, 0);
+            constexpr bool G = ACT == Act::Gelu;
+            float y[8];
+            y[0] = gelu_if(G, pre(st, v[8 * j], ba.x, ca.x)); y[1] = gelu_if(G, pre(st, v[8 * j + 1], ba.y, ca.y));
+            y[2] = gelu_if(G, pre(st, v[8 * j + 2], ba.z, ca.z)); y[3] = gelu_if(G, pre(st, v[8 * j + 3], ba.w, ca.w));
+            y[4] = gelu_if(G, pre(st, v[8 * j + 4], bb.x, cb.x)); y[5] = gelu_if(G, pre(st, v[8 * j + 5], bb.y, cb.y));
+            y[6] = gelu_if(G, pre(st, v[8 * j + 6], bb.z, cb.z)); y[7] = gelu_if(G, pre(st, v[8 * j + 7], bb.w, cb.w));
+            if (GLU || ROT) {
+                const int pc = col0 + pofs + 8 * j;
+                const float4 a0 = *reinterpret_cast<const float4 *>(acc + pofs + 8 * j);
+                const float4 a1 = *reinterpret_cast<const float4 *>(acc + pofs + 8 * j + 4);
+                const float4 pba = __ldg(reinterpret_cast<const float4 *>(bias + pc));
+                const float4 pbb = __ldg(reinterpret_cast<const float4 *>(bias + pc + 4));
+                const float4 pca = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + pc)) : make_float4(0, 0, 0, 0);
+                const float4 pcb = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + pc + 4)) : make_float4(0, 0, 0, 0);
+                float p[8];
+                p[0] = pre(st, a0.x, pba.x, pca.x); p[1] = pre(st, a0.y, pba.y, pca.y);
+                p[2] = pre(st, a0.z, pba.z, pca.z); p[3] = pre(st, a0.w, pba.w, pca.w);
+                p[4] = pre(st, a1.x, pbb.x, pcb.x); p[5] = pre(st, a1.y, pbb.y, pcb.y);
+                p[6] = pre(st, a1.z, pbb.z, pcb.z); p[7] = pre(st, a1.w, pbb.w, pcb.w);
+                if (GLU) {
 #pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    srow[j] = make_float4(v[16 * half + 4 * j], v[16 * half + 4 * j + 1], v[16 * half + 4 * j + 2],
-                                          v[16 * half + 4 * j + 3]);
-                __syncwarp();
-                const float4 b4 = (col + 4 <= N) ? __ldg(reinterpret_cast<const float4 *>(bias + col)) : make_float4(0, 0, 0, 0);
+                    for (int k = 0; k < 8; ++k) y[k] = gelu_erf(p[k]) * y[k];          // y = gate, p = input
+                } else {
+                    // HF apply_rotary_pos_emb: x cos + rotate_half(x) sin, rotate_half = (-x[32:], x[:32])
+                    const float4 c0v = __ldg(reinterpret_cast<const float4 *>(rrow + 8 * j));
+                    const float4 c1v = __ldg(reinterpret_cast<const float4 *>(rrow + 8 * j + 4));
+                    const float4 s0v = __ldg(reinterpret_cast<const float4 *>(rrow + 32 + 8 * j));
+                    const float4 s1v = __ldg(reinterpret_cast<const float4 *>(rrow + 32 + 8 * j + 4));
+                    const float cs[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
+                    const float sn[8] = {s0v.x, s0v.y, s0v.z, s0v.w, s1v.x, s1v.y, s1v.z, s1v.w};
+                    const float sg = (col0 & 32) ? 1.f : -1.f;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int rr = r8 + 8 * i;
-                    const int grow = row_base + rr;
-                    if (grow < M && col + 4 <= N) {
-                        const float4 a = *reinterpret_cast<const float4 *>(stage + rr * GEMM_EPI_STAGE_ROW_BYTES + 16 * c);
-                        float4 o;
-                        o.x = act(a.x + b4.x); o.y = act(a.y + b4.y); o.z = act(a.z + b4.z); o.w = act(a.w + b4.w);
-                        if (MODE == 2) {
-                            const float4 rs = st.res[buf][half * 4 + i];    // requested one chunk ago
-                            o.x += rs.x; o.y += rs.y; o.z += rs.z; o.w += rs.w;
-                        }
-                        if (round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                        *reinterpret_cast<float4 *>(Yf + static_cast<int64_t>(grow) * ldy + col) = o;
-                    }
+                    for (int k = 0; k < 8; ++k) y[k] = __fadd_rn(__fmul_rn(y[k], cs[k]), __fmul_rn(sg * p[k], sn[k]));
                 }
-                __syncwarp();
+            }
+            uint4 pk;
+            __half2 h0 = __floats2half2_rn(y[0], y[1]), h1 = __floats2half2_rn(y[2], y[3]);
+            __half2 h2 = __floats2half2_rn(y[4], y[5]), h3 = __floats2half2_rn(y[6], y[7]);
+            pk.x = *reinterpret_cast<uint32_t *>(&h0); pk.y = *reinterpret_cast<uint32_t *>(&h1);
+            pk.z = *reinterpret_cast<uint32_t *>(&h2); pk.w = *reinterpret_cast<uint32_t *>(&h3);
+            srow[j] = pk;
+        }
+        __syncwarp();
+        const int r8 = lane >> 2, c = lane & 3;                               // 8 rows x 4 x 16 B per pass
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int rr = r8 + 8 * i;
+            const int grow = row_base + rr;
+            const int col = ocol0 + 8 * c;
+            if (grow < M && col + 8 <= oN) {
+                const uint4 pk = *reinterpret_cast<const uint4 *>(stage + rr * GEMM_EPI_STAGE_ROW_BYTES + 16 * c);
+                *reinterpret_cast<uint4 *>(Y + static_cast<int64_t>(grow) * ldy + col) = pk;
+            }
+        }
+        __syncwarp();
+    }
+};
+
+// fused QKV, a deferred-LayerNorm consumer: q and k (columns < vt_col0) are EpiF16 rows (ModernBERT: RoPE); V is written
+// transposed to vT[(b*H + feature) * S_pad + key] so that attention can TMA-load V^T as a K-major B operand.
+template <bool ROPE>
+struct EpiQKV : EpiBase {
+    EpiF16<ROPE ? Act::Rope : Act::None, true> qk;   // N = 3 H accumulator columns, Y = [M, 2 H] q | k
+    __half *vT;
+    int vt_col0, S_pad, H;
+    static constexpr int kPrefetchDist = 1;
+    using State = typename decltype(qk)::State;
+    __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &ti, int row, int col0, int lane, int buf) const {
+        qk.prefetch(st, ti, row, col0, lane, buf);
+    }
+    __device__ __forceinline__ void tile(State &st, const GemmTileInfo &ti, int row, int col0, const float (&v)[32],
+                                         uint8_t *stage, int lane, int buf, const float *acc) const {
+        if (row - lane >= qk.M || col0 >= qk.N) return;                     // warp-uniform
+        if (col0 < vt_col0) return qk.tile(st, ti, row, col0, v, stage, lane, buf, acc);
+        // thread = token row: lanes hold 32 consecutive keys of (mostly) one sequence -> 64-byte coalesced stores
+        if (row < qk.M) {
+            const int b = row / qk.S, key = row - b * qk.S;
+            __half *dst = vT + (static_cast<int64_t>(b) * H + (col0 - vt_col0)) * S_pad + key;
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+                const float4 b4 = __ldg(reinterpret_cast<const float4 *>(qk.bias + col0 + j));
+                const float4 c4 = __ldg(reinterpret_cast<const float4 *>(qk.c1 + col0 + j));
+                dst[static_cast<int64_t>(j) * S_pad] = __float2half_rn(qk.pre(st, v[j], b4.x, c4.x));
+                dst[static_cast<int64_t>(j + 1) * S_pad] = __float2half_rn(qk.pre(st, v[j + 1], b4.y, c4.y));
+                dst[static_cast<int64_t>(j + 2) * S_pad] = __float2half_rn(qk.pre(st, v[j + 2], b4.z, c4.z));
+                dst[static_cast<int64_t>(j + 3) * S_pad] = __float2half_rn(qk.pre(st, v[j + 3], b4.w, c4.w));
             }
         }
     }
@@ -265,16 +281,15 @@ struct EpiLinear {
 
 // ------------------------------------------------------------------------------------------------
 // deferred LayerNorm: residual epilogue that never materialises LayerNorm
-//
 //   y_new = acc + bias + LN_prev(y_old)          LN_prev(y) = (y - mu) r gamma + beta recomputed from the fp32 y_old, its
 //                                                row statistics and the pending LayerNorm's parameters
 //   writes y_new (fp32, IN PLACE over y_old: every element is read and written by the same thread), fp16(y_new) (the
-//   next GEMM's A operand, consumed through EpiLinear<.., DEFER = true>) and per-row partial (sum, sum of squares) of
+//   next GEMM's A operand, consumed through EpiF16<.., DEFER = true>) and per-row partial (sum, sum of squares) of
 //   this warp's GEMM_EPI_COLS columns into parts[column part][row]; ln_stats_kernel turns the parts into (mu, r).
 //   HBM traffic per half layer at B*S = 65536, H = 768: read y 201 MB, write y 201 MB + fp16 101 MB = 503 MB instead of
 //   905 MB (GEMM epilogue 402 MB + LayerNorm kernel 503 MB); precision: oracle/deferred_ln_study.py (CPU emulation) and tests/test_gpu_parity.py (non-trivial gamma / beta).
 // ------------------------------------------------------------------------------------------------
-struct EpiResidDefer {
+struct EpiResidDefer : EpiBase {
     const float *__restrict__ bias;        // [N]
     float *y;                              // [M, ld] fp32 residual sums: read (old) and written (new) in place
     __half *yh;                            // [M, ld] fp16 copy of the new sums
@@ -284,31 +299,19 @@ struct EpiResidDefer {
     float2 *parts;                         // [N / GEMM_EPI_COLS][part_stride] partial (sum, sumsq) of the new sums
     int64_t part_stride;
     int M, N, ld;
-
-    static constexpr int kUnrollChunks = 4;
     // The residual epilogues are HBM-bound (fp32 sums read + written, fp16 copy written per element).  The old sums of the
     // next 32-column chunk are requested one chunk ahead; a larger distance needs one more 32-register buffer per thread.
-#ifndef AC_RESID_PREFETCH
-#define AC_RESID_PREFETCH 1
-#endif
-    static constexpr int kPrefetchDist = AC_RESID_PREFETCH;
+    static constexpr int kPrefetchDist = 1;
     struct State {
         float4 res[kPrefetchDist + 1][8];  // old sums of 32-column chunks (transposed-phase layout), one buffer more than the distance
         float sum[4], sq[4];               // running partials of the new sums over this warp's GEMM_EPI_COLS columns
     };
-    __device__ __forceinline__ bool skip_kernel() const { return false; }
-    __device__ __forceinline__ void begin_cta(State &, int, int) const {}
-    __device__ __forceinline__ void end_cta(State &, int, int) const {}
-
     __device__ __forceinline__ void prefetch(State &st, const GemmTileInfo &ti, int row, int col0, int lane, int buf) const {
         const int row_base = row - lane;
         const int r8 = lane >> 2, c = lane & 3;
         if (((col0 - ti.n0) & (GEMM_EPI_COLS - 1)) == 0) {              // first chunk of this warp's column half
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                st.sum[i] = 0.f;
-                st.sq[i] = 0.f;
-            }
+            for (int i = 0; i < 4; ++i) st.sum[i] = st.sq[i] = 0.f;
         }
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -323,7 +326,6 @@ struct EpiResidDefer {
             }
         }
     }
-
     __device__ __forceinline__ void tile(State &st, const GemmTileInfo &ti, int row, int col0, const float (&v)[32], uint8_t *stage,
                                          int lane, int buf, const float *) const {
         const int row_base = row - lane;
@@ -332,11 +334,7 @@ struct EpiResidDefer {
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
             const int col = col0 + 16 * half + 4 * c;
-            float4 *srow = reinterpret_cast<float4 *>(stage + lane * GEMM_EPI_STAGE_ROW_BYTES);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-                srow[j] = make_float4(v[16 * half + 4 * j], v[16 * half + 4 * j + 1], v[16 * half + 4 * j + 2], v[16 * half + 4 * j + 3]);
-            __syncwarp();
+            stage_f32_half(v, half, stage, lane);
             const bool col_ok = col + 4 <= N;
             const float4 b4 = col_ok ? __ldg(reinterpret_cast<const float4 *>(bias + col)) : make_float4(0, 0, 0, 0);
             const float4 g4 = col_ok ? __ldg(reinterpret_cast<const float4 *>(gamma + col)) : make_float4(0, 0, 0, 0);
@@ -414,7 +412,7 @@ __global__ void fill_value_kernel(float *__restrict__ p, int n, float v) {
 //   Wp[n,k] = fp16(gamma[k] W[n,k]),  c1[n] = sum_k Wp[n,k] (fp32),  c0[n] = sum_k beta[k] W[n,k] + bias[n]
 // gamma / beta NULL = identity LayerNorm (layer 0 consumes the already normalised embeddings), bias NULL = 0.
 // glu != 0 (GeGLU weight [2I, H], N = 2I): packed row n takes source row (n / 64) 32 + n % 32 of the input half for
-// n % 64 < 32, the same row of the gate half otherwise -- the row order EpiLinear<3, ..> expects
+// n % 64 < 32, the same row of the gate half otherwise -- the row order EpiF16<Act::GeGLU, ..> expects
 __global__ void pack_defer_kernel(const float *__restrict__ W, const float *__restrict__ bias, const float *__restrict__ gamma,
                                   const float *__restrict__ beta, int N, int K, __half *__restrict__ Wp, float *__restrict__ c1,
                                   float *__restrict__ c0, int glu = 0) {
@@ -1267,10 +1265,9 @@ static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, in
 template <bool PRE_LN>
 static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids, int B, int S,
                           float *out_unit_cls, cudaStream_t s) {
-    using EpiQKV = EpiLinear<0, true, true, true, PRE_LN>;          // r (acc - mu c1) + c0 (+ RoPE on q, k), V third transposed
-    using EpiFfn1 = EpiLinear<PRE_LN ? 3 : 1, true, false, true>;   // GELU, or GeGLU input * gate, of r (acc - mu c1) + c0
-    using EpiFfn1Rows = EpiLinear<PRE_LN ? 3 : 1, true, false>;     // the same on materialised LayerNorm rows (CLS-only tail)
-    using EpiResid = EpiLinear<2, false, false>;                    // bias + residual, fp32 out (CLS-only tail)
+    constexpr Act kFfnAct = PRE_LN ? Act::GeGLU : Act::Gelu;        // GeGLU input * gate, or GELU
+    using EpiFfn1 = EpiF16<kFfnAct, true>;
+    using EpiFfn1Rows = EpiF16<kFfnAct, false>;                     // on materialised LayerNorm rows (CLS-only tail)
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden, I = c.intermediate, M = B * S;
     const int N1 = PRE_LN ? 2 * I : I;                              // FFN1 accumulator columns (GeGLU: input + gate)
@@ -1290,21 +1287,24 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
     const float *pg = e->ones, *pb = e->zeros;
     for (int l = 0; l < c.layers; ++l) {
         const Layer &ly = e->layers[l];
-        EpiQKV eq{ly.c0qkv, nullptr, e->qk, M, 3 * H, 2 * H, 0, e->vT, 2 * H, S, S_pad, H, ly.c1qkv, st_qkv,
-                  e->rope[ly.window ? 1 : 0]};
+        EpiQKV<PRE_LN> eq{.qk = {.bias = ly.c0qkv, .c1 = ly.c1qkv, .row_stats = st_qkv, .Y = e->qk, .M = M, .N = 3 * H,
+                                 .ldy = 2 * H, .S = S, .rope = e->rope[ly.window ? 1 : 0]},
+                          .vT = e->vT, .vt_col0 = 2 * H, .S_pad = S_pad, .H = H};
         if ((rc = launch_linear(e->m_xh, ly.m_wqkv, M, 3 * H, H, eq, s))) return rc;
         if ((rc = launch_attention(e, mask, B, S, ly.window, l == c.layers - 1 && cls_tail, s))) return rc;
         if (l == c.layers - 1 && cls_tail) break;
         // attention output projection + residual: y <- ctx Wo^T + bo + LN_pending(y); statistics of the new sums
-        EpiResidDefer eo{ly.bo, e->x, e->xh, pst, pg, pb, e->parts, pstride, M, H, H};
+        EpiResidDefer eo{.bias = ly.bo, .y = e->x, .yh = e->xh, .stats_prev = pst, .gamma = pg, .beta = pb, .parts = e->parts,
+                         .part_stride = pstride, .M = M, .N = H, .ld = H};
         if ((rc = launch_linear(e->m_ctx, ly.m_wo, M, H, H, eo, s))) return rc;
         ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
         AC_LAUNCH_CHECK();
-        EpiFfn1 e1{ly.c0f, nullptr, e->ffn, M, N1, I, 0, nullptr, 0, 0, 0, 0, ly.c1f, e->stats_b};
+        EpiFfn1 e1{.bias = ly.c0f, .c1 = ly.c1f, .row_stats = e->stats_b, .Y = e->ffn, .M = M, .N = N1, .ldy = I};
         if ((rc = launch_linear(e->m_xh, ly.m_w1, M, N1, H, e1, s))) return rc;
         if constexpr (!PRE_LN) { pst = e->stats_b; pg = ly.ln_ffn_w; pb = ly.ln_ffn_b; }
         // FFN output projection + residual: y <- ffn W2^T + b2 + LN_pending(y)
-        EpiResidDefer e2{ly.b2, e->x, e->xh, pst, pg, pb, e->parts, pstride, M, H, H};
+        EpiResidDefer e2{.bias = ly.b2, .y = e->x, .yh = e->xh, .stats_prev = pst, .gamma = pg, .beta = pb, .parts = e->parts,
+                         .part_stride = pstride, .M = M, .N = H, .ld = H};
         if ((rc = launch_linear(e->m_ffn, ly.m_w2, M, H, I, e2, s))) return rc;
         ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_a);
         AC_LAUNCH_CHECK();
@@ -1323,14 +1323,14 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
         else
             gather_cls_ln_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, pg, pb, c.ln_eps, e->ctx_cls, e->x_cls);
         AC_LAUNCH_CHECK();
-        EpiResid eo{last.bo, e->x_cls, e->tmp_cls, B, H, H, 0, nullptr, 0, 0, 0, 0};
+        EpiF32<false, true> eo{.bias = last.bo, .residual = e->x_cls, .Y = e->tmp_cls, .M = B, .N = H, .ldy = H};
         if ((rc = launch_linear(e->m_ctx_cls, last.m_wo, B, H, H, eo, s))) return rc;
         layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->tmp_cls, last.ln_ffn_w, last.ln_ffn_b, c.ln_eps, B, H, PRE_LN ? nullptr : res,
                                                  e->xh_cls);
         AC_LAUNCH_CHECK();
-        EpiFfn1Rows e1{e->b1_last, nullptr, e->ffn_cls, B, N1, I, 0, nullptr, 0, 0, 0, 0};
+        EpiFfn1Rows e1{.bias = e->b1_last, .Y = e->ffn_cls, .M = B, .N = N1, .ldy = I};
         if ((rc = launch_linear(e->m_xh_cls, e->p_w1_last, B, N1, H, e1, s))) return rc;
-        EpiResid e2{last.b2, res, sum, B, H, H, 0, nullptr, 0, 0, 0, 0};
+        EpiF32<false, true> e2{.bias = last.b2, .residual = res, .Y = sum, .M = B, .N = H, .ldy = H};
         if ((rc = launch_linear(e->m_ffn_cls, last.m_w2, B, H, I, e2, s))) return rc;
         layernorm_kernel<<<cb, wpb * 32, 0, s>>>(sum, last.ln_out_w, last.ln_out_b, c.ln_eps, B, H, res, nullptr);
         AC_LAUNCH_CHECK();
@@ -1394,11 +1394,24 @@ extern "C" int ac_encoder_last_hidden(ac_encoder *e, float *out, int64_t n_float
 // generic tensor-core linear exposed for parity tests / roofline measurement (the encoder's GEMM with a plain epilogue).
 //   precision AC_PREC_TF32: X, W fp32 (used as stored, tf32 truncation by the MMA unless pre-rounded), Y fp32
 //   precision AC_PREC_F16 : X, W fp16, Y fp32 (out_half = 0) or fp16 (out_half = 1)
-template <int MODE, bool OUT_HALF, int KIND>
-static int linear_tc_dispatch(const CUtensorMap &ta, const CUtensorMap &tb, const float *bias, const float *residual, void *Y,
-                              int M, int N, int K, int round_out, cudaStream_t s) {
-    EpiLinear<MODE, OUT_HALF, false> e{bias, residual, Y, M, N, N, round_out, nullptr, 0, 0, 0, 0};
-    return launch_gemm_tc<EpiLinear<MODE, OUT_HALF, false>, false, KIND>(ta, tb, M, N, K, e, s);
+template <int KIND>
+static int linear_tc(const CUtensorMap &ta, const CUtensorMap &tb, const float *bias, const float *residual, void *Y, int M,
+                     int N, int K, int epi, int round_out, int out_half, cudaStream_t s) {
+    const auto run = [&](const auto &e) {
+        return launch_gemm_tc<std::decay_t<decltype(e)>, false, KIND>(ta, tb, M, N, K, e, s);
+    };
+    if constexpr (KIND == GEMM_KIND_F16) {
+        if (out_half) {
+            __half *Yh = static_cast<__half *>(Y);
+            if (epi == 0) return run(EpiF16<Act::None, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
+            return run(EpiF16<Act::Gelu, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
+        }
+    }
+    float *Yf = static_cast<float *>(Y);
+    if (epi == 0) return run(EpiF32<false, false>{.bias = bias, .Y = Yf, .M = M, .N = N, .ldy = N, .round_out = round_out});
+    if (epi == 1) return run(EpiF32<true, false>{.bias = bias, .Y = Yf, .M = M, .N = N, .ldy = N, .round_out = round_out});
+    return run(EpiF32<false, true>{.bias = bias, .residual = residual, .Y = Yf, .M = M, .N = N, .ldy = N,
+                                   .round_out = round_out});
 }
 
 extern "C" int ac_linear_tc(const void *X, const void *W, const float *bias, const float *residual, void *Y, int M, int N,
@@ -1418,15 +1431,7 @@ extern "C" int ac_linear_tc(const void *X, const void *W, const float *bias, con
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (precision == AC_PREC_TF32) {
         AC_REQUIRE(!out_half, "ac_linear_tc: tf32 path writes fp32");
-        if (epi == 0) return linear_tc_dispatch<0, false, GEMM_KIND_TF32>(ta, tb, bias, residual, Y, M, N, K, round_out, s);
-        if (epi == 1) return linear_tc_dispatch<1, false, GEMM_KIND_TF32>(ta, tb, bias, residual, Y, M, N, K, round_out, s);
-        return linear_tc_dispatch<2, false, GEMM_KIND_TF32>(ta, tb, bias, residual, Y, M, N, K, round_out, s);
+        return linear_tc<GEMM_KIND_TF32>(ta, tb, bias, residual, Y, M, N, K, epi, round_out, 0, s);
     }
-    if (out_half) {
-        if (epi == 0) return linear_tc_dispatch<0, true, GEMM_KIND_F16>(ta, tb, bias, residual, Y, M, N, K, 0, s);
-        return linear_tc_dispatch<1, true, GEMM_KIND_F16>(ta, tb, bias, residual, Y, M, N, K, 0, s);
-    }
-    if (epi == 0) return linear_tc_dispatch<0, false, GEMM_KIND_F16>(ta, tb, bias, residual, Y, M, N, K, 0, s);
-    if (epi == 1) return linear_tc_dispatch<1, false, GEMM_KIND_F16>(ta, tb, bias, residual, Y, M, N, K, 0, s);
-    return linear_tc_dispatch<2, false, GEMM_KIND_F16>(ta, tb, bias, residual, Y, M, N, K, 0, s);
+    return linear_tc<GEMM_KIND_F16>(ta, tb, bias, residual, Y, M, N, K, epi, 0, out_half, s);
 }
