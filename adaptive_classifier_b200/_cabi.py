@@ -8,6 +8,7 @@ makes every compute call raise AdaptiveB200Error.
 from __future__ import annotations
 
 import ctypes
+import math
 import threading
 import os
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int64, c_size_t, c_uint64, c_void_p
@@ -25,7 +26,7 @@ AC_ACT_LOGITS, AC_ACT_SOFTMAX, AC_ACT_SIGMOID = 0, 1, 2
 AC_LOSS_CE, AC_LOSS_BCE, AC_LOSS_CE_STRATEGIC = 0, 1, 2
 AC_COST_LINEAR, AC_COST_SEPARABLE = 0, 1
 AC_STRATEGIC_CANDIDATES = 50
-AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT = 0, 1, 2
+AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT, AC_ARCH_MPNET = 0, 1, 2, 3
 AC_ENCODER_MAX_S = 512
 AC_MODERNBERT_MAX_S = 8192
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
@@ -74,7 +75,7 @@ class EncoderConfig(Structure):
                 ("vocab", c_int), ("max_pos", c_int), ("type_vocab", c_int), ("pad_idx", c_int),
                 ("ln_eps", c_float), ("precision", c_int), ("max_tokens", c_int), ("cls_only", c_int),
                 ("sliding_window", c_int), ("layer_sliding", POINTER(ctypes.c_int32)),
-                ("rope_full", c_void_p), ("rope_sliding", c_void_p)]
+                ("rope_full", c_void_p), ("rope_sliding", c_void_p), ("rel_bias", c_void_p)]
 
 
 _PP = POINTER(c_void_p)
@@ -552,6 +553,54 @@ def distilbert_to_bert_state_dict(sd: dict, c):
     return out, dims
 
 
+def mpnet_relative_bias_table(weight: torch.Tensor, heads: int) -> torch.Tensor:
+    """[heads, 2 AC_ENCODER_MAX_S - 1] fp32 table of ac_encoder_config.rel_bias: entry (h, AC_ENCODER_MAX_S - 1 + key - query)
+    = weight[bucket(key - query), h], with HF MPNetEncoder.relative_position_bucket's formula and fp32 arithmetic (32 buckets:
+    16 per direction, exact below distance 8, log-spaced up to 128, saturated beyond)."""
+    weight = weight.detach().to(device="cpu", dtype=torch.float32)
+    assert weight.shape == (32, heads), weight.shape
+    n = -torch.arange(-(AC_ENCODER_MAX_S - 1), AC_ENCODER_MAX_S, dtype=torch.long)     # query - key
+    num_buckets, max_exact, max_distance = 16, 8, 128
+    ret = (n < 0).to(torch.long) * num_buckets
+    n = torch.abs(n)
+    large = max_exact + (torch.log(n.float() / max_exact) / math.log(max_distance / max_exact)
+                         * (num_buckets - max_exact)).to(torch.long)
+    large = torch.min(large, torch.full_like(large, num_buckets - 1))
+    bucket = ret + torch.where(n < max_exact, n, large)
+    return weight[bucket].t().contiguous()
+
+
+def mpnet_to_bert_state_dict(sd: dict, c):
+    """MPNet (HF models/mpnet/modeling_mpnet.py) is the post-LN BERT block with RoBERTa's position rule (padding_idx 1), no
+    token-type embeddings and a relative position bias on the attention scores: rename its parameters to the BERT names the
+    encoder consumes, supply an all-zero single-row type table and turn encoder.relative_attention_bias into the rel_bias
+    table.  pooler.* is not used.  Raises AdaptiveB200Error naming any setting the CUDA path does not implement."""
+    if c.hidden_act != "gelu":
+        raise AdaptiveB200Error(f"MPNet hidden_act={c.hidden_act!r}: only exact-erf 'gelu' is implemented")
+    heads = c.num_attention_heads
+    if heads <= 0 or c.hidden_size != 64 * heads:
+        raise AdaptiveB200Error(f"MPNet head_dim={c.hidden_size / heads:g} (hidden={c.hidden_size}, heads={heads}): only "
+                                "head_dim 64 is implemented")
+    if c.relative_attention_num_buckets != 32:
+        raise AdaptiveB200Error(f"MPNet relative_attention_num_buckets={c.relative_attention_num_buckets}: only 32 is "
+                                "implemented (the bucket count HF's forward uses)")
+    out = {k: sd[k] for k in ("embeddings.word_embeddings.weight", "embeddings.position_embeddings.weight",
+                              "embeddings.LayerNorm.weight", "embeddings.LayerNorm.bias")}
+    out["embeddings.token_type_embeddings.weight"] = torch.zeros((1, c.hidden_size), dtype=torch.float32)
+    ren = {"attention.attn.q": "attention.self.query", "attention.attn.k": "attention.self.key",
+           "attention.attn.v": "attention.self.value", "attention.attn.o": "attention.output.dense",
+           "attention.LayerNorm": "attention.output.LayerNorm", "intermediate.dense": "intermediate.dense",
+           "output.dense": "output.dense", "output.LayerNorm": "output.LayerNorm"}
+    for l in range(c.num_hidden_layers):
+        for src, dst in ren.items():
+            for wb in ("weight", "bias"):
+                out[f"encoder.layer.{l}.{dst}.{wb}"] = sd[f"encoder.layer.{l}.{src}.{wb}"]
+    dims = dict(layers=c.num_hidden_layers, hidden=c.hidden_size, heads=heads, intermediate=c.intermediate_size,
+                vocab=c.vocab_size, max_pos=c.max_position_embeddings, type_vocab=1, ln_eps=c.layer_norm_eps, pad_idx=1,
+                rel_bias=mpnet_relative_bias_table(sd["encoder.relative_attention_bias.weight"], heads))
+    return out, dims
+
+
 def check_head_dim(hidden: int, heads: int, what: str = "encoder") -> None:
     """The attention kernels of the BERT-family encoder take head_dim = hidden / heads of 64 (bert-base, RoBERTa, DistilBERT)
     or 32 (all-MiniLM, BGE-small, E5-small, GTE-small); raises AdaptiveB200Error naming anything else (no device call)."""
@@ -609,12 +658,14 @@ def modernbert_settings(c) -> dict:
 
 
 class Encoder:
-    """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors)."""
+    """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors).  arch "mpnet"
+    takes the BERT names (mpnet_to_bert_state_dict) and rel_bias, the [heads, 2 AC_ENCODER_MAX_S - 1] table of
+    mpnet_relative_bias_table."""
 
     def __init__(self, sd: dict, *, arch: str, layers: int, hidden: int, heads: int, intermediate: int, vocab: int,
                  max_pos: int = AC_ENCODER_MAX_S, type_vocab: int = 1, ln_eps: float, pad_idx: int = 0,
                  max_tokens: int = 65536, device="cuda", cls_only: bool = True, sliding_window: int = 0,
-                 layer_sliding=None, rope_theta=None):
+                 layer_sliding=None, rope_theta=None, rel_bias: Optional[torch.Tensor] = None):
         L = load_library()
         self._L = L
         self.hidden = hidden
@@ -664,8 +715,13 @@ class Encoder:
             w.ff1_w, w.ff1_b = arr(p + "intermediate.dense.weight"), arr(p + "intermediate.dense.bias")
             w.ff2_w, w.ff2_b = arr(p + "output.dense.weight"), arr(p + "output.dense.bias")
             w.out_ln_w, w.out_ln_b = arr(p + "output.LayerNorm.weight"), arr(p + "output.LayerNorm.bias")
-            cfg = EncoderConfig(AC_ARCH_BERT if arch == "bert" else AC_ARCH_ROBERTA, layers, hidden, heads, intermediate,
-                                vocab, max_pos, type_vocab, pad_idx, ln_eps, AC_PREC_F16, max_tokens, 1 if cls_only else 0)
+            code = {"bert": AC_ARCH_BERT, "roberta": AC_ARCH_ROBERTA, "mpnet": AC_ARCH_MPNET}[arch]
+            cfg = EncoderConfig(code, layers, hidden, heads, intermediate, vocab, max_pos, type_vocab, pad_idx, ln_eps,
+                                AC_PREC_F16, max_tokens, 1 if cls_only else 0)
+            if rel_bias is not None:      # ac_encoder_create refuses an MPNet encoder without it
+                rb = rel_bias.detach().to(device=dev, dtype=torch.float32).contiguous()
+                keep["rel_bias"] = rb
+                cfg.rel_bias = rb.data_ptr()
         h = c_void_p()
         with torch.cuda.device(dev):
             check(L.ac_encoder_create(ctypes.byref(cfg), ctypes.byref(w), ctypes.byref(h)), "ac_encoder_create")
@@ -674,15 +730,19 @@ class Encoder:
 
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
-        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel (post-LN blocks) or ModernBertModel (pre-LN,
-        RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for the post-LN family, 64 for ModernBERT.  Sequences up to 512
-        tokens, or for ModernBERT up to max(512, max_position_embeddings) <= AC_MODERNBERT_MAX_S."""
+        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel (post-LN blocks) or
+        ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for BERT / RoBERTa / DistilBERT, 64
+        for MPNet and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
+        AC_MODERNBERT_MAX_S."""
         c = model.config
         mt = getattr(c, "model_type", "bert")
         if mt == "modernbert":
             dims = modernbert_settings(c)
             return cls(dict(model.state_dict()), arch="modernbert", max_tokens=max_tokens, device=device, cls_only=cls_only,
                        **dims)
+        if mt == "mpnet":
+            sd, dims = mpnet_to_bert_state_dict(dict(model.state_dict()), c)
+            return cls(sd, arch="mpnet", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
         if mt == "distilbert":
             check_head_dim(c.dim, c.n_heads, "DistilBERT")
             sd, dims = distilbert_to_bert_state_dict(dict(model.state_dict()), c)

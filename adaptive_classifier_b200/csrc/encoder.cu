@@ -496,6 +496,7 @@ __global__ void layernorm_kernel(const float *__restrict__ in, const float *__re
 }
 
 // modeling_bert.py:53-113 / modeling_roberta.py:146-159: (word + type) + position -> LayerNorm
+// modeling_mpnet.py MPNetEmbeddings: RoBERTa's positions (padding_idx 1); the type table is one zero row
 // modeling_modernbert.py ModernBertEmbeddings: pos = type = NULL, LayerNorm(word) (b = zeros: norm_bias=False)
 __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *__restrict__ type_ids,
                                 const float *__restrict__ word, const float *__restrict__ pos,
@@ -512,7 +513,7 @@ __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *
     int tt = type_ids ? type_ids[row] : 0;
     tt = min(max(tt, 0), type_vocab - 1);
     int p = s;
-    if (arch == AC_ARCH_ROBERTA) {
+    if (arch == AC_ARCH_ROBERTA || arch == AC_ARCH_MPNET) {
         // position = cumsum(ids != pad)[s] * (id != pad) + pad_idx
         int cnt = 0;
         for (int j = lane; j <= s; j += 32) cnt += (ids[bq * S + j] != pad_idx) ? 1 : 0;
@@ -600,6 +601,8 @@ constexpr int ATT_S_BYTES = 128 * ATT_S_LD * 4;
 constexpr int ATT_REGION_BYTES = (ATT_S_BYTES + 1023) / 1024 * 1024;
 constexpr int ATT_SMEM = ATT_REGION_BYTES + 16 * 1024 + 1024 /*align*/ + 64;
 static_assert(2 * (ATT_SMEM + 1024) <= 228 * 1024, "two attention CTAs must fit one SM");
+constexpr int ATT_SMEM_BIAS = ATT_SMEM + 1024;               // + the 255 staged relative-bias entries (MPNet)
+static_assert(2 * (ATT_SMEM_BIAS + 1024) <= 228 * 1024, "two attention CTAs must fit one SM");
 
 // S[128 x 128] = Q K^T for the query tile sQ and key tile sK (both [128 rows x 128 B], 128B swizzle) -> sS (fp32, ld ATT_S_LD).
 // Issued by the whole warpgroup; returns once the products are in shared memory (the caller synchronises the CTA).
@@ -701,11 +704,27 @@ __device__ __forceinline__ void att_exp_pack(const float (&r)[32], uint32_t km, 
     }
 }
 
-// window: ModernBERT sliding_attention half-window (keys |q - key| <= window), 0 = full attention
-template <int DH>
+// MPNet relative position bias (modeling_mpnet.py MPNetEncoder.compute_position_bias), the BIAS instantiations of both
+// kernels.  rel_bias row h holds the head's bias at entry (AC_ENCODER_MAX_S - 1) + key - q.  A CTA of queries q0 .. q0 + 127
+// and keys 0 .. nkeys - 1 stages entries from (AC_ENCODER_MAX_S - 128) - q0 on, times log2(e), so that query row qrow
+// (q = q0 + qrow) finds the bias of key at sB[127 - qrow + key]: 32 lanes read 32 consecutive words, conflict-free.
+constexpr int ATT_BIAS_OFS = AC_ENCODER_MAX_S - 128;
+__device__ __forceinline__ void att_stage_bias(const float *__restrict__ row, int q0, int nkeys, float *sB, int tid) {
+    for (int t = tid; t < nkeys + 127; t += ATT_THREADS) sB[t] = __ldg(row + ATT_BIAS_OFS - q0 + t) * 1.44269504088896340736f;
+}
+// scores of 32 keys -> ex2-domain logits s scale log2(e) + bias log2(e), which the softmax then uses with scale 1
+__device__ __forceinline__ void att_add_bias(float (&r)[32], const float *bq, float scale_log2) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) r[j] = fmaf(r[j], scale_log2, bq[j]);
+}
+
+// window: ModernBERT sliding_attention half-window (keys |q - key| <= window), 0 = full attention.
+// BIAS: rel_bias [heads, 2 AC_ENCODER_MAX_S - 1] is added to the scaled scores before the mask (MPNet; window 0)
+template <int DH, bool BIAS = false>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
-                 const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
+                 const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx,
+                 const float *__restrict__ rel_bias) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                    // [128 rows x 128 B]
@@ -735,6 +754,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
         tma_load_2d(sVt, &tmap_vt, bar_load, 0, vrow);
         tma_load_2d(sVt + 8 * 1024, &tmap_vt, bar_load, 64, vrow);
     }
+    float *sB = reinterpret_cast<float *>(smem + ATT_REGION_BYTES + 16 * 1024 + 64);   // BIAS: 255 entries
+    if constexpr (BIAS) att_stage_bias(rel_bias + h * (2 * AC_ENCODER_MAX_S - 1), 0, 128, sB, tid);
     // ---- S = Q K^T: both 64-row chains retire before the score tile overwrites Q and K
     mbar_wait_guarded(bar_load, 0);
     {
@@ -760,11 +781,14 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     uint32_t kmask[4];
     att_key_bits(mask, row0, S, 0, qrow, window, lane, kmask);
     const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
+    const float sl2 = BIAS ? 1.f : scale_log2;   // BIAS: att_add_bias has scaled the row already
+    const float *bq = sB + 127 - qrow;
     float mx = -CUDART_INF_F;
 #pragma unroll 1
     for (int c = 0; c < 128; c += 32) {
         float r[32];
         acc_row_ld32(srow + c, r);
+        if constexpr (BIAS) att_add_bias(r, bq + c, scale_log2);
         const uint32_t km = c == 0 ? kmask[0] : c == 32 ? kmask[1] : c == 64 ? kmask[2] : kmask[3];
 #pragma unroll
         for (int j = 0; j < 32; ++j)
@@ -776,7 +800,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     for (int ci = 0; ci < 4; ++ci) {
         float r[32];
         acc_row_ld32(srow + 32 * ci, r);
-        att_exp_pack(r, kmask[ci], scale_log2, mx * scale_log2, sum, pk + 16 * ci);
+        if constexpr (BIAS) att_add_bias(r, bq + 32 * ci, scale_log2);
+        att_exp_pack(r, kmask[ci], sl2, mx * sl2, sum, pk + 16 * ci);
     }
     __syncthreads();                       // every score row has been read
     const uint32_t sp_base = smem_u32(sP);
@@ -809,17 +834,21 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
 //                 a sliding query block, holes in the mask) keeps m = -inf, P = 0 and a zero accumulator: the factor is
 //                 0 there rather than exp((-inf) - (-inf))
 //   P fp16, every accumulator fp32, as in the kernel above.  q_blocks = 1 (CLS-only tail next) computes rows 0..127 only.
-// smem: Q 16 KB | K 2 x 16 KB | V^T 2 x 16 KB | P 32 KB | score tile 66 KB | factors 512 B | 2 barriers: one CTA per SM.
+// smem: Q 16 KB | K 2 x 16 KB | V^T 2 x 16 KB | P 32 KB | score tile 66 KB | factors 512 B | 2 barriers (| BIAS: the staged
+// relative bias): one CTA per SM.
 // ------------------------------------------------------------------------------------------------
 constexpr int ATTS_STAGE_BYTES = 16 * 1024;
 constexpr int ATTS_OFF_K = 16 * 1024, ATTS_OFF_VT = 48 * 1024, ATTS_OFF_P = 80 * 1024, ATTS_OFF_S = 112 * 1024;
 constexpr int ATTS_SMEM = ATTS_OFF_S + ATT_S_BYTES + 128 * 4 + 2 * 8 + 1024 /*align*/;
 static_assert(ATTS_SMEM <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
+constexpr int ATTS_SMEM_BIAS = ATTS_SMEM + (AC_ENCODER_MAX_S + 128) * 4;   // + up to 639 staged relative-bias entries
+static_assert(ATTS_SMEM_BIAS <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
 
-template <int DH>
+template <int DH, bool BIAS = false>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
-                        const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx) {
+                        const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx,
+                        const float *__restrict__ rel_bias) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                              // [128 x 128 B]
@@ -863,11 +892,14 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         issue(0);
         if (nblk > 1) issue(1);
     }
+    float *sB = reinterpret_cast<float *>(bar + 2);               // BIAS (window 0, so kb0 = 0): 128 nblk + 127 entries
+    if constexpr (BIAS) att_stage_bias(rel_bias + h * (2 * AC_ENCODER_MAX_S - 1), q0, 128 * nblk, sB, tid);
 
     const int qrow = warp * 32 + lane;                            // row inside the query block
     const int qglob = q0 + qrow;                                  // position inside the sequence
     const float *srow = sS + qrow * ATT_S_LD;
     const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
+    const float sl2 = BIAS ? 1.f : scale_log2;                    // BIAS: att_add_bias has scaled the row already
     const int frow = 16 * warp + (lane >> 2);                     // accumulator fragment rows frow, frow + 8 (+ 64)
     const uint32_t sp_base = smem_u32(sP);
     float mx = -CUDART_INF_F, sum = 0.f;
@@ -886,25 +918,28 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
 
         uint32_t kmask[4];
         att_key_bits(mask, row0, S, key0, qglob, window, lane, kmask);
+        const float *bq = sB + 127 - qrow + key0;
         float bmx = -CUDART_INF_F;
 #pragma unroll
         for (int ci = 0; ci < 4; ++ci) {
             float r[32];
             acc_row_ld32(srow + 32 * ci, r);
+            if constexpr (BIAS) att_add_bias(r, bq + 32 * ci, scale_log2);
 #pragma unroll
             for (int jj = 0; jj < 32; ++jj)
                 if ((kmask[ci] >> jj) & 1u) bmx = fmaxf(bmx, r[jj]);
         }
         const float mnew = fmaxf(mx, bmx);
-        const float alpha = (mx == -CUDART_INF_F) ? 0.f : ex2_approx((mx - mnew) * scale_log2);
-        const float mxs = (mnew == -CUDART_INF_F) ? 0.f : mnew * scale_log2;   // no valid key yet: every P below is 0
+        const float alpha = (mx == -CUDART_INF_F) ? 0.f : ex2_approx((mx - mnew) * sl2);
+        const float mxs = (mnew == -CUDART_INF_F) ? 0.f : mnew * sl2;   // no valid key yet: every P below is 0
         float bsum = 0.f;
 #pragma unroll
         for (int ci = 0; ci < 4; ++ci) {
             float r[32];
             acc_row_ld32(srow + 32 * ci, r);
+            if constexpr (BIAS) att_add_bias(r, bq + 32 * ci, scale_log2);
             uint32_t pk[16];
-            att_exp_pack(r, kmask[ci], scale_log2, mxs, bsum, pk);
+            att_exp_pack(r, kmask[ci], sl2, mxs, bsum, pk);
             att_store_p(sp_base, qrow, 32 * ci, pk);
         }
         sum = fmaf(sum, alpha, bsum);
@@ -1004,6 +1039,7 @@ struct ac_encoder {
     float2 *stats_a = nullptr, *stats_b = nullptr, *stats_id = nullptr, *parts = nullptr;
     float *ones = nullptr, *zeros = nullptr;   // ones [H]; zeros [max(3H, 2I)]: beta / bias of the bias-free ModernBERT
     float *rope[2] = {nullptr, nullptr};       // ModernBERT RoPE tables [max_pos, 64] (full, sliding layers)
+    float *rel_bias = nullptr;                 // MPNet relative position bias [heads, 2 AC_ENCODER_MAX_S - 1]; NULL otherwise
     std::vector<void *> allocs;
     int last_B = 0, last_S = 0;           // shape of the previous forward; its full hidden state (cls_only = 0) is in tmp
     bool last_cls_only = false;
@@ -1016,13 +1052,15 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
     return AC_OK;
 }
 
-// softmax(Q K^T / sqrt(head_dim) + mask) V out of e->qk / e->vT into e->ctx; window = sliding half-window, 0 = full attention.
-// S <= 128 runs attention_kernel, longer sequences attention_stream_kernel over 128-query blocks.  cls_rows: only row 0 of
-// every sequence is read afterwards (the CLS-only tail), so only the first query block is computed.
+// softmax(Q K^T / sqrt(head_dim) [+ MPNet relative bias] + mask) V out of e->qk / e->vT into e->ctx; window = sliding
+// half-window, 0 = full attention.  S <= 128 runs attention_kernel, longer sequences attention_stream_kernel over 128-query
+// blocks.  cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail), so only the first query block is
+// computed.
 static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, cudaStream_t s) {
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden;
-    const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create)
+    const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create); 64 with a relative bias
+    const float *rb = e->rel_bias;
     AC_REQUIRE(S <= AC_ENCODER_MAX_S || dh == 64, "attention: S=%d > %d needs head_dim 64 (ModernBERT)", S, AC_ENCODER_MAX_S);
     // per-device: the attribute is a property of the (function, device) pair
     static bool att_attr[64] = {};
@@ -1031,8 +1069,11 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, in
     if (dev < 0 || dev >= 64 || !att_attr[dev]) {
         AC_CUDA(cudaFuncSetAttribute(attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
         AC_CUDA(cudaFuncSetAttribute(attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_BIAS));
         AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
         AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
+        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     ATTS_SMEM_BIAS));
         if (dev >= 0 && dev < 64) att_attr[dev] = true;
     }
     // algorithmic flops over the keys each computed query attends to at the true sequence length (the 128-wide tiles do
@@ -1047,12 +1088,13 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, in
     }
     const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * keys * dh, 0.0, s);
     if (S <= 128) {
-        auto kern = dh == 32 ? attention_kernel<32> : attention_kernel<64>;
-        kern<<<B * c.heads, ATT_THREADS, ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx);
+        auto kern = rb ? attention_kernel<64, true> : dh == 32 ? attention_kernel<32> : attention_kernel<64>;
+        kern<<<B * c.heads, ATT_THREADS, rb ? ATT_SMEM_BIAS : ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H,
+                                                                            window, e->ctx, rb);
     } else {
-        auto kern = dh == 32 ? attention_stream_kernel<32> : attention_stream_kernel<64>;
-        kern<<<dim3(B * c.heads, q_blocks), ATT_THREADS, ATTS_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window,
-                                                                          e->ctx);
+        auto kern = rb ? attention_stream_kernel<64, true> : dh == 32 ? attention_stream_kernel<32> : attention_stream_kernel<64>;
+        kern<<<dim3(B * c.heads, q_blocks), ATT_THREADS, rb ? ATTS_SMEM_BIAS : ATTS_SMEM, s>>>(
+            e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx, rb);
     }
     prof_end(slot, s);
     AC_LAUNCH_CHECK();
@@ -1123,6 +1165,9 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
                    (cfg->hidden / cfg->heads == 64 || (!mb && cfg->hidden / cfg->heads == 32)),
                "ac_encoder_create: head_dim must be %s (hidden=%d heads=%d)", mb ? "64 for ModernBERT" : "64 or 32", cfg->hidden,
                cfg->heads);
+    const bool mp = cfg->arch == AC_ARCH_MPNET;
+    AC_REQUIRE(!mp || (cfg->rel_bias && cfg->hidden == 64 * cfg->heads),
+               "ac_encoder_create: MPNet needs rel_bias and head_dim 64 (hidden=%d heads=%d)", cfg->hidden, cfg->heads);
     AC_REQUIRE(cfg->intermediate % 64 == 0 && cfg->layers > 0 && cfg->max_tokens > 0, "ac_encoder_create: bad dims");
     int rc = ac_device_check();
     if (rc) return rc;
@@ -1134,6 +1179,7 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
 #define TRY(x) do { rc = (x); if (rc) { ac_encoder_destroy(e); return rc; } } while (0)
     e->cfg.layer_sliding = nullptr;   // copied into e->layers / e->rope below
     e->cfg.rope_full = e->cfg.rope_sliding = nullptr;
+    e->cfg.rel_bias = nullptr;        // copied into e->rel_bias below
     // ones / zeros are filled with the other constants after packing; the bias-free ModernBERT roles point at zeros
     const int nzeros = std::max(3 * H, 2 * I);
     TRY(dev_alloc(e, &e->ones, H));
@@ -1172,6 +1218,7 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
         TRY(pack_f32(e, &e->type, w->type_emb, static_cast<size_t>(cfg->type_vocab) * H));
         TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
         TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, H));
+        if (mp) TRY(pack_f32(e, &e->rel_bias, cfg->rel_bias, static_cast<size_t>(cfg->heads) * (2 * AC_ENCODER_MAX_S - 1)));
         for (int l = 0; l < L; ++l) {
             Layer &ly = e->layers[l];
             // the fused QKV [3H, H] of layer l consumes the sums pending the output LayerNorm of layer l-1 (identity for

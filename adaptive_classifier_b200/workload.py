@@ -28,6 +28,19 @@ def modernbert_base(seed: int = 1234):
     return m, cfg
 
 
+def mpnet_base(seed: int = 1234):
+    """HF MPNetModel of the sentence-transformers/all-mpnet-base-v2 shape (12 x 768, 12 heads, I = 3072, vocab 30527,
+    max_position_embeddings 514, LayerNorm eps 1e-5, 32 relative-attention buckets), random init under
+    torch.manual_seed(seed)."""
+    from transformers import MPNetConfig, MPNetModel
+    torch.manual_seed(seed)
+    cfg = MPNetConfig(vocab_size=30527, hidden_size=768, num_hidden_layers=12, num_attention_heads=12,
+                      intermediate_size=3072, max_position_embeddings=514, layer_norm_eps=1e-5)
+    m = MPNetModel(cfg, add_pooling_layer=False)
+    m.eval()
+    return m, cfg
+
+
 def modernbert_ids(B: int, S: int, seed: int = 7) -> torch.Tensor:
     """uniform in [1000, 50000), [CLS]=50281 first, [SEP]=50282 last, never the pad id 50283; int32 [B,S] on the host."""
     g = torch.Generator().manual_seed(seed)

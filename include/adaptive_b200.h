@@ -244,7 +244,8 @@ int ac_head_train_strategic(const float *X, const int64_t *targets, const int64_
  * Stage E -- encoder.  Replaces `self.model(**inputs).last_hidden_state[:,0,:]` + F.normalize at
  *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel / ModernBertModel forward).
  * ------------------------------------------------------------------------------------------ */
-enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2 };
+enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2,
+       AC_ARCH_MPNET = 3 /* post-LN BERT block, RoBERTa positions, relative position bias (rel_bias); head_dim 64 */ };
 #define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts for BERT / RoBERTa / DistilBERT (their
                                   position tables stop at 512) */
 #define AC_MODERNBERT_MAX_S 8192   /* largest max_pos of an AC_ARCH_MODERNBERT encoder (max_position_embeddings of the
@@ -258,9 +259,9 @@ enum {
 typedef struct {
     int arch;            /* AC_ARCH_* */
     int layers, hidden, heads, intermediate;   /* hidden % 128 == 0; head_dim = hidden / heads is 64 or 32
-                                                  (64 only for AC_ARCH_MODERNBERT) */
+                                                  (64 only for AC_ARCH_MODERNBERT and AC_ARCH_MPNET) */
     int vocab, max_pos, type_vocab;
-    int pad_idx;         /* roberta: position ids start at pad_idx+1 */
+    int pad_idx;         /* roberta, mpnet: position ids start at pad_idx+1 */
     float ln_eps;
     int precision;       /* AC_PREC_* */
     int max_tokens;      /* workspace is sized for B*S <= max_tokens */
@@ -273,6 +274,10 @@ typedef struct {
     const float *rope_full;      /* DEVICE [max_pos, 64] fp32 RoPE table of the full-attention layers:              */
     const float *rope_sliding;   /*   row = position, [0, 32) cos, [32, 64) sin of the 32 frequencies (HF
                                        ModernBertRotaryEmbedding's formula, built by the caller); the sliding layers' table */
+    /* AC_ARCH_MPNET only (ignored otherwise), copied by ac_encoder_create.  DEVICE [heads, 2 AC_ENCODER_MAX_S - 1] fp32:
+       entry (h, AC_ENCODER_MAX_S - 1 + key - query) is the bias every layer adds to head h's scaled score of (query, key)
+       (HF MPNetEncoder.compute_position_bias: relative_attention_bias.weight[bucket(key - query), h], built by the caller) */
+    const float *rel_bias;
 } ac_encoder_config;
 
 /* device pointers to the HF state_dict tensors (fp32, HF layout [out,in]).
