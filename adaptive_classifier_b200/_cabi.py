@@ -37,7 +37,8 @@ EXPORTS = [
     "ac_segment_mean", "ac_memory_append_prune",
     "ac_head_forward", "ac_head_train_workspace_bytes", "ac_head_train_step", "ac_head_train_epoch", "ac_head_phase_timing", "ac_head_train_plan", "ac_head_grad", "ac_ewc_penalty",
     "ac_strategic_workspace_bytes", "ac_strategic_best_response", "ac_head_train_strategic_workspace_bytes", "ac_head_train_strategic",
-    "ac_encoder_create", "ac_encoder_destroy", "ac_encoder_forward_cls", "ac_encoder_last_hidden", "ac_linear_tc",
+    "ac_encoder_create", "ac_encoder_destroy", "ac_encoder_forward_cls", "ac_encoder_last_hidden", "ac_encoder_attention",
+    "ac_linear_tc",
     "ac_proto_class_scores", "ac_proto_class_scores_n", "ac_blend_dense", "ac_topk_desc_workspace_bytes", "ac_topk_desc", "ac_blend_topk",
     "ac_pipeline_create", "ac_pipeline_destroy", "ac_pipeline_predict_device", "ac_pipeline_predict_host",
     "ac_pipeline_encode", "ac_pipeline_embeddings", "ac_pipeline_search_shard", "ac_pipeline_finish_sharded",
@@ -138,6 +139,7 @@ def load_library() -> ctypes.CDLL:
     L.ac_encoder_destroy.argtypes = [c_void_p]
     L.ac_encoder_forward_cls.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
     L.ac_encoder_last_hidden.argtypes = [c_void_p, c_void_p, c_int64, c_void_p]
+    L.ac_encoder_attention.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
     L.ac_linear_tc.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                c_int, c_int, c_void_p]
     L.ac_proto_class_scores.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]
@@ -669,6 +671,7 @@ class Encoder:
         L = load_library()
         self._L = L
         self.hidden = hidden
+        self.heads = heads
         self.max_tokens = max_tokens
         dev = torch.device(device)
         keep = {}
@@ -778,6 +781,25 @@ class Encoder:
         check(self._L.ac_encoder_last_hidden(self.handle, out.data_ptr(), out.numel(), stream_ptr()),
               "ac_encoder_last_hidden")
         return out
+
+    def attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask: Optional[torch.Tensor] = None, *,
+                  window: int = 0, cls_rows: bool = False, pad_fill: float = 0.0) -> torch.Tensor:
+        """Parity entry: this encoder's attention stage alone (ac_encoder_attention).  q, k, v [B, S, heads, head_dim] are
+        rounded to fp16 and laid out as the QKV epilogue leaves them (q | k rows; V transposed per (sequence, feature) with
+        the keys padded to a multiple of 8, the pad keys holding pad_fill, which a correct kernel never lets through).
+        Returns the context [B, S, heads, head_dim] fp16; with cls_rows only rows 0..127 of every sequence are computed."""
+        B, S, heads, dh = q.shape
+        assert heads == self.heads and heads * dh == self.hidden and k.shape == q.shape and v.shape == q.shape and q.is_cuda
+        qk = torch.cat([q.reshape(B * S, self.hidden), k.reshape(B * S, self.hidden)], dim=1).to(torch.float16).contiguous()
+        S_pad = (S + 7) // 8 * 8
+        vT = torch.full((B, self.hidden, S_pad), pad_fill, dtype=torch.float16, device=q.device)
+        vT[:, :, :S] = v.reshape(B, S, self.hidden).transpose(1, 2)
+        if mask is not None:
+            mask = mask.to(torch.int32).contiguous()
+        ctx = torch.empty((B * S, self.hidden), dtype=torch.float16, device=q.device)
+        check(self._L.ac_encoder_attention(self.handle, qk.data_ptr(), vT.data_ptr(), ptr(mask), B, S, window,
+                                           1 if cls_rows else 0, ctx.data_ptr(), stream_ptr()), "ac_encoder_attention")
+        return ctx.view(B, S, heads, dh)
 
     def close(self):
         if getattr(self, "handle", None):

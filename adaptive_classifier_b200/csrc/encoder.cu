@@ -1394,37 +1394,59 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
     return AC_OK;
 }
 
+// Shape checks every entry that runs attention shares, then the V^T view of a (B, S) call: rows (b, h, d), S_pad keys per
+// row; box = 64 keys x 64 rows (one head of 64, or a head of 32 and its neighbour; rows past B*H read as zeros).  The view
+// is cached on the handle, keyed on (B, S).
+static int check_shape_map_vt(ac_encoder *e, const char *who, int B, int S) {
+    AC_REQUIRE(B > 0 && S > 0, "%s: B=%d S=%d", who, B, S);
+    if (e->cfg.arch == AC_ARCH_MODERNBERT) {
+        // RoPE has no position table: any S up to the encoder's max_pos (<= AC_MODERNBERT_MAX_S) runs
+        AC_REQUIRE(S <= e->cfg.max_pos, "%s: S=%d exceeds this ModernBERT encoder's max_pos=%d (max_position_embeddings)", who,
+                   S, e->cfg.max_pos);
+    } else if (S > 512) {
+        set_error("%s: S=%d > 512 is not supported (the reference truncates at max_length = 512)", who, S);
+        return AC_E_UNSUPPORTED;
+    }
+    AC_REQUIRE(static_cast<int64_t>(B) * S <= e->cfg.max_tokens, "%s: B*S=%lld exceeds max_tokens=%d", who,
+               static_cast<long long>(B) * S, e->cfg.max_tokens);
+    AC_REQUIRE(S <= e->cfg.max_pos, "%s: S exceeds max_position_embeddings", who);
+    const int H = e->cfg.hidden;
+    const int S_pad = (S + 7) / 8 * 8;
+    AC_REQUIRE(static_cast<size_t>(B) * H * S_pad <= e->vt_elems,
+               "%s: B=%d sequences of S=%d exceed the transposed-V workspace; split the batch", who, B, S);
+    if (e->vt_B != B || e->vt_S != S) {
+        int rc = make_tmap_2d(&e->m_vt_att, e->vT, 2, static_cast<uint64_t>(B) * H, S_pad, static_cast<uint64_t>(S_pad) * 2, 64, 64);
+        if (rc) return rc;
+        e->vt_B = B; e->vt_S = S;
+    }
+    return AC_OK;
+}
+
 extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids,
                                       int B, int S, float *out_unit_cls, ac_stream_t stream) {
     AC_REQUIRE(e && ids && out_unit_cls, "ac_encoder_forward_cls: null argument");
-    AC_REQUIRE(B > 0 && S > 0, "ac_encoder_forward_cls: B=%d S=%d", B, S);
-    if (e->cfg.arch == AC_ARCH_MODERNBERT) {
-        // RoPE has no position table: any S up to the encoder's max_pos (<= AC_MODERNBERT_MAX_S) runs
-        AC_REQUIRE(S <= e->cfg.max_pos, "ac_encoder_forward_cls: S=%d exceeds this ModernBERT encoder's max_pos=%d "
-                   "(max_position_embeddings)", S, e->cfg.max_pos);
-    } else if (S > 512) {
-        set_error("ac_encoder_forward_cls: S=%d > 512 is not supported (the reference truncates at max_length = 512)", S);
-        return AC_E_UNSUPPORTED;
-    }
-    AC_REQUIRE(static_cast<int64_t>(B) * S <= e->cfg.max_tokens, "ac_encoder_forward_cls: B*S=%lld exceeds max_tokens=%d",
-               static_cast<long long>(B) * S, e->cfg.max_tokens);
-    AC_REQUIRE(S <= e->cfg.max_pos, "ac_encoder_forward_cls: S exceeds max_position_embeddings");
+    int rc = check_shape_map_vt(e, "ac_encoder_forward_cls", B, S);
+    if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const ac_encoder_config &c = e->cfg;
-    const int H = c.hidden;
-    const int S_pad = (S + 7) / 8 * 8;
-    AC_REQUIRE(static_cast<size_t>(B) * H * S_pad <= e->vt_elems,
-               "ac_encoder_forward_cls: B=%d sequences of S=%d exceed the transposed-V workspace; split the batch", B, S);
-    int rc;
-    if (e->vt_B != B || e->vt_S != S) {
-        // V^T view of this call: rows (b, h, d), S_pad keys per row; box = 64 keys x 64 rows (one head of 64, or a head of
-        // 32 and its neighbour; rows past B*H read as zeros)
-        if ((rc = make_tmap_2d(&e->m_vt_att, e->vT, 2, static_cast<uint64_t>(B) * H, S_pad, static_cast<uint64_t>(S_pad) * 2, 64, 64)))
-            return rc;
-        e->vt_B = B; e->vt_S = S;
-    }
-    return c.arch == AC_ARCH_MODERNBERT ? forward_layers<true>(e, ids, mask, type_ids, B, S, out_unit_cls, s)
-                                        : forward_layers<false>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    return e->cfg.arch == AC_ARCH_MODERNBERT ? forward_layers<true>(e, ids, mask, type_ids, B, S, out_unit_cls, s)
+                                             : forward_layers<false>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+}
+
+// parity entry: the attention stage alone, through the handle's own buffers, V^T view and launch_attention
+extern "C" int ac_encoder_attention(ac_encoder *e, const void *qk, const void *vT, const int32_t *mask, int B, int S, int window,
+                                    int cls_rows, void *ctx_out, ac_stream_t stream) {
+    AC_REQUIRE(e && qk && vT && ctx_out, "ac_encoder_attention: null argument");
+    AC_REQUIRE(window >= 0 && (window == 0 || e->cfg.arch == AC_ARCH_MODERNBERT),
+               "ac_encoder_attention: window=%d needs an AC_ARCH_MODERNBERT encoder (0 = full attention)", window);
+    int rc = check_shape_map_vt(e, "ac_encoder_attention", B, S);
+    if (rc) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const size_t H = e->cfg.hidden, M = static_cast<size_t>(B) * S, S_pad = (S + 7) / 8 * 8;
+    AC_CUDA(cudaMemcpyAsync(e->qk, qk, M * 2 * H * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    AC_CUDA(cudaMemcpyAsync(e->vT, vT, B * H * S_pad * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    if ((rc = launch_attention(e, mask, B, S, window, cls_rows != 0, s))) return rc;
+    AC_CUDA(cudaMemcpyAsync(ctx_out, e->ctx, M * H * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    return AC_OK;
 }
 
 extern "C" int ac_encoder_last_hidden(ac_encoder *e, float *out, int64_t n_floats, ac_stream_t stream) {

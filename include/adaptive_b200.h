@@ -318,6 +318,16 @@ int ac_encoder_forward_cls(ac_encoder *enc, const int32_t *ids, const int32_t *m
 /* debugging / parity: copy the full last hidden state [B*S,H] of the previous forward */
 int ac_encoder_last_hidden(ac_encoder *enc, float *out, int64_t n_floats, ac_stream_t stream);
 
+/* debugging / parity: run this encoder's attention stage alone.  qk [B*S, 2H] fp16 (q then k, head h at columns h*dh),
+ * vT fp16 in the layout the QKV epilogue writes ((b*H + feature) * S_pad + key, S_pad = roundup(S, 8); the pad keys may
+ * hold any finite value), mask as in ac_encoder_forward_cls, window = sliding half-window (keys |query - key| <= window;
+ * 0 = full; must be 0 unless AC_ARCH_MODERNBERT), cls_rows != 0 computes the first 128-query block only (later rows of
+ * ctx_out are then unspecified).  ctx_out [B*S, H] fp16 = softmax(q k^T / sqrt(dh) + rel_bias + mask) v per head; a query
+ * with no valid key in reach gets zeros.  Uses the encoder's heads, head_dim and rel_bias, and accepts and refuses the
+ * shapes ac_encoder_forward_cls does.  All pointers DEVICE. */
+int ac_encoder_attention(ac_encoder *enc, const void *qk, const void *vT, const int32_t *mask, int B, int S, int window,
+                         int cls_rows, void *ctx_out, ac_stream_t stream);
+
 /* generic tensor-core linear (the encoder's GEMM with its fused epilogues), exposed for parity tests and roofline
  * measurement: Y[M,N] = epi(X[M,K] W[N,K]^T + bias) (+ residual).  epi: 0 bias, 1 bias+GELU(erf), 2 bias+fp32 residual.
  * precision AC_PREC_TF32: X, W, Y fp32 (operands used as stored; round_out != 0 rounds Y to tf32);
