@@ -12,7 +12,7 @@ import math
 import threading
 import os
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int64, c_size_t, c_uint64, c_void_p
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 
@@ -26,7 +26,7 @@ AC_ACT_LOGITS, AC_ACT_SOFTMAX, AC_ACT_SIGMOID = 0, 1, 2
 AC_LOSS_CE, AC_LOSS_BCE, AC_LOSS_CE_STRATEGIC = 0, 1, 2
 AC_COST_LINEAR, AC_COST_SEPARABLE = 0, 1
 AC_STRATEGIC_CANDIDATES = 50
-AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT, AC_ARCH_MPNET = 0, 1, 2, 3
+AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERTA = 0, 1, 2, 3, 4
 AC_ENCODER_MAX_S = 512
 AC_MODERNBERT_MAX_S = 8192
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
@@ -76,7 +76,8 @@ class EncoderConfig(Structure):
                 ("vocab", c_int), ("max_pos", c_int), ("type_vocab", c_int), ("pad_idx", c_int),
                 ("ln_eps", c_float), ("precision", c_int), ("max_tokens", c_int), ("cls_only", c_int),
                 ("sliding_window", c_int), ("layer_sliding", POINTER(ctypes.c_int32)),
-                ("rope_full", c_void_p), ("rope_sliding", c_void_p), ("rel_bias", c_void_p)]
+                ("rope_full", c_void_p), ("rope_sliding", c_void_p), ("rel_bias", c_void_p),
+                ("pos_key", c_void_p), ("pos_query", c_void_p), ("pos_span", c_int), ("rel_index", c_void_p)]
 
 
 _PP = POINTER(c_void_p)
@@ -603,6 +604,97 @@ def mpnet_to_bert_state_dict(sd: dict, c):
     return out, dims
 
 
+def deberta_rel_index(position_buckets: int, max_relative_positions: int) -> Tuple[torch.Tensor, int]:
+    """(rel_index, span) of ac_encoder_config: int32 [2 AC_ENCODER_MAX_S - 1] with entry AC_ENCODER_MAX_S - 1 + r =
+    c(r) = clamp(bucket(r) + span, 0, 2 span - 1) for r = query - key, with HF build_relative_position's arithmetic
+    (make_log_bucket_position: identity below span / 2, log-spaced up to max_relative_positions; no buckets when either
+    setting is < 1), span = position_buckets, or max_relative_positions without buckets."""
+    r = torch.arange(-(AC_ENCODER_MAX_S - 1), AC_ENCODER_MAX_S, dtype=torch.long)
+    if position_buckets > 0 and max_relative_positions > 0:
+        sign = torch.sign(r)
+        mid = position_buckets // 2
+        abs_pos = torch.where((r < mid) & (r > -mid), torch.tensor(mid - 1).type_as(r), torch.abs(r))
+        log_pos = torch.ceil(torch.log(abs_pos / mid) / torch.log(torch.tensor((max_relative_positions - 1) / mid))
+                             * (mid - 1)) + mid
+        r = torch.where(abs_pos <= mid, r.type_as(log_pos), log_pos * sign).to(torch.long)
+    span = position_buckets if position_buckets > 0 else max_relative_positions
+    return torch.clamp(r + span, 0, 2 * span - 1).to(torch.int32), span
+
+
+def deberta_settings(c) -> None:
+    """Raises AdaptiveB200Error naming any DebertaV2Config setting the CUDA path does not implement (no device call)."""
+    heads = c.num_attention_heads
+    head_dim = getattr(c, "attention_head_size", None) or (c.hidden_size // heads if heads > 0 else 0)
+    pat = c.pos_att_type if c.pos_att_type is not None else []
+    pat = [x.strip() for x in pat.lower().split("|")] if isinstance(pat, str) else list(pat)
+    refusals = [
+        (getattr(c, "conv_kernel_size", 0) > 0,
+         f"conv_kernel_size={getattr(c, 'conv_kernel_size', 0)}: the ConvLayer of deberta-v2-xlarge/xxlarge"),
+        (getattr(c, "embedding_size", c.hidden_size) != c.hidden_size,
+         f"embedding_size={getattr(c, 'embedding_size', None)} != hidden_size={c.hidden_size}: the embed_proj"),
+        (not getattr(c, "relative_attention", False), "relative_attention=False"),
+        (len(pat) != 2 or set(pat) != {"c2p", "p2c"}, f"pos_att_type={pat!r}: only exactly ['c2p', 'p2c']"),
+        (c.hidden_act != "gelu", f"hidden_act={c.hidden_act!r}: only exact-erf 'gelu'"),
+        (head_dim != 64 or c.hidden_size != 64 * heads,
+         f"head_dim={head_dim} (hidden={c.hidden_size}, heads={heads}, attention_head_size="
+         f"{getattr(c, 'attention_head_size', None)}): only head_dim 64"),
+        (c.max_position_embeddings > AC_ENCODER_MAX_S,
+         f"max_position_embeddings={c.max_position_embeddings}: at most {AC_ENCODER_MAX_S}"),
+    ]
+    for bad, what in refusals:
+        if bad:
+            raise AdaptiveB200Error(f"DeBERTa {what} is not implemented in the CUDA path")
+
+
+def deberta_to_bert_state_dict(sd: dict, c):
+    """DeBERTa-v2 / v3 (HF models/deberta_v2/modeling_deberta_v2.py) is the post-LN BERT block with disentangled attention:
+    rename its parameters to the BERT names the encoder consumes, supply all-zero position (BERT ids) and single-row type
+    tables where the checkpoint has none (position_biased_input off, type_vocab_size 0), and build the per-layer fp32
+    position tables pos_key / pos_query [layers, 2 span, H] (from the encoder's rel_embeddings, LayerNorm-ed under
+    norm_rel_ebd = layer_norm, through key_proj / query_proj or pos_key_proj / pos_query_proj) and rel_index
+    (deberta_rel_index).  Raises AdaptiveB200Error naming any setting the CUDA path does not implement."""
+    deberta_settings(c)
+    H, L = c.hidden_size, c.num_hidden_layers
+    f32 = lambda t: t.detach().to(device="cpu", dtype=torch.float32)
+    out = {k: sd[k] for k in ("embeddings.word_embeddings.weight", "embeddings.LayerNorm.weight",
+                              "embeddings.LayerNorm.bias")}
+    out["embeddings.position_embeddings.weight"] = (
+        sd["embeddings.position_embeddings.weight"] if getattr(c, "position_biased_input", True)
+        else torch.zeros((c.max_position_embeddings, H), dtype=torch.float32))
+    out["embeddings.token_type_embeddings.weight"] = (
+        sd["embeddings.token_type_embeddings.weight"] if c.type_vocab_size > 0 else torch.zeros((1, H), dtype=torch.float32))
+    ren = {"attention.self.query_proj": "attention.self.query", "attention.self.key_proj": "attention.self.key",
+           "attention.self.value_proj": "attention.self.value", "attention.output.dense": "attention.output.dense",
+           "attention.output.LayerNorm": "attention.output.LayerNorm", "intermediate.dense": "intermediate.dense",
+           "output.dense": "output.dense", "output.LayerNorm": "output.LayerNorm"}
+    for l in range(L):
+        for src, dst in ren.items():
+            for wb in ("weight", "bias"):
+                out[f"encoder.layer.{l}.{dst}.{wb}"] = sd[f"encoder.layer.{l}.{src}.{wb}"]
+    buckets = getattr(c, "position_buckets", -1)
+    max_rel = getattr(c, "max_relative_positions", -1)
+    if max_rel < 1:
+        max_rel = c.max_position_embeddings
+    rel_index, span = deberta_rel_index(buckets, max_rel)
+    rel = f32(sd["encoder.rel_embeddings.weight"])
+    norm = [x.strip() for x in getattr(c, "norm_rel_ebd", "none").lower().split("|")]
+    if "layer_norm" in norm:
+        rel = torch.nn.functional.layer_norm(rel, (H,), f32(sd["encoder.LayerNorm.weight"]),
+                                             f32(sd["encoder.LayerNorm.bias"]), c.layer_norm_eps)
+    rel = rel[:2 * span]
+    share = getattr(c, "share_att_key", False)
+    pk, pq = [], []
+    for l in range(L):
+        p = f"encoder.layer.{l}.attention.self."
+        kname, qname = ("key_proj", "query_proj") if share else ("pos_key_proj", "pos_query_proj")
+        pk.append(torch.nn.functional.linear(rel, f32(sd[p + kname + ".weight"]), f32(sd[p + kname + ".bias"])))
+        pq.append(torch.nn.functional.linear(rel, f32(sd[p + qname + ".weight"]), f32(sd[p + qname + ".bias"])))
+    dims = dict(layers=L, hidden=H, heads=c.num_attention_heads, intermediate=c.intermediate_size, vocab=c.vocab_size,
+                max_pos=c.max_position_embeddings, type_vocab=max(c.type_vocab_size, 1), ln_eps=c.layer_norm_eps,
+                pad_idx=0, pos_key=torch.stack(pk), pos_query=torch.stack(pq), pos_span=span, rel_index=rel_index)
+    return out, dims
+
+
 def check_head_dim(hidden: int, heads: int, what: str = "encoder") -> None:
     """The attention kernels of the BERT-family encoder take head_dim = hidden / heads of 64 (bert-base, RoBERTa, DistilBERT)
     or 32 (all-MiniLM, BGE-small, E5-small, GTE-small); raises AdaptiveB200Error naming anything else (no device call)."""
@@ -662,12 +754,15 @@ def modernbert_settings(c) -> dict:
 class Encoder:
     """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors).  arch "mpnet"
     takes the BERT names (mpnet_to_bert_state_dict) and rel_bias, the [heads, 2 AC_ENCODER_MAX_S - 1] table of
-    mpnet_relative_bias_table."""
+    mpnet_relative_bias_table; arch "deberta" the BERT names and the pos_key / pos_query / pos_span / rel_index of
+    deberta_to_bert_state_dict."""
 
     def __init__(self, sd: dict, *, arch: str, layers: int, hidden: int, heads: int, intermediate: int, vocab: int,
                  max_pos: int = AC_ENCODER_MAX_S, type_vocab: int = 1, ln_eps: float, pad_idx: int = 0,
                  max_tokens: int = 65536, device="cuda", cls_only: bool = True, sliding_window: int = 0,
-                 layer_sliding=None, rope_theta=None, rel_bias: Optional[torch.Tensor] = None):
+                 layer_sliding=None, rope_theta=None, rel_bias: Optional[torch.Tensor] = None,
+                 pos_key: Optional[torch.Tensor] = None, pos_query: Optional[torch.Tensor] = None, pos_span: int = 0,
+                 rel_index: Optional[torch.Tensor] = None):
         L = load_library()
         self._L = L
         self.hidden = hidden
@@ -718,13 +813,19 @@ class Encoder:
             w.ff1_w, w.ff1_b = arr(p + "intermediate.dense.weight"), arr(p + "intermediate.dense.bias")
             w.ff2_w, w.ff2_b = arr(p + "output.dense.weight"), arr(p + "output.dense.bias")
             w.out_ln_w, w.out_ln_b = arr(p + "output.LayerNorm.weight"), arr(p + "output.LayerNorm.bias")
-            code = {"bert": AC_ARCH_BERT, "roberta": AC_ARCH_ROBERTA, "mpnet": AC_ARCH_MPNET}[arch]
+            code = {"bert": AC_ARCH_BERT, "roberta": AC_ARCH_ROBERTA, "mpnet": AC_ARCH_MPNET, "deberta": AC_ARCH_DEBERTA}[arch]
             cfg = EncoderConfig(code, layers, hidden, heads, intermediate, vocab, max_pos, type_vocab, pad_idx, ln_eps,
                                 AC_PREC_F16, max_tokens, 1 if cls_only else 0)
             if rel_bias is not None:      # ac_encoder_create refuses an MPNet encoder without it
                 rb = rel_bias.detach().to(device=dev, dtype=torch.float32).contiguous()
                 keep["rel_bias"] = rb
                 cfg.rel_bias = rb.data_ptr()
+            if arch == "deberta":         # ac_encoder_create refuses a DeBERTa encoder without its tables
+                pos = [t.detach().to(device=dev, dtype=dt).contiguous() if t is not None else None
+                       for t, dt in ((pos_key, torch.float32), (pos_query, torch.float32), (rel_index, torch.int32))]
+                keep["pos"] = pos
+                cfg.pos_key, cfg.pos_query, cfg.rel_index = (ptr(t) for t in pos)
+                cfg.pos_span = pos_span
         h = c_void_p()
         with torch.cuda.device(dev):
             check(L.ac_encoder_create(ctypes.byref(cfg), ctypes.byref(w), ctypes.byref(h)), "ac_encoder_create")
@@ -733,9 +834,9 @@ class Encoder:
 
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
-        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel (post-LN blocks) or
-        ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for BERT / RoBERTa / DistilBERT, 64
-        for MPNet and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
+        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel / DebertaV2Model (post-LN
+        blocks) or ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for BERT / RoBERTa /
+        DistilBERT, 64 for MPNet, DeBERTa and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
         AC_MODERNBERT_MAX_S."""
         c = model.config
         mt = getattr(c, "model_type", "bert")
@@ -746,6 +847,12 @@ class Encoder:
         if mt == "mpnet":
             sd, dims = mpnet_to_bert_state_dict(dict(model.state_dict()), c)
             return cls(sd, arch="mpnet", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
+        if mt == "deberta":
+            raise AdaptiveB200Error("encoder architecture model_type='deberta' (DeBERTa v1) is not implemented in the CUDA "
+                                    "path (DeBERTa-v2 / v3, model_type 'deberta-v2', is)")
+        if mt == "deberta-v2":
+            sd, dims = deberta_to_bert_state_dict(dict(model.state_dict()), c)
+            return cls(sd, arch="deberta", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
         if mt == "distilbert":
             check_head_dim(c.dim, c.n_heads, "DistilBERT")
             sd, dims = distilbert_to_bert_state_dict(dict(model.state_dict()), c)

@@ -844,11 +844,60 @@ static_assert(ATTS_SMEM <= 227 * 1024, "streamed attention CTA exceeds the share
 constexpr int ATTS_SMEM_BIAS = ATTS_SMEM + (AC_ENCODER_MAX_S + 128) * 4;   // + up to 639 staged relative-bias entries
 static_assert(ATTS_SMEM_BIAS <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
 
-template <int DH, bool BIAS = false>
+// DeBERTa disentangled attention (modeling_deberta_v2.py DisentangledSelfAttention), the DISENT instantiation of the streamed
+// kernel, which runs every DeBERTa sequence length (S <= 128 as one key block).  For query i and key j, r = i - j:
+//     s(i, j) = (q_i . k_j + q_i . PosK[c(r)] + k_j . PosQ[c(r)]) / sqrt(3 dh)
+// (HF gathers p2c at -bucket(j - i) + span, which is c(r) because the log bucket is odd).  In the tile of query block q0
+// and key block k0, with a = i - q0, b = j - k0 and delta = q0 - k0, r = delta + a - b takes 255 values.  The ac_encoder
+// holds, per (layer, delta, head), two fp16 boxes of 256 rows x 64 (ac_encoder::pos_g, built by pos_gather_kernel):
+//     c2p  G[t] = PosK[c(delta + t - 127)]    C = Q G^T    (a, t) -> score (a, b = a - t + 127)
+//     p2c  G[u] = PosQ[c(delta + 127 - u)]    C = K G^T    (b, u) -> score (a = b - u + 127, b)
+// Each product is 2 x 2 wgmma m64n128k64 (query / key rows 0-63, 64-127 by G rows 0-127, 128-255) whose fragments are
+// added straight into the fp32 score tile: every fragment element lands on at most one score and every score receives
+// exactly one element per term, so a pass needs no atomics (the two passes are separated by a barrier).  Row 255 of a box
+// is zero and never lands.  delta = 128 (blockIdx.y - key block) is one of 7 values for S <= 512.
+// smem: the c2p box has its own 32 KB; the p2c box goes through the P slabs, free between PV and the next softmax.
+constexpr int ATTS_POS_DELTAS = 2 * (AC_ENCODER_MAX_S / 128) - 1;
+constexpr int ATTS_OFF_G = (ATTS_OFF_S + ATT_S_BYTES + 128 * 4 + 4 * 8 + 1023) / 1024 * 1024;
+constexpr int ATTS_SMEM_DISENT = ATTS_OFF_G + 2 * ATTS_STAGE_BYTES + 1024 /*align*/;
+static_assert(ATTS_SMEM_DISENT <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
+
+// C = A G^T of one relative term over the 128 A rows (sA: Q or this key block's K) and the 256-row box sG, added into the
+// score tile: c2p (P2C false) at (row, row - n + 127), p2c at (row - n + 127, row); n = the box row of the product column
+template <bool P2C>
+__device__ __forceinline__ void att_rel_term(const uint8_t *sA, const uint8_t *sG, float *sS) {
+    const int t = threadIdx.x & 127;
+    const int r0 = 16 * (t >> 5) + ((t & 31) >> 2), c0 = 2 * (t & 3);
+#pragma unroll 1
+    for (int half = 0; half < 2; ++half) {
+#pragma unroll 1
+        for (int nc = 0; nc < 2; ++nc) {
+            float c[64];
+            const uint64_t a = wgmma_desc_sw128(smem_u32(sA + half * 8192));
+            const uint64_t bd = wgmma_desc_sw128(smem_u32(sG + nc * 16384));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(c, a + 2 * k, bd + 2 * k, k != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int j = 0; j < 64; ++j) {
+                const int row = 64 * half + r0 + 8 * ((j >> 1) & 1);
+                const int other = row - (128 * nc + 8 * (j >> 2) + c0 + (j & 1)) + 127;
+                if (other >= 0 && other < 128) {
+                    float *dst = P2C ? sS + other * ATT_S_LD + row : sS + row * ATT_S_LD + other;
+                    *dst += c[j];
+                }
+            }
+        }
+    }
+}
+
+template <int DH, bool BIAS = false, bool DISENT = false>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
                         const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx,
-                        const float *__restrict__ rel_bias) {
+                        const float *__restrict__ rel_bias, const __grid_constant__ CUtensorMap tmap_pos, int pos_row0) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                              // [128 x 128 B]
@@ -880,17 +929,34 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         tma_load_2d(sVt + st * ATTS_STAGE_BYTES, &tmap_vt, bar + st, key0, vrow);
         tma_load_2d(sVt + st * ATTS_STAGE_BYTES + 8192, &tmap_vt, bar + st, key0 + 64, vrow);
     };
+    // DISENT: the c2p box of visit i -> sG (barrier 2), the p2c box -> the P slabs (barrier 3); window 0, so kb0 = 0
+    uint8_t *sG = smem + ATTS_OFF_G;
+    auto issue_pos = [&](int i, int term) {
+        const int row = pos_row0 + (((static_cast<int>(blockIdx.y) - i + ATTS_POS_DELTAS / 2) * heads + h) * 2 + term) * 256;
+        uint8_t *dst = term ? sP : sG;
+        mbar_arrive_expect_tx(bar + 2 + term, 2 * ATTS_STAGE_BYTES);
+        tma_load_2d(dst, &tmap_pos, bar + 2 + term, 0, row);
+        tma_load_2d(dst + ATTS_STAGE_BYTES, &tmap_pos, bar + 2 + term, 0, row + 128);
+    };
     if (tid == 0) {
         tma_prefetch_desc(&tmap_qk);
         tma_prefetch_desc(&tmap_vt);
         mbar_init(bar, 1);
         mbar_init(bar + 1, 1);
+        if constexpr (DISENT) {
+            mbar_init(bar + 2, 1);
+            mbar_init(bar + 3, 1);
+        }
         fence_mbar_init();
     }
     __syncthreads();
     if (tid == 0) {
         issue(0);
         if (nblk > 1) issue(1);
+        if constexpr (DISENT) {
+            issue_pos(0, 0);
+            issue_pos(0, 1);
+        }
     }
     float *sB = reinterpret_cast<float *>(bar + 2);               // BIAS (window 0, so kb0 = 0): 128 nblk + 127 entries
     if constexpr (BIAS) att_stage_bias(rel_bias + h * (2 * AC_ENCODER_MAX_S - 1), q0, 128 * nblk, sB, tid);
@@ -898,7 +964,7 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
     const int qrow = warp * 32 + lane;                            // row inside the query block
     const int qglob = q0 + qrow;                                  // position inside the sequence
     const float *srow = sS + qrow * ATT_S_LD;
-    const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
+    const float scale_log2 = rsqrtf(static_cast<float>(DISENT ? 3 * DH : DH)) * 1.44269504088896340736f;
     const float sl2 = BIAS ? 1.f : scale_log2;                    // BIAS: att_add_bias has scaled the row already
     const int frow = 16 * warp + (lane >> 2);                     // accumulator fragment rows frow, frow + 8 (+ 64)
     const uint32_t sp_base = smem_u32(sP);
@@ -915,6 +981,15 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         mbar_wait_guarded(bar + st, (i >> 1) & 1);
         att_scores<DH>(sQ, sK + st * ATTS_STAGE_BYTES, sS);
         __syncthreads();
+        if constexpr (DISENT) {
+            mbar_wait_guarded(bar + 2, i & 1);
+            att_rel_term<false>(sQ, sG, sS);
+            __syncthreads();                                      // c2p added; sG is free
+            if (tid == 0 && i + 1 < nblk) issue_pos(i + 1, 0);
+            mbar_wait_guarded(bar + 3, i & 1);
+            att_rel_term<true>(sK + st * ATTS_STAGE_BYTES, sP, sS);
+            __syncthreads();                                      // p2c added; the P slabs are free
+        }
 
         uint32_t kmask[4];
         att_key_bits(mask, row0, S, key0, qglob, window, lane, kmask);
@@ -962,6 +1037,9 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         att_pv<DH>(sP, sVt + st * ATTS_STAGE_BYTES, o, true);
         __syncthreads();                                          // stage st, P, the score tile and the factors are free
         if (tid == 0 && i + 2 < nblk) issue(i + 2);
+        if constexpr (DISENT) {
+            if (tid == 0 && i + 1 < nblk) issue_pos(i + 1, 1);
+        }
     }
 
     wgmma_store_acc(o[0], sS, ATT_S_LD);
@@ -987,6 +1065,29 @@ __global__ void gather_cls_ln_kernel(const __half *__restrict__ ctx, const float
     for (int i = 0; i < LN_MAXV; ++i)
         if (i < nv) x[i] = *reinterpret_cast<const float4 *>(y + src + (lane + 32 * i) * 4);
     ln_row(x, nv, H, g, b, eps, lane, x_cls + dst, nullptr);
+}
+
+// DeBERTa operand boxes of attention_stream_kernel<64, false, true> (see att_rel_term): row ((((l ATTS_POS_DELTAS + d) heads
+// + h) 2 + term) 256 + t) = fp16 (RNE) of PosK (term 0) / PosQ (term 1) [l, c(r), 64 h .. 64 h + 63] with delta = 128 (d - 3),
+// r = delta + t - 127 (c2p) or delta + 127 - t (p2c), c(r) = rel_index[AC_ENCODER_MAX_S - 1 + r]; row t = 255 is zero.
+// pos_key / pos_query [layers, 2 span, H] fp32.  64 threads per row, 4 rows per block.
+__global__ void pos_gather_kernel(const float *__restrict__ pos_key, const float *__restrict__ pos_query,
+                                  const int32_t *__restrict__ rel_index, int span, int heads, int H, __half *__restrict__ out) {
+    const int64_t row = static_cast<int64_t>(blockIdx.x) * 4 + (threadIdx.x >> 6);
+    const int col = threadIdx.x & 63;
+    const int t = static_cast<int>(row % 256), term = static_cast<int>((row / 256) % 2);
+    const int h = static_cast<int>((row / 512) % heads);
+    const int64_t ld = row / (512 * static_cast<int64_t>(heads));          // l ATTS_POS_DELTAS + d
+    const int d = static_cast<int>(ld % ATTS_POS_DELTAS);
+    const int64_t l = ld / ATTS_POS_DELTAS;
+    float v = 0.f;
+    if (t < 255) {
+        const int delta = 128 * (d - ATTS_POS_DELTAS / 2);
+        const int r = term ? delta + 127 - t : delta + t - 127;
+        const int c = min(max(rel_index[AC_ENCODER_MAX_S - 1 + r], 0), 2 * span - 1);
+        v = (term ? pos_query : pos_key)[(l * 2 * span + c) * H + 64 * h + col];
+    }
+    out[row * 64 + col] = __float2half_rn(v);
 }
 
 }  // namespace ac
@@ -1040,6 +1141,10 @@ struct ac_encoder {
     float *ones = nullptr, *zeros = nullptr;   // ones [H]; zeros [max(3H, 2I)]: beta / bias of the bias-free ModernBERT
     float *rope[2] = {nullptr, nullptr};       // ModernBERT RoPE tables [max_pos, 64] (full, sliding layers)
     float *rel_bias = nullptr;                 // MPNet relative position bias [heads, 2 AC_ENCODER_MAX_S - 1]; NULL otherwise
+    // DeBERTa c2p / p2c operand boxes [layers, ATTS_POS_DELTAS, heads, 2 (c2p, p2c), 256, 64] fp16 (pos_gather_kernel) and
+    // their 128-row-box map; NULL otherwise
+    __half *pos_g = nullptr;
+    CUtensorMap m_pos;
     std::vector<void *> allocs;
     int last_B = 0, last_S = 0;           // shape of the previous forward; its full hidden state (cls_only = 0) is in tmp
     bool last_cls_only = false;
@@ -1054,9 +1159,10 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
 
 // softmax(Q K^T / sqrt(head_dim) [+ MPNet relative bias] + mask) V out of e->qk / e->vT into e->ctx; window = sliding
 // half-window, 0 = full attention.  S <= 128 runs attention_kernel, longer sequences attention_stream_kernel over 128-query
-// blocks.  cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail), so only the first query block is
-// computed.
-static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, cudaStream_t s) {
+// blocks; DeBERTa runs attention_stream_kernel<64, false, true> at every length, with layer `layer`'s c2p / p2c boxes.
+// cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail), so only the first query block is computed.
+static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, int layer,
+                            cudaStream_t s) {
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden;
     const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create); 64 with a relative bias
@@ -1074,6 +1180,8 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, in
         AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
         AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      ATTS_SMEM_BIAS));
+        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     ATTS_SMEM_DISENT));
         if (dev >= 0 && dev < 64) att_attr[dev] = true;
     }
     // algorithmic flops over the keys each computed query attends to at the true sequence length (the 128-wide tiles do
@@ -1087,14 +1195,18 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, in
         keys = static_cast<double>(nq) * S;
     }
     const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * keys * dh, 0.0, s);
-    if (S <= 128) {
+    if (e->pos_g) {
+        const int pos_row0 = layer * ATTS_POS_DELTAS * c.heads * 2 * 256;
+        attention_stream_kernel<64, false, true><<<dim3(B * c.heads, q_blocks), ATT_THREADS, ATTS_SMEM_DISENT, s>>>(
+            e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx, nullptr, e->m_pos, pos_row0);
+    } else if (S <= 128) {
         auto kern = rb ? attention_kernel<64, true> : dh == 32 ? attention_kernel<32> : attention_kernel<64>;
         kern<<<B * c.heads, ATT_THREADS, rb ? ATT_SMEM_BIAS : ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H,
                                                                             window, e->ctx, rb);
     } else {
         auto kern = rb ? attention_stream_kernel<64, true> : dh == 32 ? attention_stream_kernel<32> : attention_stream_kernel<64>;
         kern<<<dim3(B * c.heads, q_blocks), ATT_THREADS, rb ? ATTS_SMEM_BIAS : ATTS_SMEM, s>>>(
-            e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx, rb);
+            e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx, rb, e->m_qk_att, 0);
     }
     prof_end(slot, s);
     AC_LAUNCH_CHECK();
@@ -1168,6 +1280,11 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     const bool mp = cfg->arch == AC_ARCH_MPNET;
     AC_REQUIRE(!mp || (cfg->rel_bias && cfg->hidden == 64 * cfg->heads),
                "ac_encoder_create: MPNet needs rel_bias and head_dim 64 (hidden=%d heads=%d)", cfg->hidden, cfg->heads);
+    const bool db = cfg->arch == AC_ARCH_DEBERTA;
+    AC_REQUIRE(!db || (cfg->pos_key && cfg->pos_query && cfg->rel_index && cfg->pos_span > 0 &&
+                       cfg->hidden == 64 * cfg->heads),
+               "ac_encoder_create: DeBERTa needs pos_key, pos_query, rel_index, pos_span > 0 (pos_span=%d) and head_dim 64 "
+               "(hidden=%d heads=%d)", cfg->pos_span, cfg->hidden, cfg->heads);
     AC_REQUIRE(cfg->intermediate % 64 == 0 && cfg->layers > 0 && cfg->max_tokens > 0, "ac_encoder_create: bad dims");
     int rc = ac_device_check();
     if (rc) return rc;
@@ -1180,6 +1297,8 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     e->cfg.layer_sliding = nullptr;   // copied into e->layers / e->rope below
     e->cfg.rope_full = e->cfg.rope_sliding = nullptr;
     e->cfg.rel_bias = nullptr;        // copied into e->rel_bias below
+    e->cfg.pos_key = e->cfg.pos_query = nullptr;   // gathered into e->pos_g below
+    e->cfg.rel_index = nullptr;
     // ones / zeros are filled with the other constants after packing; the bias-free ModernBERT roles point at zeros
     const int nzeros = std::max(3 * H, 2 * I);
     TRY(dev_alloc(e, &e->ones, H));
@@ -1219,6 +1338,14 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
         TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
         TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, H));
         if (mp) TRY(pack_f32(e, &e->rel_bias, cfg->rel_bias, static_cast<size_t>(cfg->heads) * (2 * AC_ENCODER_MAX_S - 1)));
+        if (db) {
+            const size_t rows = static_cast<size_t>(L) * ATTS_POS_DELTAS * cfg->heads * 2 * 256;
+            TRY(dev_alloc(e, &e->pos_g, rows * 64));
+            pos_gather_kernel<<<static_cast<unsigned>(rows / 4), 256>>>(cfg->pos_key, cfg->pos_query, cfg->rel_index,
+                                                                        cfg->pos_span, cfg->heads, H, e->pos_g);
+            TRY(check_cuda(cudaGetLastError(), "pos_gather_kernel"));
+            TRY(make_tmap_2d(&e->m_pos, e->pos_g, 2, rows, 64, 128, 128, 64));
+        }
         for (int l = 0; l < L; ++l) {
             Layer &ly = e->layers[l];
             // the fused QKV [3H, H] of layer l consumes the sums pending the output LayerNorm of layer l-1 (identity for
@@ -1338,7 +1465,7 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
                                  .ldy = 2 * H, .S = S, .rope = e->rope[ly.window ? 1 : 0]},
                           .vT = e->vT, .vt_col0 = 2 * H, .S_pad = S_pad, .H = H};
         if ((rc = launch_linear(e->m_xh, ly.m_wqkv, M, 3 * H, H, eq, s))) return rc;
-        if ((rc = launch_attention(e, mask, B, S, ly.window, l == c.layers - 1 && cls_tail, s))) return rc;
+        if ((rc = launch_attention(e, mask, B, S, ly.window, l == c.layers - 1 && cls_tail, l, s))) return rc;
         if (l == c.layers - 1 && cls_tail) break;
         // attention output projection + residual: y <- ctx Wo^T + bo + LN_pending(y); statistics of the new sums
         EpiResidDefer eo{.bias = ly.bo, .y = e->x, .yh = e->xh, .stats_prev = pst, .gamma = pg, .beta = pb, .parts = e->parts,
@@ -1444,7 +1571,7 @@ extern "C" int ac_encoder_attention(ac_encoder *e, const void *qk, const void *v
     const size_t H = e->cfg.hidden, M = static_cast<size_t>(B) * S, S_pad = (S + 7) / 8 * 8;
     AC_CUDA(cudaMemcpyAsync(e->qk, qk, M * 2 * H * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     AC_CUDA(cudaMemcpyAsync(e->vT, vT, B * H * S_pad * sizeof(__half), cudaMemcpyDeviceToDevice, s));
-    if ((rc = launch_attention(e, mask, B, S, window, cls_rows != 0, s))) return rc;
+    if ((rc = launch_attention(e, mask, B, S, window, cls_rows != 0, 0, s))) return rc;
     AC_CUDA(cudaMemcpyAsync(ctx_out, e->ctx, M * H * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     return AC_OK;
 }

@@ -41,6 +41,22 @@ def mpnet_base(seed: int = 1234):
     return m, cfg
 
 
+def deberta_base(seed: int = 1234):
+    """HF DebertaV2Model of the microsoft/deberta-v3-base shape (12 x 768, 12 heads, I = 3072, vocab 128100, 256 position
+    buckets, share_att_key, LayerNorm-ed relative embeddings, no position or token-type table, LayerNorm eps 1e-7), random
+    init under torch.manual_seed(seed), with the relative embeddings drawn N(0, 1) (the init's std 0.02 goes through the
+    encoder's LayerNorm either way) so that the position terms move the scores."""
+    from transformers import DebertaV2Config, DebertaV2Model
+    torch.manual_seed(seed)
+    cfg = DebertaV2Config(vocab_size=128100, hidden_size=768, num_hidden_layers=12, num_attention_heads=12,
+                          intermediate_size=3072, max_position_embeddings=512, type_vocab_size=0, relative_attention=True,
+                          position_buckets=256, norm_rel_ebd="layer_norm", share_att_key=True, pos_att_type=["p2c", "c2p"],
+                          position_biased_input=False, layer_norm_eps=1e-7, hidden_act="gelu", pad_token_id=0)
+    m = DebertaV2Model(cfg)
+    m.eval()
+    return m, cfg
+
+
 def modernbert_ids(B: int, S: int, seed: int = 7) -> torch.Tensor:
     """uniform in [1000, 50000), [CLS]=50281 first, [SEP]=50282 last, never the pad id 50283; int32 [B,S] on the host."""
     g = torch.Generator().manual_seed(seed)

@@ -245,7 +245,9 @@ int ac_head_train_strategic(const float *X, const int64_t *targets, const int64_
  *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel / ModernBertModel forward).
  * ------------------------------------------------------------------------------------------ */
 enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2,
-       AC_ARCH_MPNET = 3 /* post-LN BERT block, RoBERTa positions, relative position bias (rel_bias); head_dim 64 */ };
+       AC_ARCH_MPNET = 3 /* post-LN BERT block, RoBERTa positions, relative position bias (rel_bias); head_dim 64 */,
+       AC_ARCH_DEBERTA = 4 /* DeBERTa-v2/v3: post-LN BERT block, BERT positions, disentangled c2p + p2c attention
+                              (pos_key, pos_query, pos_span, rel_index); head_dim 64 */ };
 #define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts for BERT / RoBERTa / DistilBERT (their
                                   position tables stop at 512) */
 #define AC_MODERNBERT_MAX_S 8192   /* largest max_pos of an AC_ARCH_MODERNBERT encoder (max_position_embeddings of the
@@ -259,7 +261,7 @@ enum {
 typedef struct {
     int arch;            /* AC_ARCH_* */
     int layers, hidden, heads, intermediate;   /* hidden % 128 == 0; head_dim = hidden / heads is 64 or 32
-                                                  (64 only for AC_ARCH_MODERNBERT and AC_ARCH_MPNET) */
+                                                  (64 only for AC_ARCH_MODERNBERT, AC_ARCH_MPNET and AC_ARCH_DEBERTA) */
     int vocab, max_pos, type_vocab;
     int pad_idx;         /* roberta, mpnet: position ids start at pad_idx+1 */
     float ln_eps;
@@ -278,6 +280,16 @@ typedef struct {
        entry (h, AC_ENCODER_MAX_S - 1 + key - query) is the bias every layer adds to head h's scaled score of (query, key)
        (HF MPNetEncoder.compute_position_bias: relative_attention_bias.weight[bucket(key - query), h], built by the caller) */
     const float *rel_bias;
+    /* AC_ARCH_DEBERTA only (ignored otherwise), read by ac_encoder_create, which gathers them into fp16 (RNE) attention
+       operands; all DEVICE.  For query i and key j, r = i - j, every layer l adds to the unscaled score q_i . k_j
+           q_i . pos_key[l, c(r), head]  +  k_j . pos_query[l, c(r), head]
+       and scales the sum by 1 / sqrt(3 head_dim) (HF DisentangledSelfAttention with pos_att_type c2p|p2c). */
+    const float *pos_key;        /* [layers, 2 pos_span, H] fp32: key_proj(rel) (share_att_key) or pos_key_proj(rel), with
+                                    rel = rel_embeddings (LayerNorm-ed when norm_rel_ebd = layer_norm), biases included */
+    const float *pos_query;      /* [layers, 2 pos_span, H] fp32: query_proj(rel) or pos_query_proj(rel) */
+    int pos_span;                /* position_buckets, or max_relative_positions without buckets */
+    const int32_t *rel_index;    /* [2 AC_ENCODER_MAX_S - 1] int32: entry AC_ENCODER_MAX_S - 1 + r is
+                                    c(r) = clamp(bucket(r) + pos_span, 0, 2 pos_span - 1) (HF build_relative_position) */
 } ac_encoder_config;
 
 /* device pointers to the HF state_dict tensors (fp32, HF layout [out,in]).
@@ -324,7 +336,8 @@ int ac_encoder_last_hidden(ac_encoder *enc, float *out, int64_t n_floats, ac_str
  * 0 = full; must be 0 unless AC_ARCH_MODERNBERT), cls_rows != 0 computes the first 128-query block only (later rows of
  * ctx_out are then unspecified).  ctx_out [B*S, H] fp16 = softmax(q k^T / sqrt(dh) + rel_bias + mask) v per head; a query
  * with no valid key in reach gets zeros.  Uses the encoder's heads, head_dim and rel_bias, and accepts and refuses the
- * shapes ac_encoder_forward_cls does.  All pointers DEVICE. */
+ * shapes ac_encoder_forward_cls does.  On an AC_ARCH_DEBERTA encoder the scores are those of layer 0: (q k^T + c2p + p2c)
+ * / sqrt(3 dh) with layer 0's pos_key / pos_query.  All pointers DEVICE. */
 int ac_encoder_attention(ac_encoder *enc, const void *qk, const void *vT, const int32_t *mask, int B, int S, int window,
                          int cls_rows, void *ctx_out, ac_stream_t stream);
 
