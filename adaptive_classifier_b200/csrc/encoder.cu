@@ -599,10 +599,10 @@ constexpr int ATT_THREADS = 128;
 constexpr int ATT_S_LD = 128 + 4;                            // score tile row stride (floats): conflict-free row reads
 constexpr int ATT_S_BYTES = 128 * ATT_S_LD * 4;
 constexpr int ATT_REGION_BYTES = (ATT_S_BYTES + 1023) / 1024 * 1024;
-constexpr int ATT_SMEM = ATT_REGION_BYTES + 16 * 1024 + 1024 /*align*/ + 64;
-static_assert(2 * (ATT_SMEM + 1024) <= 228 * 1024, "two attention CTAs must fit one SM");
-constexpr int ATT_SMEM_BIAS = ATT_SMEM + 1024;               // + the 255 staged relative-bias entries (MPNet)
-static_assert(2 * (ATT_SMEM_BIAS + 1024) <= 228 * 1024, "two attention CTAs must fit one SM");
+// after the region: V^T 16 KB | the load barrier (64 B) | the score term's own bytes (Score::SMEM_BLOCK)
+constexpr int ATT_OFF_VT = ATT_REGION_BYTES, ATT_OFF_BAR = ATT_OFF_VT + 16 * 1024, ATT_OFF_TERM = ATT_OFF_BAR + 64;
+template <class Score>
+constexpr int ATT_SMEM = ATT_OFF_TERM + Score::SMEM_BLOCK + 1024 /*align*/;
 
 // S[128 x 128] = Q K^T for the query tile sQ and key tile sK (both [128 rows x 128 B], 128B swizzle) -> sS (fp32, ld ATT_S_LD).
 // Issued by the whole warpgroup; returns once the products are in shared memory (the caller synchronises the CTA).
@@ -704,39 +704,81 @@ __device__ __forceinline__ void att_exp_pack(const float (&r)[32], uint32_t km, 
     }
 }
 
-// MPNet relative position bias (modeling_mpnet.py MPNetEncoder.compute_position_bias), the BIAS instantiations of both
-// kernels.  rel_bias row h holds the head's bias at entry (AC_ENCODER_MAX_S - 1) + key - q.  A CTA of queries q0 .. q0 + 127
-// and keys 0 .. nkeys - 1 stages entries from (AC_ENCODER_MAX_S - 128) - q0 on, times log2(e), so that query row qrow
-// (q = q0 + qrow) finds the bias of key at sB[127 - qrow + key]: 32 lanes read 32 consecutive words, conflict-free.
-constexpr int ATT_BIAS_OFS = AC_ENCODER_MAX_S - 128;
-__device__ __forceinline__ void att_stage_bias(const float *__restrict__ row, int q0, int nkeys, float *sB, int tid) {
-    for (int t = tid; t < nkeys + 127; t += ATT_THREADS) sB[t] = __ldg(row + ATT_BIAS_OFS - q0 + t) * 1.44269504088896340736f;
-}
-// scores of 32 keys -> ex2-domain logits s scale log2(e) + bias log2(e), which the softmax then uses with scale 1
-__device__ __forceinline__ void att_add_bias(float (&r)[32], const float *bq, float scale_log2) {
+// ---- score terms: what an encoder family adds to Q K^T before the softmax.  Both kernels take one as the `Score` template
+// parameter and kernel argument, and call its hooks at fixed points; a hook a family does not need is empty.
+// Where the calling CTA stands:
+struct AttCta {
+    uint8_t *smem;        // 1 KB-aligned base of the kernel's layout
+    uint8_t *term;        // the score term's own bytes behind that layout (ATT_OFF_TERM / ATTS_OFF_TERM)
+    int tid, h, heads;    // thread = query row of the block, head, heads of the encoder
+    int q0, nblk;         // first query of the block, key blocks it visits from key 0 (attention_kernel: 0, 1)
+};
+
+// BERT, RoBERTa, DistilBERT, MiniLM (DH 32), ModernBERT: softmax(Q K^T / sqrt(DH) + mask), nothing added
+struct ScorePlain {
+    static constexpr int MIN_DH = 32;             // head dimensions the term is written for: MIN_DH .. 64
+    static constexpr bool ONE_BLOCK = true;       // runs on attention_kernel as well as on attention_stream_kernel
+    static constexpr int SCALE_TERMS = 1;         // logits are scores / sqrt(SCALE_TERMS DH)
+    static constexpr bool EX2_ROWS = false;       // true: row() leaves ex2-domain logits, so the softmax scales by 1
+    static constexpr int SMEM_BLOCK = 0, SMEM_STREAM = 0;   // own bytes in attention_kernel / attention_stream_kernel
+    // the hooks, in call order.  init_barriers: thread 0, with the kernel's own barriers.  begin: every thread, once the
+    // barriers are visible (first loads into the term's bytes).  add_block_terms / after_pv: every thread, visit i of the
+    // streamed kernel, with the CTA synchronised after Q K^T reached the score tile / after P V retired (the P slabs are
+    // free).  row: the 32 scores of the thread's row from key `key` on, after every read of them.
+    __device__ __forceinline__ void init_barriers(const AttCta &) const {}
+    __device__ __forceinline__ void begin(const AttCta &) const {}
+    __device__ __forceinline__ void add_block_terms(const AttCta &, int) const {}
+    __device__ __forceinline__ void row(float (&)[32], const AttCta &, int, float) const {}
+    __device__ __forceinline__ void after_pv(const AttCta &, int) const {}
+};
+
+// MPNet relative position bias (modeling_mpnet.py MPNetEncoder.compute_position_bias), added to the scaled scores before
+// the mask (window 0).  rel_bias row h holds the head's bias at entry (AC_ENCODER_MAX_S - 1) + key - q.  A CTA of queries
+// q0 .. q0 + 127 and keys 0 .. 128 nblk - 1 stages entries from (AC_ENCODER_MAX_S - 128) - q0 on, times log2(e), so that
+// query row qrow (q = q0 + qrow) finds the bias of key at sB[127 - qrow + key]: 32 lanes read 32 consecutive words,
+// conflict-free.
+struct ScoreRelBias : ScorePlain {
+    const float *rel_bias;                        // [heads, 2 AC_ENCODER_MAX_S - 1]
+    static constexpr int MIN_DH = 64;
+    static constexpr bool EX2_ROWS = true;
+    static constexpr int ATT_BIAS_OFS = AC_ENCODER_MAX_S - 128;
+    // the staged entries: 255, and up to 128 (AC_ENCODER_MAX_S / 128) + 127
+    static constexpr int SMEM_BLOCK = 1024, SMEM_STREAM = (AC_ENCODER_MAX_S + 128) * 4;
+    __device__ __forceinline__ void begin(const AttCta &cta) const {
+        const float *row = rel_bias + cta.h * (2 * AC_ENCODER_MAX_S - 1);
+        float *sB = reinterpret_cast<float *>(cta.term);
+        for (int t = cta.tid; t < 128 * cta.nblk + 127; t += ATT_THREADS)
+            sB[t] = __ldg(row + ATT_BIAS_OFS - cta.q0 + t) * 1.44269504088896340736f;
+    }
+    // scores of 32 keys -> ex2-domain logits s scale log2(e) + bias log2(e)
+    __device__ __forceinline__ void row(float (&r)[32], const AttCta &cta, int key, float scale_log2) const {
+        const float *bq = reinterpret_cast<const float *>(cta.term) + 127 - cta.tid;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) r[j] = fmaf(r[j], scale_log2, bq[j]);
-}
+        for (int j = 0; j < 32; ++j) r[j] = fmaf(r[j], scale_log2, bq[key + j]);
+    }
+};
 
 // window: ModernBERT sliding_attention half-window (keys |q - key| <= window), 0 = full attention.
-// BIAS: rel_bias [heads, 2 AC_ENCODER_MAX_S - 1] is added to the scaled scores before the mask (MPNet; window 0)
-template <int DH, bool BIAS = false>
+template <int DH, class Score>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
                  const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx,
-                 const float *__restrict__ rel_bias) {
+                 const __grid_constant__ Score score) {
+    static_assert(Score::ONE_BLOCK && DH >= Score::MIN_DH, "score term not written for this kernel or head dimension");
+    static_assert(2 * (ATT_SMEM<Score> + 1024) <= 228 * 1024, "two attention CTAs must fit one SM");
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                    // [128 rows x 128 B]
     uint8_t *sK = smem + 16 * 1024;        // [128 rows x 128 B]
     float *sS = reinterpret_cast<float *>(smem);   // score tile, then output tile (after QK^T / PV retired)
     uint8_t *sP = smem;                    // 2 slabs x [128 rows x 128 B (64 keys)]   (after every score row was read)
-    uint8_t *sVt = smem + ATT_REGION_BYTES;  // 2 slabs x [64 rows (d) x 128 B (64 keys)]
-    uint64_t *bar_load = reinterpret_cast<uint64_t *>(smem + ATT_REGION_BYTES + 16 * 1024);
+    uint8_t *sVt = smem + ATT_OFF_VT;      // 2 slabs x [64 rows (d) x 128 B (64 keys)]
+    uint64_t *bar_load = reinterpret_cast<uint64_t *>(smem + ATT_OFF_BAR);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int b = blockIdx.x / heads, h = blockIdx.x % heads;
     const int64_t row0 = static_cast<int64_t>(b) * S;
+    const AttCta cta = {smem, smem + ATT_OFF_TERM, tid, h, heads, 0, 1};
 
     if (tid == 0) {
         tma_prefetch_desc(&tmap_qk);
@@ -754,8 +796,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
         tma_load_2d(sVt, &tmap_vt, bar_load, 0, vrow);
         tma_load_2d(sVt + 8 * 1024, &tmap_vt, bar_load, 64, vrow);
     }
-    float *sB = reinterpret_cast<float *>(smem + ATT_REGION_BYTES + 16 * 1024 + 64);   // BIAS: 255 entries
-    if constexpr (BIAS) att_stage_bias(rel_bias + h * (2 * AC_ENCODER_MAX_S - 1), 0, 128, sB, tid);
+    score.begin(cta);
     // ---- S = Q K^T: both 64-row chains retire before the score tile overwrites Q and K
     mbar_wait_guarded(bar_load, 0);
     {
@@ -780,15 +821,14 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     const float *srow = sS + qrow * ATT_S_LD;
     uint32_t kmask[4];
     att_key_bits(mask, row0, S, 0, qrow, window, lane, kmask);
-    const float scale_log2 = rsqrtf(static_cast<float>(DH)) * 1.44269504088896340736f;
-    const float sl2 = BIAS ? 1.f : scale_log2;   // BIAS: att_add_bias has scaled the row already
-    const float *bq = sB + 127 - qrow;
+    const float scale_log2 = rsqrtf(static_cast<float>(Score::SCALE_TERMS * DH)) * 1.44269504088896340736f;
+    const float sl2 = Score::EX2_ROWS ? 1.f : scale_log2;
     float mx = -CUDART_INF_F;
 #pragma unroll 1
     for (int c = 0; c < 128; c += 32) {
         float r[32];
         acc_row_ld32(srow + c, r);
-        if constexpr (BIAS) att_add_bias(r, bq + c, scale_log2);
+        score.row(r, cta, c, scale_log2);
         const uint32_t km = c == 0 ? kmask[0] : c == 32 ? kmask[1] : c == 64 ? kmask[2] : kmask[3];
 #pragma unroll
         for (int j = 0; j < 32; ++j)
@@ -800,7 +840,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
     for (int ci = 0; ci < 4; ++ci) {
         float r[32];
         acc_row_ld32(srow + 32 * ci, r);
-        if constexpr (BIAS) att_add_bias(r, bq + 32 * ci, scale_log2);
+        score.row(r, cta, 32 * ci, scale_log2);
         att_exp_pack(r, kmask[ci], sl2, mx * sl2, sum, pk + 16 * ci);
     }
     __syncthreads();                       // every score row has been read
@@ -834,18 +874,17 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_const
 //                 a sliding query block, holes in the mask) keeps m = -inf, P = 0 and a zero accumulator: the factor is
 //                 0 there rather than exp((-inf) - (-inf))
 //   P fp16, every accumulator fp32, as in the kernel above.  q_blocks = 1 (CLS-only tail next) computes rows 0..127 only.
-// smem: Q 16 KB | K 2 x 16 KB | V^T 2 x 16 KB | P 32 KB | score tile 66 KB | factors 512 B | 2 barriers (| BIAS: the staged
-// relative bias): one CTA per SM.
+// smem: Q 16 KB | K 2 x 16 KB | V^T 2 x 16 KB | P 32 KB | score tile 66 KB | factors 512 B | 2 barriers | the score term's
+// own bytes (Score::SMEM_STREAM): one CTA per SM.
 // ------------------------------------------------------------------------------------------------
 constexpr int ATTS_STAGE_BYTES = 16 * 1024;
 constexpr int ATTS_OFF_K = 16 * 1024, ATTS_OFF_VT = 48 * 1024, ATTS_OFF_P = 80 * 1024, ATTS_OFF_S = 112 * 1024;
-constexpr int ATTS_SMEM = ATTS_OFF_S + ATT_S_BYTES + 128 * 4 + 2 * 8 + 1024 /*align*/;
-static_assert(ATTS_SMEM <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
-constexpr int ATTS_SMEM_BIAS = ATTS_SMEM + (AC_ENCODER_MAX_S + 128) * 4;   // + up to 639 staged relative-bias entries
-static_assert(ATTS_SMEM_BIAS <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
+constexpr int ATTS_OFF_BAR = ATTS_OFF_S + ATT_S_BYTES + 128 * 4, ATTS_OFF_TERM = ATTS_OFF_BAR + 2 * 8;
+template <class Score>
+constexpr int ATTS_SMEM = ATTS_OFF_TERM + Score::SMEM_STREAM + 1024 /*align*/;
 
-// DeBERTa disentangled attention (modeling_deberta_v2.py DisentangledSelfAttention), the DISENT instantiation of the streamed
-// kernel, which runs every DeBERTa sequence length (S <= 128 as one key block).  For query i and key j, r = i - j:
+// DeBERTa disentangled attention (modeling_deberta_v2.py DisentangledSelfAttention), on the streamed kernel only, which
+// runs every DeBERTa sequence length (S <= 128 as one key block).  For query i and key j, r = i - j:
 //     s(i, j) = (q_i . k_j + q_i . PosK[c(r)] + k_j . PosQ[c(r)]) / sqrt(3 dh)
 // (HF gathers p2c at -bucket(j - i) + span, which is c(r) because the log bucket is odd).  In the tile of query block q0
 // and key block k0, with a = i - q0, b = j - k0 and delta = q0 - k0, r = delta + a - b takes 255 values.  The ac_encoder
@@ -858,9 +897,6 @@ static_assert(ATTS_SMEM_BIAS <= 227 * 1024, "streamed attention CTA exceeds the 
 // is zero and never lands.  delta = 128 (blockIdx.y - key block) is one of 7 values for S <= 512.
 // smem: the c2p box has its own 32 KB; the p2c box goes through the P slabs, free between PV and the next softmax.
 constexpr int ATTS_POS_DELTAS = 2 * (AC_ENCODER_MAX_S / 128) - 1;
-constexpr int ATTS_OFF_G = (ATTS_OFF_S + ATT_S_BYTES + 128 * 4 + 4 * 8 + 1023) / 1024 * 1024;
-constexpr int ATTS_SMEM_DISENT = ATTS_OFF_G + 2 * ATTS_STAGE_BYTES + 1024 /*align*/;
-static_assert(ATTS_SMEM_DISENT <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
 
 // C = A G^T of one relative term over the 128 A rows (sA: Q or this key block's K) and the 256-row box sG, added into the
 // score tile: c2p (P2C false) at (row, row - n + 127), p2c at (row - n + 127, row); n = the box row of the product column
@@ -893,11 +929,58 @@ __device__ __forceinline__ void att_rel_term(const uint8_t *sA, const uint8_t *s
     }
 }
 
-template <int DH, bool BIAS = false, bool DISENT = false>
+struct ScoreDisent : ScorePlain {
+    CUtensorMap tmap_pos;                         // 128-row boxes over ac_encoder::pos_g
+    int pos_row0;                                 // first row of the layer's boxes
+    static constexpr int MIN_DH = 64;
+    static constexpr bool ONE_BLOCK = false;
+    static constexpr int SCALE_TERMS = 3;
+    // own bytes: two barriers (the c2p box has landed, the p2c box has), then the c2p box at the layout's next 1 KB boundary
+    static constexpr int OFF_G = (ATTS_OFF_TERM + 2 * 8 + 1023) / 1024 * 1024 - ATTS_OFF_TERM;
+    static constexpr int SMEM_STREAM = OFF_G + 2 * ATTS_STAGE_BYTES;
+    // the c2p (term 0) / p2c (term 1) box of visit i -> its own 32 KB / the P slabs; window 0, so visit i is key block i
+    __device__ __forceinline__ void issue_pos(const AttCta &cta, int i, int term) const {
+        const int row =
+            pos_row0 + (((static_cast<int>(blockIdx.y) - i + ATTS_POS_DELTAS / 2) * cta.heads + cta.h) * 2 + term) * 256;
+        uint64_t *bar = reinterpret_cast<uint64_t *>(cta.term) + term;
+        uint8_t *dst = term ? cta.smem + ATTS_OFF_P : cta.term + OFF_G;
+        mbar_arrive_expect_tx(bar, 2 * ATTS_STAGE_BYTES);
+        tma_load_2d(dst, &tmap_pos, bar, 0, row);
+        tma_load_2d(dst + ATTS_STAGE_BYTES, &tmap_pos, bar, 0, row + 128);
+    }
+    __device__ __forceinline__ void init_barriers(const AttCta &cta) const {
+        mbar_init(reinterpret_cast<uint64_t *>(cta.term), 1);
+        mbar_init(reinterpret_cast<uint64_t *>(cta.term) + 1, 1);
+    }
+    __device__ __forceinline__ void begin(const AttCta &cta) const {
+        if (cta.tid == 0) {
+            issue_pos(cta, 0, 0);
+            issue_pos(cta, 0, 1);
+        }
+    }
+    __device__ __forceinline__ void add_block_terms(const AttCta &cta, int i) const {
+        uint64_t *bar = reinterpret_cast<uint64_t *>(cta.term);
+        float *sS = reinterpret_cast<float *>(cta.smem + ATTS_OFF_S);
+        mbar_wait_guarded(bar, i & 1);
+        att_rel_term<false>(cta.smem, cta.term + OFF_G, sS);
+        __syncthreads();                                          // c2p added; its box is free
+        if (cta.tid == 0 && i + 1 < cta.nblk) issue_pos(cta, i + 1, 0);
+        mbar_wait_guarded(bar + 1, i & 1);
+        att_rel_term<true>(cta.smem + ATTS_OFF_K + (i & 1) * ATTS_STAGE_BYTES, cta.smem + ATTS_OFF_P, sS);
+        __syncthreads();                                          // p2c added; the P slabs are free
+    }
+    __device__ __forceinline__ void after_pv(const AttCta &cta, int i) const {
+        if (cta.tid == 0 && i + 1 < cta.nblk) issue_pos(cta, i + 1, 1);
+    }
+};
+
+template <int DH, class Score>
 __global__ void __launch_bounds__(ATT_THREADS)
 attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
                         const int32_t *__restrict__ mask, int B, int S, int heads, int H, int window, __half *__restrict__ ctx,
-                        const float *__restrict__ rel_bias, const __grid_constant__ CUtensorMap tmap_pos, int pos_row0) {
+                        const __grid_constant__ Score score) {
+    static_assert(DH >= Score::MIN_DH, "score term not written for this head dimension");
+    static_assert(ATTS_SMEM<Score> <= 227 * 1024, "streamed attention CTA exceeds the shared-memory limit");
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t *sQ = smem;                              // [128 x 128 B]
@@ -906,7 +989,7 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
     uint8_t *sP = smem + ATTS_OFF_P;                 // 2 slabs x [128 x 128 B (64 keys)]
     float *sS = reinterpret_cast<float *>(smem + ATTS_OFF_S);
     float *sAlpha = sS + 128 * ATT_S_LD;             // [128] rescale factor of each query row
-    uint64_t *bar = reinterpret_cast<uint64_t *>(sAlpha + 128);
+    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + ATTS_OFF_BAR);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int b = blockIdx.x / heads, h = blockIdx.x % heads;
@@ -919,6 +1002,7 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         kb1 = min(q0 + 127 + window, S - 1) / 128 + 1;
     }
     const int nblk = kb1 - kb0;
+    const AttCta cta = {smem, smem + ATTS_OFF_TERM, tid, h, heads, q0, nblk};
 
     // visit i -> stage i & 1; the first visit also brings Q
     auto issue = [&](int i) {
@@ -929,43 +1013,26 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         tma_load_2d(sVt + st * ATTS_STAGE_BYTES, &tmap_vt, bar + st, key0, vrow);
         tma_load_2d(sVt + st * ATTS_STAGE_BYTES + 8192, &tmap_vt, bar + st, key0 + 64, vrow);
     };
-    // DISENT: the c2p box of visit i -> sG (barrier 2), the p2c box -> the P slabs (barrier 3); window 0, so kb0 = 0
-    uint8_t *sG = smem + ATTS_OFF_G;
-    auto issue_pos = [&](int i, int term) {
-        const int row = pos_row0 + (((static_cast<int>(blockIdx.y) - i + ATTS_POS_DELTAS / 2) * heads + h) * 2 + term) * 256;
-        uint8_t *dst = term ? sP : sG;
-        mbar_arrive_expect_tx(bar + 2 + term, 2 * ATTS_STAGE_BYTES);
-        tma_load_2d(dst, &tmap_pos, bar + 2 + term, 0, row);
-        tma_load_2d(dst + ATTS_STAGE_BYTES, &tmap_pos, bar + 2 + term, 0, row + 128);
-    };
     if (tid == 0) {
         tma_prefetch_desc(&tmap_qk);
         tma_prefetch_desc(&tmap_vt);
         mbar_init(bar, 1);
         mbar_init(bar + 1, 1);
-        if constexpr (DISENT) {
-            mbar_init(bar + 2, 1);
-            mbar_init(bar + 3, 1);
-        }
+        score.init_barriers(cta);
         fence_mbar_init();
     }
     __syncthreads();
     if (tid == 0) {
         issue(0);
         if (nblk > 1) issue(1);
-        if constexpr (DISENT) {
-            issue_pos(0, 0);
-            issue_pos(0, 1);
-        }
     }
-    float *sB = reinterpret_cast<float *>(bar + 2);               // BIAS (window 0, so kb0 = 0): 128 nblk + 127 entries
-    if constexpr (BIAS) att_stage_bias(rel_bias + h * (2 * AC_ENCODER_MAX_S - 1), q0, 128 * nblk, sB, tid);
+    score.begin(cta);
 
     const int qrow = warp * 32 + lane;                            // row inside the query block
     const int qglob = q0 + qrow;                                  // position inside the sequence
     const float *srow = sS + qrow * ATT_S_LD;
-    const float scale_log2 = rsqrtf(static_cast<float>(DISENT ? 3 * DH : DH)) * 1.44269504088896340736f;
-    const float sl2 = BIAS ? 1.f : scale_log2;                    // BIAS: att_add_bias has scaled the row already
+    const float scale_log2 = rsqrtf(static_cast<float>(Score::SCALE_TERMS * DH)) * 1.44269504088896340736f;
+    const float sl2 = Score::EX2_ROWS ? 1.f : scale_log2;
     const int frow = 16 * warp + (lane >> 2);                     // accumulator fragment rows frow, frow + 8 (+ 64)
     const uint32_t sp_base = smem_u32(sP);
     float mx = -CUDART_INF_F, sum = 0.f;
@@ -981,25 +1048,16 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         mbar_wait_guarded(bar + st, (i >> 1) & 1);
         att_scores<DH>(sQ, sK + st * ATTS_STAGE_BYTES, sS);
         __syncthreads();
-        if constexpr (DISENT) {
-            mbar_wait_guarded(bar + 2, i & 1);
-            att_rel_term<false>(sQ, sG, sS);
-            __syncthreads();                                      // c2p added; sG is free
-            if (tid == 0 && i + 1 < nblk) issue_pos(i + 1, 0);
-            mbar_wait_guarded(bar + 3, i & 1);
-            att_rel_term<true>(sK + st * ATTS_STAGE_BYTES, sP, sS);
-            __syncthreads();                                      // p2c added; the P slabs are free
-        }
+        score.add_block_terms(cta, i);
 
         uint32_t kmask[4];
         att_key_bits(mask, row0, S, key0, qglob, window, lane, kmask);
-        const float *bq = sB + 127 - qrow + key0;
         float bmx = -CUDART_INF_F;
 #pragma unroll
         for (int ci = 0; ci < 4; ++ci) {
             float r[32];
             acc_row_ld32(srow + 32 * ci, r);
-            if constexpr (BIAS) att_add_bias(r, bq + 32 * ci, scale_log2);
+            score.row(r, cta, key0 + 32 * ci, scale_log2);
 #pragma unroll
             for (int jj = 0; jj < 32; ++jj)
                 if ((kmask[ci] >> jj) & 1u) bmx = fmaxf(bmx, r[jj]);
@@ -1012,7 +1070,7 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         for (int ci = 0; ci < 4; ++ci) {
             float r[32];
             acc_row_ld32(srow + 32 * ci, r);
-            if constexpr (BIAS) att_add_bias(r, bq + 32 * ci, scale_log2);
+            score.row(r, cta, key0 + 32 * ci, scale_log2);
             uint32_t pk[16];
             att_exp_pack(r, kmask[ci], sl2, mxs, bsum, pk);
             att_store_p(sp_base, qrow, 32 * ci, pk);
@@ -1037,9 +1095,7 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
         att_pv<DH>(sP, sVt + st * ATTS_STAGE_BYTES, o, true);
         __syncthreads();                                          // stage st, P, the score tile and the factors are free
         if (tid == 0 && i + 2 < nblk) issue(i + 2);
-        if constexpr (DISENT) {
-            if (tid == 0 && i + 1 < nblk) issue_pos(i + 1, 1);
-        }
+        score.after_pv(cta, i);
     }
 
     wgmma_store_acc(o[0], sS, ATT_S_LD);
@@ -1067,7 +1123,7 @@ __global__ void gather_cls_ln_kernel(const __half *__restrict__ ctx, const float
     ln_row(x, nv, H, g, b, eps, lane, x_cls + dst, nullptr);
 }
 
-// DeBERTa operand boxes of attention_stream_kernel<64, false, true> (see att_rel_term): row ((((l ATTS_POS_DELTAS + d) heads
+// DeBERTa operand boxes of attention_stream_kernel<64, ScoreDisent> (see att_rel_term): row ((((l ATTS_POS_DELTAS + d) heads
 // + h) 2 + term) 256 + t) = fp16 (RNE) of PosK (term 0) / PosQ (term 1) [l, c(r), 64 h .. 64 h + 63] with delta = 128 (d - 3),
 // r = delta + t - 127 (c2p) or delta + 127 - t (p2c), c(r) = rel_index[AC_ENCODER_MAX_S - 1 + r]; row t = 255 is zero.
 // pos_key / pos_query [layers, 2 span, H] fp32.  64 threads per row, 4 rows per block.
@@ -1157,31 +1213,37 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
     return AC_OK;
 }
 
+// Every attention variant the library runs, with the dynamic shared memory the kernel is allowed and launched with (rows in
+// the enum's order).  All take the same arguments up to their score term.
+struct AttVariant { const void *kernel; int smem; };
+enum { ATT_PLAIN64, ATT_PLAIN32, ATT_RELBIAS, ATTS_PLAIN64, ATTS_PLAIN32, ATTS_RELBIAS, ATTS_DISENT, ATT_VARIANTS };
+static const AttVariant att_variants[ATT_VARIANTS] = {
+    {reinterpret_cast<const void *>(attention_kernel<64, ScorePlain>), ATT_SMEM<ScorePlain>},
+    {reinterpret_cast<const void *>(attention_kernel<32, ScorePlain>), ATT_SMEM<ScorePlain>},
+    {reinterpret_cast<const void *>(attention_kernel<64, ScoreRelBias>), ATT_SMEM<ScoreRelBias>},
+    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScorePlain>), ATTS_SMEM<ScorePlain>},
+    {reinterpret_cast<const void *>(attention_stream_kernel<32, ScorePlain>), ATTS_SMEM<ScorePlain>},
+    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScoreRelBias>), ATTS_SMEM<ScoreRelBias>},
+    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScoreDisent>), ATTS_SMEM<ScoreDisent>},
+};
+
 // softmax(Q K^T / sqrt(head_dim) [+ MPNet relative bias] + mask) V out of e->qk / e->vT into e->ctx; window = sliding
 // half-window, 0 = full attention.  S <= 128 runs attention_kernel, longer sequences attention_stream_kernel over 128-query
-// blocks; DeBERTa runs attention_stream_kernel<64, false, true> at every length, with layer `layer`'s c2p / p2c boxes.
+// blocks; DeBERTa runs attention_stream_kernel<64, ScoreDisent> at every length, with layer `layer`'s c2p / p2c boxes.
 // cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail), so only the first query block is computed.
 static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, int layer,
                             cudaStream_t s) {
     const ac_encoder_config &c = e->cfg;
-    const int H = c.hidden;
-    const int dh = H / c.heads;               // 64 or 32 (ac_encoder_create); 64 with a relative bias
-    const float *rb = e->rel_bias;
+    int H = c.hidden, heads = c.heads;
+    const int dh = H / heads;                 // 64 or 32 (ac_encoder_create); 64 with a relative bias or DeBERTa's boxes
     AC_REQUIRE(S <= AC_ENCODER_MAX_S || dh == 64, "attention: S=%d > %d needs head_dim 64 (ModernBERT)", S, AC_ENCODER_MAX_S);
     // per-device: the attribute is a property of the (function, device) pair
     static bool att_attr[64] = {};
     int dev = 0;
     AC_CUDA(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !att_attr[dev]) {
-        AC_CUDA(cudaFuncSetAttribute(attention_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_BIAS));
-        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTS_SMEM));
-        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     ATTS_SMEM_BIAS));
-        AC_CUDA(cudaFuncSetAttribute(attention_stream_kernel<64, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     ATTS_SMEM_DISENT));
+        for (const AttVariant &v : att_variants)
+            AC_CUDA(cudaFuncSetAttribute(v.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, v.smem));
         if (dev >= 0 && dev < 64) att_attr[dev] = true;
     }
     // algorithmic flops over the keys each computed query attends to at the true sequence length (the 128-wide tiles do
@@ -1195,19 +1257,26 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, in
         keys = static_cast<double>(nq) * S;
     }
     const int slot = prof_begin(PROF_ATTENTION, 4.0 * B * c.heads * keys * dh, 0.0, s);
+    const bool streamed = e->pos_g || S > 128;
+    ScorePlain plain;
+    ScoreRelBias bias;
+    ScoreDisent disent;
+    void *score = &plain;
+    int id = dh == 32 ? (streamed ? ATTS_PLAIN32 : ATT_PLAIN32) : (streamed ? ATTS_PLAIN64 : ATT_PLAIN64);
     if (e->pos_g) {
-        const int pos_row0 = layer * ATTS_POS_DELTAS * c.heads * 2 * 256;
-        attention_stream_kernel<64, false, true><<<dim3(B * c.heads, q_blocks), ATT_THREADS, ATTS_SMEM_DISENT, s>>>(
-            e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx, nullptr, e->m_pos, pos_row0);
-    } else if (S <= 128) {
-        auto kern = rb ? attention_kernel<64, true> : dh == 32 ? attention_kernel<32> : attention_kernel<64>;
-        kern<<<B * c.heads, ATT_THREADS, rb ? ATT_SMEM_BIAS : ATT_SMEM, s>>>(e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H,
-                                                                            window, e->ctx, rb);
-    } else {
-        auto kern = rb ? attention_stream_kernel<64, true> : dh == 32 ? attention_stream_kernel<32> : attention_stream_kernel<64>;
-        kern<<<dim3(B * c.heads, q_blocks), ATT_THREADS, rb ? ATTS_SMEM_BIAS : ATTS_SMEM, s>>>(
-            e->m_qk_att, e->m_vt_att, mask, B, S, c.heads, H, window, e->ctx, rb, e->m_qk_att, 0);
+        disent.tmap_pos = e->m_pos;
+        disent.pos_row0 = layer * ATTS_POS_DELTAS * heads * 2 * 256;
+        score = &disent;
+        id = ATTS_DISENT;
+    } else if (e->rel_bias) {
+        bias.rel_bias = e->rel_bias;
+        score = &bias;
+        id = streamed ? ATTS_RELBIAS : ATT_RELBIAS;
     }
+    const AttVariant &v = att_variants[id];
+    void *args[] = {&e->m_qk_att, &e->m_vt_att, &mask, &B, &S, &heads, &H, &window, &e->ctx, score};
+    // a launch error is the runtime's last error, which AC_LAUNCH_CHECK reads
+    cudaLaunchKernel(v.kernel, dim3(B * heads, streamed ? q_blocks : 1), dim3(ATT_THREADS), args, v.smem, s);
     prof_end(slot, s);
     AC_LAUNCH_CHECK();
     return AC_OK;

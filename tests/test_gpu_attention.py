@@ -1,6 +1,7 @@
 """The two encoder attention kernels (attention_kernel for S <= 128, attention_stream_kernel with the online softmax above;
-head_dim 64, 32 and 64 + MPNet relative bias each) run alone through Encoder.attention and are compared with a plain fp64
-reference of the same operation, on the fp16-rounded operands, at every row of every (sequence, head):
+ScorePlain at head_dim 64 and 32, ScoreRelBias, the MPNet relative bias, at 64) run alone through Encoder.attention and are
+compared with a plain fp64 reference of the same operation, on the fp16-rounded operands, at every row of every (sequence,
+head):
 
     out[b, q, h, :] = softmax_key( q.k / sqrt(dh) + bias[h, 511 + key - q] + M[b, q, key] ) . v
     M = 0 where mask[b, key] != 0 and (window == 0 or |q - key| <= window), -inf elsewhere
@@ -38,7 +39,8 @@ import torch
 MAX_S = 512           # AC_ENCODER_MAX_S: the bias table has 2 * MAX_S - 1 entries per head
 INF = float("inf")
 
-# kind -> (arch, head_dim): the three template instantiations of each kernel, and ModernBERT (head_dim 64 with a band)
+# kind -> (arch, head_dim): <64, ScorePlain>, <32, ScorePlain> and <64, ScoreRelBias> of each kernel, and ModernBERT
+# (head_dim 64 with a band)
 KINDS = {"dh64": ("bert", 64), "dh32": ("bert", 32), "bias": ("mpnet", 64), "modern": ("modernbert", 64)}
 HEADS = {"dh64": 4, "dh32": 8, "bias": 4, "modern": 2}     # >= 3 heads where S stays <= 512: inner heads have two neighbours
 BERT_KINDS = ["dh64", "dh32", "bias"]

@@ -51,7 +51,8 @@ def _check_cls(out, ref, abs_bound=2e-4):
 @pytest.mark.parametrize("B,S,pad", [(2, 128, False), (3, 16, True), (5, 77, True), (8, 128, False),
                                      (3, 129, False), (2, 300, True), (1, 512, False)])
 def test_minilm_l6_encoder_matches_oracle(cabi, B, S, pad):
-    """6 x 384, 12 heads of 32; S <= 128 runs attention_kernel<32>, 128 < S <= 512 attention_stream_kernel<32>"""
+    """6 x 384, 12 heads of 32; S <= 128 runs attention_kernel<32, ScorePlain>, 128 < S <= 512
+    attention_stream_kernel<32, ScorePlain>"""
     sd, cfg = _minilm(6)
     ids, mask = _ids_mask(B, S, pad)
     ref = eo.encoder_forward_cls(sd, ids, mask, num_heads=12)

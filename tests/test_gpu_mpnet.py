@@ -34,9 +34,9 @@ def _hf_sd(m):
 @pytest.mark.parametrize("B,S,pad", [(3, 16, False), (5, 77, True), (4, 128, False), (3, 129, False), (3, 200, True),
                                      (2, 384, False), (1, 512, False)])
 def test_mpnet_encoder_matches_oracle(cabi, B, S, pad, cls_only):
-    """2 x 768, 12 heads of 64, O(1) bias table and perturbed LayerNorms; S <= 128 runs attention_kernel<64, true>, longer
-    sequences attention_stream_kernel<64, true>.  cls_only off also compares the whole last hidden state (bounds of
-    test_gpu_parity.py::test_encoder_with_nontrivial_layernorms_matches_oracle and ::test_encoder_long_sequences)"""
+    """2 x 768, 12 heads of 64, O(1) bias table and perturbed LayerNorms; S <= 128 runs attention_kernel<64, ScoreRelBias>,
+    longer sequences attention_stream_kernel<64, ScoreRelBias>.  cls_only off also compares the whole last hidden state
+    (bounds of test_gpu_parity.py::test_encoder_with_nontrivial_layernorms_matches_oracle and ::test_encoder_long_sequences)"""
     m = mpnet_model(num_hidden_layers=2, **WIDE)
     ids, mask = mpnet_ids(B, S, pad, vocab=WIDE["vocab_size"])
     ref, ref_hidden = mo.mpnet_forward_cls(_hf_sd(m), ids, mask, num_heads=12, ln_eps=1e-5, return_hidden=True)
