@@ -30,6 +30,9 @@ AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERT
 AC_ENCODER_MAX_S = 512
 AC_MODERNBERT_MAX_S = 8192
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
+AC_FFN_GELU_ERF, AC_FFN_GELU_TANH = 0, 1
+# hidden_act of a post-LN (BERT-family) config -> ac_encoder_config.ffn_act
+FFN_ACTS = {"gelu": AC_FFN_GELU_ERF, "gelu_new": AC_FFN_GELU_TANH, "gelu_pytorch_tanh": AC_FFN_GELU_TANH}
 
 EXPORTS = [
     "ac_version", "ac_last_error", "ac_device_check",
@@ -77,7 +80,8 @@ class EncoderConfig(Structure):
                 ("ln_eps", c_float), ("precision", c_int), ("max_tokens", c_int), ("cls_only", c_int),
                 ("sliding_window", c_int), ("layer_sliding", POINTER(ctypes.c_int32)),
                 ("rope_full", c_void_p), ("rope_sliding", c_void_p), ("rel_bias", c_void_p),
-                ("pos_key", c_void_p), ("pos_query", c_void_p), ("pos_span", c_int), ("rel_index", c_void_p)]
+                ("pos_key", c_void_p), ("pos_query", c_void_p), ("pos_span", c_int), ("rel_index", c_void_p),
+                ("embedding_size", c_int), ("ffn_act", c_int)]
 
 
 _PP = POINTER(c_void_p)
@@ -90,7 +94,8 @@ class EncoderWeights(Structure):
                 ("ao_w", _PP), ("ao_b", _PP), ("ao_ln_w", _PP), ("ao_ln_b", _PP),
                 ("ff1_w", _PP), ("ff1_b", _PP), ("ff2_w", _PP), ("ff2_b", _PP),
                 ("out_ln_w", _PP), ("out_ln_b", _PP),
-                ("attn_norm_w", _PP), ("final_norm_w", c_void_p), ("wqkv", _PP), ("wi", _PP)]
+                ("attn_norm_w", _PP), ("final_norm_w", c_void_p), ("wqkv", _PP), ("wi", _PP),
+                ("emb_proj_w", c_void_p), ("emb_proj_b", c_void_p)]
 
 
 _lib = None
@@ -695,6 +700,91 @@ def deberta_to_bert_state_dict(sd: dict, c):
     return out, dims
 
 
+def _factorized_settings(c, family: str) -> None:
+    """Refusals shared by ALBERT and ELECTRA (post-LN BERT blocks behind factorized embeddings), raised before any device call
+    with the setting's name."""
+    H, E = c.hidden_size, getattr(c, "embedding_size", c.hidden_size)
+    if H % 128 != 0 or H > 1024:
+        raise AdaptiveB200Error(f"{family} hidden_size={H} is not implemented in the CUDA path: the encoder takes hidden "
+                                "<= 1024 in multiples of 128")
+    check_head_dim(H, c.num_attention_heads, family)
+    if E % 128 != 0 or E <= 0 or E > H:
+        raise AdaptiveB200Error(f"{family} embedding_size={E} (hidden_size={H}) is not implemented in the CUDA path: it must "
+                                "be a multiple of 128 and <= hidden_size")
+    if c.hidden_act not in FFN_ACTS:
+        raise AdaptiveB200Error(f"{family} hidden_act={c.hidden_act!r} is not implemented in the CUDA path (only "
+                                f"{', '.join(repr(a) for a in FFN_ACTS)})")
+    pet = getattr(c, "position_embedding_type", "absolute")
+    if pet != "absolute":
+        raise AdaptiveB200Error(f"{family} position_embedding_type={pet!r} is not implemented in the CUDA path (only "
+                                "'absolute')")
+
+
+def albert_settings(c) -> None:
+    """Raises AdaptiveB200Error naming any AlbertConfig setting the CUDA path does not implement (no device call):
+    albert-xlarge / xxlarge (hidden 2048 / 4096), head_dim other than 64 / 32, embedding_size not a multiple of 128 or
+    larger than hidden, hidden_act other than gelu / gelu_new / gelu_pytorch_tanh, non-absolute positions, and a layer walk
+    HF itself cannot run (num_hidden_groups outside 1 .. num_hidden_layers, inner_group_num < 1)."""
+    _factorized_settings(c, "ALBERT")
+    if not 1 <= c.num_hidden_groups <= c.num_hidden_layers or c.inner_group_num < 1:
+        raise AdaptiveB200Error(f"ALBERT num_hidden_groups={c.num_hidden_groups}, inner_group_num={c.inner_group_num} "
+                                f"(num_hidden_layers={c.num_hidden_layers}) is not a valid layer walk")
+
+
+def electra_settings(c) -> None:
+    """Raises AdaptiveB200Error naming any ElectraConfig setting the CUDA path does not implement (no device call)."""
+    _factorized_settings(c, "ELECTRA")
+
+
+def albert_layer_sources(c) -> list:
+    """(group, inner layer) of every effective layer of an ALBERT encoder, in order: HF AlbertTransformer runs group
+    int(i / (num_hidden_layers / num_hidden_groups)) for i < num_hidden_layers, each group its inner_group_num layers."""
+    return [(int(i / (c.num_hidden_layers / c.num_hidden_groups)), j)
+            for i in range(c.num_hidden_layers) for j in range(c.inner_group_num)]
+
+
+def albert_to_bert_state_dict(sd: dict, c):
+    """ALBERT (HF models/albert/modeling_albert.py) is the post-LN BERT block behind factorized embeddings (tables and
+    LayerNorm at width embedding_size, then encoder.embedding_hidden_mapping_in to hidden) with cross-layer parameter
+    sharing.  Returns the BERT names per effective layer -- layers that share parameters map to the SAME source tensor, which
+    Encoder packs once -- plus the projection as embeddings_project.*, and the Encoder dims.  pooler.* is not used."""
+    albert_settings(c)
+    out = {k: sd[k] for k in ("embeddings.word_embeddings.weight", "embeddings.position_embeddings.weight",
+                              "embeddings.token_type_embeddings.weight", "embeddings.LayerNorm.weight",
+                              "embeddings.LayerNorm.bias")}
+    for wb in ("weight", "bias"):
+        out[f"embeddings_project.{wb}"] = sd[f"encoder.embedding_hidden_mapping_in.{wb}"]
+    ren = {"attention.query": "attention.self.query", "attention.key": "attention.self.key",
+           "attention.value": "attention.self.value", "attention.dense": "attention.output.dense",
+           "attention.LayerNorm": "attention.output.LayerNorm", "ffn": "intermediate.dense", "ffn_output": "output.dense",
+           "full_layer_layer_norm": "output.LayerNorm"}
+    walk = albert_layer_sources(c)
+    for l, (g, j) in enumerate(walk):
+        for src, dst in ren.items():
+            for wb in ("weight", "bias"):
+                out[f"encoder.layer.{l}.{dst}.{wb}"] = sd[f"encoder.albert_layer_groups.{g}.albert_layers.{j}.{src}.{wb}"]
+    dims = dict(layers=len(walk), hidden=c.hidden_size, heads=c.num_attention_heads, intermediate=c.intermediate_size,
+                vocab=c.vocab_size, max_pos=c.max_position_embeddings, type_vocab=c.type_vocab_size, ln_eps=c.layer_norm_eps,
+                pad_idx=0, embedding_size=c.embedding_size, ffn_act=FFN_ACTS[c.hidden_act])
+    return out, dims
+
+
+def electra_to_bert_state_dict(sd: dict, c):
+    """ELECTRA (HF models/electra/modeling_electra.py) is BERT with embedding tables at width embedding_size and, when that
+    differs from hidden, embeddings_project to hidden after the embedding LayerNorm.  The layer names are BERT's already;
+    returns them plus embeddings_project.* when present, and the Encoder dims."""
+    electra_settings(c)
+    out = {k: v for k, v in sd.items() if k.startswith(("embeddings.", "embeddings_project.", "encoder.layer."))}
+    out.pop("embeddings.position_ids", None)
+    out.pop("embeddings.token_type_ids", None)
+    E = c.embedding_size
+    dims = dict(layers=c.num_hidden_layers, hidden=c.hidden_size, heads=c.num_attention_heads,
+                intermediate=c.intermediate_size, vocab=c.vocab_size, max_pos=c.max_position_embeddings,
+                type_vocab=c.type_vocab_size, ln_eps=c.layer_norm_eps, pad_idx=0,
+                embedding_size=E if E != c.hidden_size else 0, ffn_act=FFN_ACTS[c.hidden_act])
+    return out, dims
+
+
 def check_head_dim(hidden: int, heads: int, what: str = "encoder") -> None:
     """The attention kernels of the BERT-family encoder take head_dim = hidden / heads of 64 (bert-base, RoBERTa, DistilBERT)
     or 32 (all-MiniLM, BGE-small, E5-small, GTE-small); raises AdaptiveB200Error naming anything else (no device call)."""
@@ -755,14 +845,16 @@ class Encoder:
     """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors).  arch "mpnet"
     takes the BERT names (mpnet_to_bert_state_dict) and rel_bias, the [heads, 2 AC_ENCODER_MAX_S - 1] table of
     mpnet_relative_bias_table; arch "deberta" the BERT names and the pos_key / pos_query / pos_span / rel_index of
-    deberta_to_bert_state_dict."""
+    deberta_to_bert_state_dict.  embedding_size (0 = hidden) and the "embeddings_project.*" tensors give factorized
+    embeddings (albert_to_bert_state_dict, electra_to_bert_state_dict); ffn_act is AC_FFN_GELU_ERF or AC_FFN_GELU_TANH.
+    Names that refer to the same source tensor (ALBERT's shared layers) are copied and packed once."""
 
     def __init__(self, sd: dict, *, arch: str, layers: int, hidden: int, heads: int, intermediate: int, vocab: int,
                  max_pos: int = AC_ENCODER_MAX_S, type_vocab: int = 1, ln_eps: float, pad_idx: int = 0,
                  max_tokens: int = 65536, device="cuda", cls_only: bool = True, sliding_window: int = 0,
                  layer_sliding=None, rope_theta=None, rel_bias: Optional[torch.Tensor] = None,
                  pos_key: Optional[torch.Tensor] = None, pos_query: Optional[torch.Tensor] = None, pos_span: int = 0,
-                 rel_index: Optional[torch.Tensor] = None):
+                 rel_index: Optional[torch.Tensor] = None, embedding_size: int = 0, ffn_act: int = AC_FFN_GELU_ERF):
         L = load_library()
         self._L = L
         self.hidden = hidden
@@ -770,11 +862,16 @@ class Encoder:
         self.max_tokens = max_tokens
         dev = torch.device(device)
         keep = {}
+        copies = {}
 
         def g(name):
-            t = sd[name].detach().to(device=dev, dtype=torch.float32).contiguous()
-            keep[name] = t
-            return t.data_ptr()
+            # one device copy per source tensor: names that share a tensor (ALBERT's shared layers) pass the same pointer,
+            # which ac_encoder_create packs once
+            src = sd[name]
+            key = (src.data_ptr(), tuple(src.shape), tuple(src.stride()), src.dtype, src.device)
+            if key not in copies:
+                copies[key] = (src, src.detach().to(device=dev, dtype=torch.float32).contiguous())
+            return copies[key][1].data_ptr()
 
         def arr(fmt):
             a = (c_void_p * layers)(*[g(fmt.format(l)) for l in range(layers)])
@@ -813,9 +910,12 @@ class Encoder:
             w.ff1_w, w.ff1_b = arr(p + "intermediate.dense.weight"), arr(p + "intermediate.dense.bias")
             w.ff2_w, w.ff2_b = arr(p + "output.dense.weight"), arr(p + "output.dense.bias")
             w.out_ln_w, w.out_ln_b = arr(p + "output.LayerNorm.weight"), arr(p + "output.LayerNorm.bias")
+            if "embeddings_project.weight" in sd:      # factorized embeddings (ALBERT, ELECTRA)
+                w.emb_proj_w, w.emb_proj_b = g("embeddings_project.weight"), g("embeddings_project.bias")
             code = {"bert": AC_ARCH_BERT, "roberta": AC_ARCH_ROBERTA, "mpnet": AC_ARCH_MPNET, "deberta": AC_ARCH_DEBERTA}[arch]
             cfg = EncoderConfig(code, layers, hidden, heads, intermediate, vocab, max_pos, type_vocab, pad_idx, ln_eps,
                                 AC_PREC_F16, max_tokens, 1 if cls_only else 0)
+            cfg.embedding_size, cfg.ffn_act = embedding_size, ffn_act
             if rel_bias is not None:      # ac_encoder_create refuses an MPNet encoder without it
                 rb = rel_bias.detach().to(device=dev, dtype=torch.float32).contiguous()
                 keep["rel_bias"] = rb
@@ -830,12 +930,12 @@ class Encoder:
         with torch.cuda.device(dev):
             check(L.ac_encoder_create(ctypes.byref(cfg), ctypes.byref(w), ctypes.byref(h)), "ac_encoder_create")
         self.handle = h
-        del keep  # the handle holds its own packed copies
+        del keep, copies  # the handle holds its own packed copies
 
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
-        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel / DebertaV2Model (post-LN
-        blocks) or ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for BERT / RoBERTa /
+        """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel / DebertaV2Model / AlbertModel /
+        ElectraModel (post-LN blocks) or ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for BERT / RoBERTa /
         DistilBERT, 64 for MPNet, DeBERTa and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
         AC_MODERNBERT_MAX_S."""
         c = model.config
@@ -857,17 +957,25 @@ class Encoder:
             check_head_dim(c.dim, c.n_heads, "DistilBERT")
             sd, dims = distilbert_to_bert_state_dict(dict(model.state_dict()), c)
             return cls(sd, arch="bert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
+        if mt == "albert":
+            # state_dict() lists every shared parameter once; the renaming maps the shared layers onto those tensors
+            sd, dims = albert_to_bert_state_dict(dict(model.state_dict()), c)
+            return cls(sd, arch="bert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
+        if mt == "electra":
+            sd, dims = electra_to_bert_state_dict(dict(model.state_dict()), c)
+            return cls(sd, arch="bert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
         if mt not in ("bert", "roberta", "xlm-roberta"):
             raise AdaptiveB200Error(f"encoder architecture '{mt}' is not implemented in the CUDA path yet")
-        if getattr(c, "hidden_act", "gelu") != "gelu" or getattr(c, "position_embedding_type", "absolute") != "absolute":
-            raise AdaptiveB200Error("only exact-erf GELU and absolute position embeddings are implemented")
+        if getattr(c, "hidden_act", "gelu") not in FFN_ACTS or getattr(c, "position_embedding_type", "absolute") != "absolute":
+            raise AdaptiveB200Error(f"hidden_act={getattr(c, 'hidden_act', None)!r}: only GELU (exact erf 'gelu', tanh "
+                                    "'gelu_new' / 'gelu_pytorch_tanh') and absolute position embeddings are implemented")
         check_head_dim(c.hidden_size, c.num_attention_heads, mt)
         sd = {k: v for k, v in model.state_dict().items()}
         return cls(sd, arch="bert" if mt == "bert" else "roberta", layers=c.num_hidden_layers, hidden=c.hidden_size,
                    heads=c.num_attention_heads, intermediate=c.intermediate_size, vocab=c.vocab_size,
                    max_pos=c.max_position_embeddings, type_vocab=c.type_vocab_size, ln_eps=c.layer_norm_eps,
                    pad_idx=(c.pad_token_id if c.pad_token_id is not None else 0), max_tokens=max_tokens, device=device,
-                   cls_only=cls_only)
+                   cls_only=cls_only, ffn_act=FFN_ACTS[getattr(c, "hidden_act", "gelu")])
 
     def forward_cls(self, ids: torch.Tensor, mask: Optional[torch.Tensor] = None,
                     type_ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -12,7 +12,8 @@
 // tensor rate and half the operand bytes.
 //
 //   projections   wgmma GEMM of gemm_tc.cuh (.f16) with compile-time-specialised fused epilogues:
-//                 bias | bias+GELU(erf) | bias+residual, fp16 or fp32 output, V written TRANSPOSED per (sequence, head)
+//                 bias | bias+GELU(erf or tanh) | bias+residual, fp16 or fp32 output, V written TRANSPOSED per (sequence, head);
+//                 ALBERT / ELECTRA: LayerNorm at the embedding width E, then one E -> H projection (EpiEmbProj)
 //   attention     one CTA per (sequence, head): Q, K and V^T tiles by TMA, QK^T and PV as wgmma with the score tile
 //                 staged in shared memory, thread-per-query-row softmax in between (S <= 128; head_dim 64 or 32); longer
 //                 sequences (up to 512, ModernBERT up to 8192) run 128-query blocks over streamed key blocks in one pass with
@@ -24,6 +25,7 @@
 #include <cuda_fp16.h>
 #include <math_constants.h>
 #include <algorithm>
+#include <array>
 #include <type_traits>
 #include <vector>
 
@@ -54,6 +56,18 @@ __device__ __forceinline__ float gelu_erf(float y) {
     const float e = ex2_approx((y * y) * (-0.5f * 1.4426950408889634f));   // exp(-y^2/2)
     const float h = (p * t) * e;                                             // erfc(|y|/sqrt2) / 2
     return fmaxf(y, 0.f) - fabsf(y * h);
+}
+// tanh-approximated GELU (HF "gelu_new" = "gelu_pytorch_tanh", ALBERT v2):  0.5 y (1 + tanh(u)) = y / (1 + exp(-2 u)),
+// u = sqrt(2/pi) (y + 0.044715 y^3), with exp(-2 u) = 2^t, t = y (k1 + k3 y^2).  2 MUFU + 6 FP32 ops.  Relative error
+// < 2^-15: k1 and k3 are formed in double and rounded once (1/2 ulp each, so the sum k1 + k3 y^2 carries at most 1/2 ulp of
+// constant error); y^2, the fma and the product add 1/2 ulp each: |dt| <= 4 * 2^-24 |t|, an exp error <= 4 ln2 |t| 2^-24 <=
+// 2.1e-5 for |t| <= 126, where 2^t stays finite (outputs that are normal fp16 need |t| <= ~30: <= 5e-6).  ex2.approx <= 2 ulp,
+// rcp.approx <= 1 ulp, the add and the product 1/2 ulp each (< 5e-7 together).  Below t = -126 / above 126 the result is y / -0.
+__device__ __forceinline__ float gelu_tanh(float y) {
+    constexpr float k1 = static_cast<float>(-2.0 * 0.79788456080286535588 * 1.4426950408889634074);   // -2 sqrt(2/pi) log2(e)
+    constexpr float k3 = static_cast<float>(-2.0 * 0.79788456080286535588 * 1.4426950408889634074 * 0.044715);
+    const float t = y * fmaf(k3, y * y, k1);
+    return y * rcp_approx(1.f + ex2_approx(t));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -142,6 +156,7 @@ struct EpiF32 : EpiBase {
 
 // fp16 output, the next GEMM's A operand: pre-activation acc + bias, or with DEFER the deferred-LayerNorm form below, then
 //   Act::Gelu   exact-erf GELU
+//   Act::GeluTanh  tanh-approximated GELU (post-LN encoders with hidden_act "gelu_new" / "gelu_pytorch_tanh")
 //   Act::GeGLU  (ModernBERT's mlp.Wi) pack_defer_kernel interleaved the weight rows in 32-row groups, so a warp's slice
 //               holds [input cols 32 g .. + 31 | gate cols 32 g .. + 31]; the gate chunk re-reads the input chunk from the
 //               accumulator tile and writes fp16(GELU_erf(input) * gate) to columns 32 g.. of Y (N = 2 I, ldy = I)
@@ -150,7 +165,14 @@ struct EpiF32 : EpiBase {
 // DEFER: the A operand was the UN-normalised residual sum y (fp16) and the weights were packed as fp16(gamma * W):
 //   LayerNorm(y) W^T + b = r (acc - mu c1) + c0  with the row statistics (mu, r) of y, c1 = rowsum(W'), and `bias`
 //   holding c0 = W beta + b  (producer side: EpiResidDefer)
-enum class Act { None, Gelu, GeGLU, Rope };
+enum class Act { None, Gelu, GeGLU, Rope, GeluTanh };
+// the activation an EpiF16 applies to every pre-activation (GeGLU and RoPE combine a chunk with its partner instead)
+template <Act ACT>
+__device__ __forceinline__ float act_elem(float y) {
+    if constexpr (ACT == Act::Gelu) return gelu_erf(y);
+    else if constexpr (ACT == Act::GeluTanh) return gelu_tanh(y);
+    else return y;
+}
 template <Act ACT, bool DEFER>
 struct EpiF16 : EpiBase {
     const float *__restrict__ bias;       // [N]   (DEFER: c0)
@@ -188,12 +210,11 @@ struct EpiF16 : EpiBase {
             const float4 bb = __ldg(reinterpret_cast<const float4 *>(bias + col0 + 8 * j + 4));
             const float4 ca = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + col0 + 8 * j)) : make_float4(0, 0, 0, 0);
             const float4 cb = DEFER ? __ldg(reinterpret_cast<const float4 *>(c1 + col0 + 8 * j + 4)) : make_float4(0, 0, 0, 0);
-            constexpr bool G = ACT == Act::Gelu;
             float y[8];
-            y[0] = gelu_if(G, pre(st, v[8 * j], ba.x, ca.x)); y[1] = gelu_if(G, pre(st, v[8 * j + 1], ba.y, ca.y));
-            y[2] = gelu_if(G, pre(st, v[8 * j + 2], ba.z, ca.z)); y[3] = gelu_if(G, pre(st, v[8 * j + 3], ba.w, ca.w));
-            y[4] = gelu_if(G, pre(st, v[8 * j + 4], bb.x, cb.x)); y[5] = gelu_if(G, pre(st, v[8 * j + 5], bb.y, cb.y));
-            y[6] = gelu_if(G, pre(st, v[8 * j + 6], bb.z, cb.z)); y[7] = gelu_if(G, pre(st, v[8 * j + 7], bb.w, cb.w));
+            y[0] = act_elem<ACT>(pre(st, v[8 * j], ba.x, ca.x)); y[1] = act_elem<ACT>(pre(st, v[8 * j + 1], ba.y, ca.y));
+            y[2] = act_elem<ACT>(pre(st, v[8 * j + 2], ba.z, ca.z)); y[3] = act_elem<ACT>(pre(st, v[8 * j + 3], ba.w, ca.w));
+            y[4] = act_elem<ACT>(pre(st, v[8 * j + 4], bb.x, cb.x)); y[5] = act_elem<ACT>(pre(st, v[8 * j + 5], bb.y, cb.y));
+            y[6] = act_elem<ACT>(pre(st, v[8 * j + 6], bb.z, cb.z)); y[7] = act_elem<ACT>(pre(st, v[8 * j + 7], bb.w, cb.w));
             if (GLU || ROT) {
                 const int pc = col0 + pofs + 8 * j;
                 const float4 a0 = *reinterpret_cast<const float4 *>(acc + pofs + 8 * j);
@@ -381,6 +402,48 @@ struct EpiResidDefer : EpiBase {
     }
 };
 
+// embedding projection E -> H (ALBERT encoder.embedding_hidden_mapping_in, ELECTRA embeddings_project): the A operand is
+// the LayerNorm-ed embedding rows at width E (fp16), the output the residual stream layer 0 starts from, y = acc + bias in
+// fp32 plus its fp16 copy yh (layer 0's QKV operand).  Nothing is pending on y: layer 0 runs with the identity LayerNorm,
+// as it does on the embeddings of an encoder without projection.
+struct EpiEmbProj : EpiBase {
+    const float *__restrict__ bias;   // [N]
+    float *y;                         // [M, ld]
+    __half *yh;                       // [M, ld]
+    int M, N, ld;
+    static constexpr int kPrefetchDist = 0;
+    struct State {};
+    __device__ __forceinline__ void prefetch(State &, const GemmTileInfo &, int, int, int, int) const {}
+    __device__ __forceinline__ void tile(State &, const GemmTileInfo &, int row, int col0, const float (&v)[32], uint8_t *stage,
+                                         int lane, int, const float *) const {
+        const int row_base = row - lane;
+        if (row_base >= M || col0 >= N) return;                              // warp-uniform
+        const int r8 = lane >> 2, c = lane & 3;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const int col = col0 + 16 * half + 4 * c;
+            stage_f32_half(v, half, stage, lane);
+            const bool col_ok = col + 4 <= N;
+            const float4 b4 = col_ok ? __ldg(reinterpret_cast<const float4 *>(bias + col)) : make_float4(0, 0, 0, 0);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int grow = row_base + r8 + 8 * i;
+                if (grow < M && col_ok) {
+                    const float4 a = *reinterpret_cast<const float4 *>(stage + (r8 + 8 * i) * GEMM_EPI_STAGE_ROW_BYTES + 16 * c);
+                    const float4 o = make_float4(a.x + b4.x, a.y + b4.y, a.z + b4.z, a.w + b4.w);
+                    *reinterpret_cast<float4 *>(y + static_cast<int64_t>(grow) * ld + col) = o;
+                    const __half2 h0 = __floats2half2_rn(o.x, o.y), h1 = __floats2half2_rn(o.z, o.w);
+                    uint2 pk;
+                    pk.x = *reinterpret_cast<const uint32_t *>(&h0);
+                    pk.y = *reinterpret_cast<const uint32_t *>(&h1);
+                    *reinterpret_cast<uint2 *>(yh + static_cast<int64_t>(grow) * ld + col) = pk;
+                }
+            }
+            __syncwarp();
+        }
+    }
+};
+
 // (sum, sumsq) partials of every GEMM_EPI_COLS-column part -> (mu, 1/sqrt(var + eps)) per row; parts are added in a fixed order.
 // Kept as a kernel of its own: folding these loads + rsqrt into the consuming epilogues puts them at the head of every tile's
 // epilogue, which is the critical path of the HBM-bound residual GEMMs.
@@ -498,6 +561,9 @@ __global__ void layernorm_kernel(const float *__restrict__ in, const float *__re
 // modeling_bert.py:53-113 / modeling_roberta.py:146-159: (word + type) + position -> LayerNorm
 // modeling_mpnet.py MPNetEmbeddings: RoBERTa's positions (padding_idx 1); the type table is one zero row
 // modeling_modernbert.py ModernBertEmbeddings: pos = type = NULL, LayerNorm(word) (b = zeros: norm_bias=False)
+// modeling_albert.py AlbertEmbeddings, modeling_electra.py ElectraEmbeddings: BERT's rule at width H = embedding_size;
+// F32_OUT = false writes the fp16 rows only (the A operand of the embedding projection, EpiEmbProj)
+template <bool F32_OUT>
 __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *__restrict__ type_ids,
                                 const float *__restrict__ word, const float *__restrict__ pos,
                                 const float *__restrict__ type, const float *__restrict__ w,
@@ -540,7 +606,8 @@ __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *
             x[i].z = (a.z + t.z) + q.z;
             x[i].w = (a.w + t.w) + q.w;
         }
-    ln_row(x, nv, H, w, b, eps, lane, out_full + static_cast<int64_t>(row) * H, out_half + static_cast<int64_t>(row) * H);
+    ln_row(x, nv, H, w, b, eps, lane, F32_OUT ? out_full + static_cast<int64_t>(row) * H : nullptr,
+           out_half + static_cast<int64_t>(row) * H);
 }
 
 // classifier.py:1272,1275: CLS row -> x / max(||x||_2, 1e-12)
@@ -1175,6 +1242,11 @@ struct ac_encoder {
     ac_encoder_config cfg;
     // packed weights (device): fp16 GEMM operands, fp32 everything else.  ModernBERT: no pos / type, emb_ln_b = zeros
     float *word = nullptr, *pos = nullptr, *type = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
+    // embedding projection [H, E] (fp16) and its bias, NULL without one; m_emb views e->ctx as the [T, E] LayerNorm-ed
+    // embedding rows it consumes (ctx is free until layer 0's attention)
+    __half *emb_proj_w = nullptr;
+    float *emb_proj_b = nullptr;
+    CUtensorMap m_emb, m_emb_proj;
     std::vector<Layer> layers;
     __half *w1_last = nullptr;            // plain fp16 FFN1 weight of the last layer (CLS-only tail runs on materialised LayerNorm rows)
     float *b1_last = nullptr;             // its bias (ModernBERT: zeros)
@@ -1355,10 +1427,24 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
                "ac_encoder_create: DeBERTa needs pos_key, pos_query, rel_index, pos_span > 0 (pos_span=%d) and head_dim 64 "
                "(hidden=%d heads=%d)", cfg->pos_span, cfg->hidden, cfg->heads);
     AC_REQUIRE(cfg->intermediate % 64 == 0 && cfg->layers > 0 && cfg->max_tokens > 0, "ac_encoder_create: bad dims");
+    AC_REQUIRE(cfg->ffn_act == AC_FFN_GELU_ERF || cfg->ffn_act == AC_FFN_GELU_TANH, "ac_encoder_create: unknown ffn_act=%d",
+               cfg->ffn_act);
+    const int E = cfg->embedding_size ? cfg->embedding_size : cfg->hidden;
+    AC_REQUIRE(!mb || cfg->ffn_act == AC_FFN_GELU_ERF, "ac_encoder_create: ModernBERT takes no ffn_act=%d (its FFN is GeGLU)",
+               cfg->ffn_act);
+    // the projection runs after the embedding LayerNorm (ALBERT, ELECTRA); DeBERTa-v2's embed_proj runs before it
+    AC_REQUIRE(!w->emb_proj_w || cfg->arch == AC_ARCH_BERT || cfg->arch == AC_ARCH_ROBERTA,
+               "ac_encoder_create: an embedding projection (emb_proj_w) is implemented for AC_ARCH_BERT / AC_ARCH_ROBERTA "
+               "only (arch=%d)", cfg->arch);
+    AC_REQUIRE(w->emb_proj_w ? (w->emb_proj_b && E > 0 && E % 128 == 0 && E <= cfg->hidden) : E == cfg->hidden,
+               "ac_encoder_create: embedding_size=%d (hidden=%d) with%s emb_proj_w: a projection needs emb_proj_b and a "
+               "width that is a multiple of 128 and <= hidden; without one embedding_size must be 0 or hidden",
+               cfg->embedding_size, cfg->hidden, w->emb_proj_w ? "" : "out");
     int rc = ac_device_check();
     if (rc) return rc;
     ac_encoder *e = new ac_encoder();
     e->cfg = *cfg;
+    e->cfg.embedding_size = E;        // 0 resolved to hidden: forward_layers reads the width from here
     const int H = cfg->hidden, I = cfg->intermediate, L = cfg->layers;
     const size_t T = static_cast<size_t>((cfg->max_tokens + 127) / 128 * 128);
     e->T = T;
@@ -1401,11 +1487,15 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
             TRY(pack_consumer(e, 1, &w->wi[L - 1], nullptr, nullptr, nullptr, 2 * I, H, 1, &e->w1_last, &c1, &c0));
         }
     } else {
-        TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
-        TRY(pack_f32(e, &e->pos, w->pos_emb, static_cast<size_t>(cfg->max_pos) * H));
-        TRY(pack_f32(e, &e->type, w->type_emb, static_cast<size_t>(cfg->type_vocab) * H));
-        TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
-        TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, H));
+        TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * E));
+        TRY(pack_f32(e, &e->pos, w->pos_emb, static_cast<size_t>(cfg->max_pos) * E));
+        TRY(pack_f32(e, &e->type, w->type_emb, static_cast<size_t>(cfg->type_vocab) * E));
+        TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, E));
+        TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, E));
+        if (w->emb_proj_w) {
+            TRY(pack_f16(e, &e->emb_proj_w, w->emb_proj_w, static_cast<size_t>(H) * E));
+            TRY(pack_f32(e, &e->emb_proj_b, w->emb_proj_b, H));
+        }
         if (mp) TRY(pack_f32(e, &e->rel_bias, cfg->rel_bias, static_cast<size_t>(cfg->heads) * (2 * AC_ENCODER_MAX_S - 1)));
         if (db) {
             const size_t rows = static_cast<size_t>(L) * ATTS_POS_DELTAS * cfg->heads * 2 * 256;
@@ -1415,24 +1505,59 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
             TRY(check_cuda(cudaGetLastError(), "pos_gather_kernel"));
             TRY(make_tmap_2d(&e->m_pos, e->pos_g, 2, rows, 64, 128, 128, 64));
         }
+        // Shared packing: a packed operand whose sources (weights, biases and the LayerNorm folded into it) are the very
+        // pointers of an earlier layer's is that layer's buffers.  ALBERT's cross-layer sharing thus packs one set of weights
+        // plus a second QKV (layer 0's consumes the embeddings, the others the sums pending full_layer_layer_norm).
+        using Src = std::array<const float *, 8>;
+        const auto qkv_src = [&](int l) {
+            return Src{w->q_w[l], w->k_w[l], w->v_w[l], w->q_b[l], w->k_b[l], w->v_b[l], l ? w->out_ln_w[l - 1] : nullptr,
+                       l ? w->out_ln_b[l - 1] : nullptr};
+        };
+        const auto ffn1_src = [&](int l) { return Src{w->ff1_w[l], w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l]}; };
+        const auto earlier = [&](int l, const auto &src) {    // first layer j < l with the same sources, or -1
+            for (int j = 0; j < l; ++j)
+                if (src(j) == src(l)) return j;
+            return -1;
+        };
+        // a single-source operand: fp32 copy (bias, LayerNorm) or fp16 copy (plain weight) of src[l], or layer j's
+        const auto copy_of = [&](auto Layer::*field, const float *const *src, int l, size_t n) -> int {
+            const int j = earlier(l, [&](int i) { return Src{src[i]}; });
+            if (j >= 0) {
+                e->layers[l].*field = e->layers[j].*field;
+                return AC_OK;
+            }
+            if constexpr (std::is_same_v<decltype(e->layers[l].*field), __half *&>)
+                return pack_f16(e, &(e->layers[l].*field), src[l], n);
+            else
+                return pack_f32(e, &(e->layers[l].*field), src[l], n);
+        };
         for (int l = 0; l < L; ++l) {
             Layer &ly = e->layers[l];
             // the fused QKV [3H, H] of layer l consumes the sums pending the output LayerNorm of layer l-1 (identity for
-            // layer 0: the embeddings arrive normalised), FFN1 the sums pending the attention-output LayerNorm of layer l
-            const float *ws[3] = {w->q_w[l], w->k_w[l], w->v_w[l]};
-            const float *bs[3] = {w->q_b[l], w->k_b[l], w->v_b[l]};
-            TRY(pack_consumer(e, 3, ws, bs, l ? w->out_ln_w[l - 1] : nullptr, l ? w->out_ln_b[l - 1] : nullptr, H, H, 0,
-                              &ly.wqkv, &ly.c1qkv, &ly.c0qkv));
-            TRY(pack_f16(e, &ly.wo, w->ao_w[l], HH));
-            TRY(pack_f32(e, &ly.bo, w->ao_b[l], H));
-            TRY(pack_f32(e, &ly.ln_ffn_w, w->ao_ln_w[l], H));
-            TRY(pack_f32(e, &ly.ln_ffn_b, w->ao_ln_b[l], H));
-            TRY(pack_consumer(e, 1, &w->ff1_w[l], &w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], I, H, 0, &ly.w1, &ly.c1f,
-                              &ly.c0f));
-            TRY(pack_f16(e, &ly.w2, w->ff2_w[l], HI));
-            TRY(pack_f32(e, &ly.b2, w->ff2_b[l], H));
-            TRY(pack_f32(e, &ly.ln_out_w, w->out_ln_w[l], H));
-            TRY(pack_f32(e, &ly.ln_out_b, w->out_ln_b[l], H));
+            // layer 0: the embeddings arrive normalised, or un-normalised from the projection), FFN1 the sums pending the
+            // attention-output LayerNorm of layer l
+            if (const int j = earlier(l, qkv_src); j >= 0) {
+                ly.wqkv = e->layers[j].wqkv, ly.c1qkv = e->layers[j].c1qkv, ly.c0qkv = e->layers[j].c0qkv;
+            } else {
+                const float *ws[3] = {w->q_w[l], w->k_w[l], w->v_w[l]};
+                const float *bs[3] = {w->q_b[l], w->k_b[l], w->v_b[l]};
+                TRY(pack_consumer(e, 3, ws, bs, l ? w->out_ln_w[l - 1] : nullptr, l ? w->out_ln_b[l - 1] : nullptr, H, H, 0,
+                                  &ly.wqkv, &ly.c1qkv, &ly.c0qkv));
+            }
+            TRY(copy_of(&Layer::wo, w->ao_w, l, HH));
+            TRY(copy_of(&Layer::bo, w->ao_b, l, H));
+            TRY(copy_of(&Layer::ln_ffn_w, w->ao_ln_w, l, H));
+            TRY(copy_of(&Layer::ln_ffn_b, w->ao_ln_b, l, H));
+            if (const int j = earlier(l, ffn1_src); j >= 0) {
+                ly.w1 = e->layers[j].w1, ly.c1f = e->layers[j].c1f, ly.c0f = e->layers[j].c0f;
+            } else {
+                TRY(pack_consumer(e, 1, &w->ff1_w[l], &w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], I, H, 0, &ly.w1, &ly.c1f,
+                                  &ly.c0f));
+            }
+            TRY(copy_of(&Layer::w2, w->ff2_w, l, HI));
+            TRY(copy_of(&Layer::b2, w->ff2_b, l, H));
+            TRY(copy_of(&Layer::ln_out_w, w->out_ln_w, l, H));
+            TRY(copy_of(&Layer::ln_out_b, w->out_ln_b, l, H));
         }
         if (cfg->cls_only) {
             TRY(pack_f16(e, &e->w1_last, w->ff1_w[L - 1], HI));
@@ -1477,6 +1602,10 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     TRY(make_tmap_2d(&e->m_xh_cls, e->xh_cls, 2, e->Bc, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_M, 64));
     TRY(make_tmap_2d(&e->m_ctx_cls, e->ctx_cls, 2, e->Bc, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_M, 64));
     TRY(make_tmap_2d(&e->m_ffn_cls, e->ffn_cls, 2, e->Bc, I, static_cast<uint64_t>(I) * 2, GEMM_BLOCK_M, 64));
+    if (e->emb_proj_w) {
+        TRY(make_tmap_2d(&e->m_emb, e->ctx, 2, T, E, static_cast<uint64_t>(E) * 2, GEMM_BLOCK_M, 64));
+        TRY(make_tmap_2d(&e->m_emb_proj, e->emb_proj_w, 2, H, E, static_cast<uint64_t>(E) * 2, GEMM_BLOCK_N, 64));
+    }
     const int n1 = mb ? 2 * I : I;    // rows of the first FFN weight (ModernBERT: GeGLU input + gate)
     for (Layer &ly : e->layers) {
         TRY(make_tmap_2d(&ly.m_wqkv, ly.wqkv, 2, 3 * H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
@@ -1505,12 +1634,13 @@ static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, in
 // deferred; the residual epilogues add LN_pending(y), carried as (row statistics, gamma, beta).  That pending LayerNorm is
 // the one decision the block kinds differ in: post-LN blocks leave LN1 / LN2 pending, pre-LN blocks keep the identity
 // (stats (0, 1), gamma 1, beta 0) pending throughout.  The rest is the epilogue type (RoPE, GeGLU) and data in e->layers.
-template <bool PRE_LN>
+// FFN_ACT: GeGLU (pre-LN), or the post-LN encoder's GELU (ac_encoder_config.ffn_act: exact erf or tanh).
+template <bool PRE_LN, Act FFN_ACT>
 static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids, int B, int S,
                           float *out_unit_cls, cudaStream_t s) {
-    constexpr Act kFfnAct = PRE_LN ? Act::GeGLU : Act::Gelu;        // GeGLU input * gate, or GELU
-    using EpiFfn1 = EpiF16<kFfnAct, true>;
-    using EpiFfn1Rows = EpiF16<kFfnAct, false>;                     // on materialised LayerNorm rows (CLS-only tail)
+    static_assert(PRE_LN == (FFN_ACT == Act::GeGLU), "GeGLU is the pre-LN block's FFN");
+    using EpiFfn1 = EpiF16<FFN_ACT, true>;
+    using EpiFfn1Rows = EpiF16<FFN_ACT, false>;                     // on materialised LayerNorm rows (CLS-only tail)
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden, I = c.intermediate, M = B * S;
     const int N1 = PRE_LN ? 2 * I : I;                              // FFN1 accumulator columns (GeGLU: input + gate)
@@ -1521,11 +1651,22 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
     const int64_t pstride = static_cast<int64_t>(e->T);
     const bool cls_tail = c.cls_only && static_cast<size_t>(B) <= e->Bc;
     int rc;
-    embed_ln_kernel<<<row_blocks, wpb * 32, 0, s>>>(ids, PRE_LN ? nullptr : type_ids, e->word, e->pos, e->type, e->emb_ln_w,
-                                                    e->emb_ln_b, c.ln_eps, B, S, H, c.arch, c.pad_idx, c.vocab, c.max_pos,
-                                                    c.type_vocab, e->x, e->xh);
-    AC_LAUNCH_CHECK();
-    // the embeddings arrive normalised: identity LayerNorm pending, and identity statistics for layer 0's QKV
+    if (!e->emb_proj_w) {
+        embed_ln_kernel<true><<<row_blocks, wpb * 32, 0, s>>>(ids, PRE_LN ? nullptr : type_ids, e->word, e->pos, e->type,
+                                                              e->emb_ln_w, e->emb_ln_b, c.ln_eps, B, S, H, c.arch, c.pad_idx,
+                                                              c.vocab, c.max_pos, c.type_vocab, e->x, e->xh);
+        AC_LAUNCH_CHECK();
+    } else {
+        // factorized embeddings: LayerNorm at width E into the ctx scratch (fp16), then y = LN(emb) Wp^T + bp at width H
+        const int E = c.embedding_size;
+        embed_ln_kernel<false><<<row_blocks, wpb * 32, 0, s>>>(ids, type_ids, e->word, e->pos, e->type, e->emb_ln_w,
+                                                               e->emb_ln_b, c.ln_eps, B, S, E, c.arch, c.pad_idx, c.vocab,
+                                                               c.max_pos, c.type_vocab, nullptr, e->ctx);
+        AC_LAUNCH_CHECK();
+        EpiEmbProj ep{.bias = e->emb_proj_b, .y = e->x, .yh = e->xh, .M = M, .N = H, .ld = H};
+        if ((rc = launch_linear(e->m_emb, e->m_emb_proj, M, H, E, ep, s))) return rc;
+    }
+    // the embeddings arrive normalised (or projected): identity LayerNorm pending, and identity statistics for layer 0's QKV
     const float2 *pst = e->stats_id, *st_qkv = e->stats_id;
     const float *pg = e->ones, *pb = e->zeros;
     for (int l = 0; l < c.layers; ++l) {
@@ -1624,8 +1765,10 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
     int rc = check_shape_map_vt(e, "ac_encoder_forward_cls", B, S);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return e->cfg.arch == AC_ARCH_MODERNBERT ? forward_layers<true>(e, ids, mask, type_ids, B, S, out_unit_cls, s)
-                                             : forward_layers<false>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    if (e->cfg.arch == AC_ARCH_MODERNBERT) return forward_layers<true, Act::GeGLU>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    if (e->cfg.ffn_act == AC_FFN_GELU_TANH)
+        return forward_layers<false, Act::GeluTanh>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    return forward_layers<false, Act::Gelu>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
 }
 
 // parity entry: the attention stage alone, through the handle's own buffers, V^T view and launch_attention
@@ -1669,6 +1812,7 @@ static int linear_tc(const CUtensorMap &ta, const CUtensorMap &tb, const float *
         if (out_half) {
             __half *Yh = static_cast<__half *>(Y);
             if (epi == 0) return run(EpiF16<Act::None, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
+            if (epi == 3) return run(EpiF16<Act::GeluTanh, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
             return run(EpiF16<Act::Gelu, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
         }
     }
@@ -1682,9 +1826,10 @@ static int linear_tc(const CUtensorMap &ta, const CUtensorMap &tb, const float *
 extern "C" int ac_linear_tc(const void *X, const void *W, const float *bias, const float *residual, void *Y, int M, int N,
                             int K, int epi, int round_out, int precision, int out_half, ac_stream_t stream) {
     AC_REQUIRE(X && W && Y && bias && M > 0 && N > 0 && K > 0, "ac_linear_tc: bad arguments (bias is required)");
-    AC_REQUIRE(epi >= 0 && epi <= 2 && (epi != 2 || residual), "ac_linear_tc: bad epilogue");
+    AC_REQUIRE(epi >= 0 && epi <= 3 && (epi != 2 || residual), "ac_linear_tc: bad epilogue");
     AC_REQUIRE(precision == AC_PREC_TF32 || precision == AC_PREC_F16, "ac_linear_tc: bad precision");
     AC_REQUIRE(!(out_half && epi == 2), "ac_linear_tc: the residual epilogue writes fp32");
+    AC_REQUIRE(epi != 3 || (out_half && precision == AC_PREC_F16), "ac_linear_tc: the tanh-GELU epilogue writes fp16");
     const int es = precision == AC_PREC_F16 ? 2 : 4;
     AC_REQUIRE((K * es) % 16 == 0 && N % 8 == 0, "ac_linear_tc: rows must be 16-byte multiples and N %% 8 == 0");
     int rc = ac_device_check();

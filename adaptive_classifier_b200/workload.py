@@ -57,6 +57,37 @@ def deberta_base(seed: int = 1234):
     return m, cfg
 
 
+def albert_base(seed: int = 1234, large: bool = False):
+    """HF AlbertModel of the albert-base-v2 shape (12 x 768, 12 heads, I = 3072, embedding_size 128, vocab 30000, one shared
+    layer, "gelu_new"), or with large the albert-large-v2 shape (24 x 1024, 16 heads, I = 4096), random init under
+    torch.manual_seed(seed)."""
+    from transformers import AlbertConfig, AlbertModel
+    torch.manual_seed(seed)
+    dims = dict(hidden_size=1024, num_hidden_layers=24, num_attention_heads=16, intermediate_size=4096) if large else \
+        dict(hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072)
+    cfg = AlbertConfig(vocab_size=30000, embedding_size=128, num_hidden_groups=1, inner_group_num=1, hidden_act="gelu_new",
+                       max_position_embeddings=512, type_vocab_size=2, layer_norm_eps=1e-12, **dims)
+    m = AlbertModel(cfg, add_pooling_layer=False)
+    m.eval()
+    return m, cfg
+
+
+def albert_large(seed: int = 1234):
+    return albert_base(seed, large=True)
+
+
+def electra_small(seed: int = 1234):
+    """HF ElectraModel of the google/electra-small-discriminator shape (12 x 256, 4 heads, I = 1024, embedding_size 128,
+    vocab 30522, "gelu"), random init under torch.manual_seed(seed)."""
+    from transformers import ElectraConfig, ElectraModel
+    torch.manual_seed(seed)
+    cfg = ElectraConfig(vocab_size=30522, embedding_size=128, hidden_size=256, num_hidden_layers=12, num_attention_heads=4,
+                        intermediate_size=1024, max_position_embeddings=512, type_vocab_size=2, hidden_act="gelu")
+    m = ElectraModel(cfg)
+    m.eval()
+    return m, cfg
+
+
 def modernbert_ids(B: int, S: int, seed: int = 7) -> torch.Tensor:
     """uniform in [1000, 50000), [CLS]=50281 first, [SEP]=50282 last, never the pad id 50283; int32 [B,S] on the host."""
     g = torch.Generator().manual_seed(seed)

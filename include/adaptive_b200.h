@@ -290,15 +290,28 @@ typedef struct {
     int pos_span;                /* position_buckets, or max_relative_positions without buckets */
     const int32_t *rel_index;    /* [2 AC_ENCODER_MAX_S - 1] int32: entry AC_ENCODER_MAX_S - 1 + r is
                                     c(r) = clamp(bucket(r) + pos_span, 0, 2 pos_span - 1) (HF build_relative_position) */
+    /* factorized embeddings (ALBERT, ELECTRA): width E of the embedding tables and their LayerNorm; 0 means hidden.  An E
+       other than hidden needs the projection ac_encoder_weights.emb_proj_w; with a projection E % 128 == 0, E <= hidden. */
+    int embedding_size;
+    int ffn_act;                 /* AC_FFN_*: the FFN activation of a post-LN encoder; AC_ARCH_MODERNBERT (GeGLU) takes 0 */
 } ac_encoder_config;
+
+enum {
+    AC_FFN_GELU_ERF = 0,         /* exact-erf GELU (HF "gelu") */
+    AC_FFN_GELU_TANH = 1         /* tanh-approximated GELU (HF "gelu_new", "gelu_pytorch_tanh"; ALBERT v2) */
+};
 
 /* device pointers to the HF state_dict tensors (fp32, HF layout [out,in]).
  * AC_ARCH_MODERNBERT (models/modernbert/modeling_modernbert.py, every bias absent) uses only
  *   word_emb   embeddings.tok_embeddings      emb_ln_w  embeddings.norm
  *   ao_w       layers.l.attn.Wo               ao_ln_w   layers.l.mlp_norm
  *   ff2_w      layers.l.mlp.Wo
- * and the fields after out_ln_b; every other pointer may be NULL. */
+ * and the fields after out_ln_b; every other pointer may be NULL.
+ * Shared layers (ALBERT's cross-layer parameter sharing): a packed operand whose source pointers -- weights, biases and the
+ * LayerNorm folded into it -- equal an earlier layer's reuses that layer's packed copy, so pass the same pointer for every
+ * layer that shares a tensor.  Sharing is by pointer identity only: equal values at different addresses are packed twice. */
 typedef struct {
+    /* width embedding_size when it is set (ALBERT, ELECTRA), else hidden */
     const float *word_emb, *pos_emb, *type_emb, *emb_ln_w, *emb_ln_b;
     /* arrays of `layers` device pointers each (host arrays of device pointers) */
     const float *const *q_w, *const *q_b, *const *k_w, *const *k_b, *const *v_w, *const *v_b;
@@ -310,6 +323,12 @@ typedef struct {
     const float *final_norm_w;        /* final_norm */
     const float *const *wqkv;         /* [layers] layers.l.attn.Wqkv [3H, H], q, k, v thirds */
     const float *const *wi;           /* [layers] layers.l.mlp.Wi [2I, H], input rows then gate rows */
+    /* embedding projection E -> H after the embedding LayerNorm: ALBERT encoder.embedding_hidden_mapping_in, ELECTRA
+       embeddings_project.  NULL = none (the embeddings are the residual stream).  AC_ARCH_BERT / AC_ARCH_ROBERTA only:
+       the projection runs AFTER the embedding LayerNorm (ALBERT / ELECTRA order; DeBERTa-v2's embed_proj, which runs
+       before it, is not implemented). */
+    const float *emb_proj_w;          /* [H, E] */
+    const float *emb_proj_b;          /* [H] */
 } ac_encoder_weights;
 
 typedef struct ac_encoder ac_encoder;
@@ -342,7 +361,8 @@ int ac_encoder_attention(ac_encoder *enc, const void *qk, const void *vT, const 
                          int cls_rows, void *ctx_out, ac_stream_t stream);
 
 /* generic tensor-core linear (the encoder's GEMM with its fused epilogues), exposed for parity tests and roofline
- * measurement: Y[M,N] = epi(X[M,K] W[N,K]^T + bias) (+ residual).  epi: 0 bias, 1 bias+GELU(erf), 2 bias+fp32 residual.
+ * measurement: Y[M,N] = epi(X[M,K] W[N,K]^T + bias) (+ residual).  epi: 0 bias, 1 bias+GELU(erf), 2 bias+fp32 residual,
+ * 3 bias+GELU(tanh) (AC_PREC_F16 with out_half != 0 only).
  * precision AC_PREC_TF32: X, W, Y fp32 (operands used as stored; round_out != 0 rounds Y to tf32);
  * precision AC_PREC_F16 : X, W fp16, Y fp32 or (out_half != 0, epi != 2) fp16. */
 int ac_linear_tc(const void *X, const void *W, const float *bias, const float *residual, void *Y,
