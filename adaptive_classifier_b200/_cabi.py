@@ -937,7 +937,10 @@ class Encoder:
         """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel / DebertaV2Model / AlbertModel /
         ElectraModel (post-LN blocks) or ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for BERT / RoBERTa /
         DistilBERT, 64 for MPNet, DeBERTa and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
-        AC_MODERNBERT_MAX_S."""
+        AC_MODERNBERT_MAX_S.  A RoBERTa / XLM-RoBERTa model with head_dim 64 whose position table has more than
+        512 + pad_token_id + 1 rows (bge-m3, snowflake-arctic-embed-l-v2.0: 8194) takes sequences up to
+        min(AC_MODERNBERT_MAX_S, max_position_embeddings - pad_token_id - 1), which run the long full-attention kernel
+        past 512 tokens; BERT-arch models keep the 512 limit."""
         c = model.config
         mt = getattr(c, "model_type", "bert")
         if mt == "modernbert":

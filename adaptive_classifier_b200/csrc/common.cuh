@@ -227,6 +227,27 @@ __device__ __forceinline__ void wgmma_m64n32_f16(float (&d)[16], uint64_t a_desc
         : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T with A in REGISTERS (f16x2 a[0..3]: rows 16 (t/32) + (t%32)/4 (+8) and
+// columns 2 (t%4) (+8) of the warp's 16 rows, the layout of an accumulator's columns 16 k .. 16 k + 15), B K-major in
+// shared memory
+__device__ __forceinline__ void wgmma_m64n64_f16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc,
+                                                    uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+}
+
 // Accumulator fragment of an m64nN wgmma -> rows of a row-major fp32 tile (ld floats per row).  Thread t of the warpgroup
 // holds, for every 8-column group j, rows 16 (t/32) + (t%32)/4 (+8) and columns 8 j + 2 (t%4) (+1).
 template <int NREG>

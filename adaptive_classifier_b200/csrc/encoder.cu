@@ -17,7 +17,9 @@
 //   attention     one CTA per (sequence, head): Q, K and V^T tiles by TMA, QK^T and PV as wgmma with the score tile
 //                 staged in shared memory, thread-per-query-row softmax in between (S <= 128; head_dim 64 or 32); longer
 //                 sequences (up to 512, ModernBERT up to 8192) run 128-query blocks over streamed key blocks in one pass with
-//                 an online softmax that visits only the key blocks inside a sliding layer's band (attention_stream_kernel)
+//                 an online softmax that visits only the key blocks inside a sliding layer's band (attention_stream_kernel);
+//                 RoBERTa-arch encoders with a long position table (XLM-R, up to 8192) run full attention past 512 with the
+//                 softmax on the wgmma fragments and P as the register A operand of the PV wgmma (attention_long_kernel)
 //   LayerNorm     never materialised inside the layer stack: the residual epilogues keep the un-normalised sums y (fp32) and
 //                 per-row (sum, sumsq) partials, the consuming projections run on gamma-scaled weights and apply the
 //                 rank-1 correction r (acc - mu c1) + c0 in their epilogue ("deferred LayerNorm" below)
@@ -1172,6 +1174,191 @@ attention_stream_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __gri
     if (qglob < S) att_write_row<DH>(srow, inv, ctx + (row0 + qglob) * H + h * DH);
 }
 
+// ------------------------------------------------------------------------------------------------
+// long full attention: RoBERTa-arch encoders past AC_ENCODER_MAX_S (XLM-R: bge-m3, arctic-embed-l-v2.0), head_dim 64,
+// window 0, no score term.  The contract of attention_stream_kernel<64, ScorePlain> (same arguments, grid, operand model
+// and empty-row rule) with the softmax on the wgmma fragments.  One CTA of 288 threads per (sequence, head, 128-query block):
+//   warp 8         producer: one lane TMA-loads Q once, then the K and V^T blocks of 128 keys through an ATTL_STAGES ring
+//                  (full barriers: bytes landed; empty barriers: one arrival per consumer warp once its P V retired)
+//   warpgroups 0-1 consumers, query rows 64 g .. 64 g + 63.  Per key block: S = Q K^T as 4 x wgmma m64n128k16 into 64 fp32
+//                  registers; keys the mask or the sequence end exclude (one bit per key of the sequence, ballotted into
+//                  shared memory once) become -inf; the row max and row sum reduce over the quad that holds a row
+//                  (shfl_xor 1, 2); O is rescaled in registers; P is packed to f16x2 and is the REGISTER A operand of
+//                  8 x wgmma m64n64k16 against the V^T slabs (the accumulator fragment of score columns [16 k, 16 k + 16) is
+//                  the A fragment of k-step k)
+// P is fp16, rounded against the running max; scores, the row sum (of the unrounded P, kept per thread and reduced once at
+// the end) and O are fp32.  A row that has seen no valid key keeps m = -inf, P = 0 and the factor 0; its context is 0.
+// Registers: 158 per thread with no spills (-Xptxas -v), so one CTA per SM; the two consumer warpgroups overlap each other's
+// softmax with their MMAs.  smem: Q 16 KB | ATTL_STAGES x (K 16 KB | V^T 16 KB) | key bits (S / 8 B, <= 1 KB) | barriers.
+// ------------------------------------------------------------------------------------------------
+constexpr int ATTL_THREADS = 288;
+constexpr int ATTL_STAGES = 4;
+constexpr int ATTL_STAGE_BYTES = 32 * 1024;                    // K block | V^T block (2 slabs of 64 keys)
+constexpr int ATTL_OFF_STAGE = 16 * 1024;
+constexpr int ATTL_OFF_BITS = ATTL_OFF_STAGE + ATTL_STAGES * ATTL_STAGE_BYTES;
+constexpr int ATTL_OFF_BAR = ATTL_OFF_BITS + AC_MODERNBERT_MAX_S / 8;
+constexpr int ATTL_SMEM = ATTL_OFF_BAR + (1 + 2 * ATTL_STAGES) * 8 + 1024 /*align*/;
+static_assert(ATTL_SMEM <= 227 * 1024, "long-attention CTA exceeds the shared-memory limit");
+
+__global__ void __launch_bounds__(ATTL_THREADS, 1)
+attention_long_kernel(const __grid_constant__ CUtensorMap tmap_qk, const __grid_constant__ CUtensorMap tmap_vt,
+                      const int32_t *__restrict__ mask, int B, int S, int heads, int H, int /*window: 0*/,
+                      __half *__restrict__ ctx, const __grid_constant__ ScorePlain) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t *sQ = smem;                                                // [128 x 128 B]: rows 64 g .. for warpgroup g
+    uint32_t *sBits = reinterpret_cast<uint32_t *>(smem + ATTL_OFF_BITS);   // bit j of word w: key 32 w + j is attended
+    uint64_t *bar_q = reinterpret_cast<uint64_t *>(smem + ATTL_OFF_BAR);
+    uint64_t *full = bar_q + 1, *empty = full + ATTL_STAGES;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+    const int q0 = blockIdx.y * 128;
+    const int row0 = b * S;
+    const int nblk = (S + 127) / 128;
+
+    if (tid == 0) {
+        tma_prefetch_desc(&tmap_qk);
+        tma_prefetch_desc(&tmap_vt);
+        mbar_init(bar_q, 1);
+        for (int st = 0; st < ATTL_STAGES; ++st) {
+            mbar_init(full + st, 1);
+            mbar_init(empty + st, 8);
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        if (lane == 0) {
+            const int vrow = (b * heads + h) * 64;
+            mbar_arrive_expect_tx(bar_q, 16 * 1024);
+            tma_load_2d(sQ, &tmap_qk, bar_q, h * 64, row0 + q0);
+            for (int i = 0; i < nblk; ++i) {
+                const int st = i % ATTL_STAGES, key0 = i * 128;
+                if (i >= ATTL_STAGES) mbar_wait_guarded(empty + st, (i / ATTL_STAGES - 1) & 1);
+                uint8_t *sK = smem + ATTL_OFF_STAGE + st * ATTL_STAGE_BYTES, *sVt = sK + 16 * 1024;
+                mbar_arrive_expect_tx(full + st, ATTL_STAGE_BYTES);
+                tma_load_2d(sK, &tmap_qk, full + st, H + h * 64, row0 + key0);
+                tma_load_2d(sVt, &tmap_vt, full + st, key0, vrow);
+                tma_load_2d(sVt + 8192, &tmap_vt, full + st, key0 + 64, vrow);
+            }
+        }
+        return;
+    }
+
+    // ---- consumers: the key bits of every key block (keys past S are clear), then the key blocks
+    for (int w = warp; w < 4 * nblk; w += 8) {
+        const int key = 32 * w + lane;
+        const bool ok = key < S && (!mask || mask[row0 + key] != 0);
+        const uint32_t bits = __ballot_sync(0xffffffffu, ok);
+        if (lane == 0) sBits[w] = bits;
+    }
+    named_bar_sync(1, 256);
+
+    const int g = warp >> 2;
+    const int r0 = 16 * (warp & 3) + (lane >> 2), c2 = 2 * (lane & 3);   // fragment rows r0, r0 + 8; columns 8 j + c2 (+1)
+    const float sl2 = 0.125f * 1.44269504088896340736f;                 // log2(e) / sqrt(64)
+    float o[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) o[j] = 0.f;
+    float mx0 = -CUDART_INF_F, mx1 = -CUDART_INF_F, sum0 = 0.f, sum1 = 0.f;
+    const uint64_t qa = wgmma_desc_sw128(smem_u32(sQ + g * 8192));
+    mbar_wait_guarded(bar_q, 0);
+
+#pragma unroll 1
+    for (int i = 0; i < nblk; ++i) {
+        const int st = i % ATTL_STAGES;
+        const uint8_t *sK = smem + ATTL_OFF_STAGE + st * ATTL_STAGE_BYTES, *sVt = sK + 16 * 1024;
+        mbar_wait_guarded(full + st, (i / ATTL_STAGES) & 1);
+        float s[64];
+        {
+            const uint64_t bd = wgmma_desc_sw128(smem_u32(sK));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_m64n128_f16(s, qa + 2 * k, bd + 2 * k, k != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+        }
+        const uint4 kw = *reinterpret_cast<const uint4 *>(sBits + 4 * i);
+        if ((kw.x & kw.y & kw.z & kw.w) != 0xffffffffu) {
+            const uint32_t words[4] = {kw.x, kw.y, kw.z, kw.w};
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const uint32_t bits = words[j >> 2] >> (8 * (j & 3) + c2);
+                if (!(bits & 1u)) s[4 * j] = s[4 * j + 2] = -CUDART_INF_F;
+                if (!(bits & 2u)) s[4 * j + 1] = s[4 * j + 3] = -CUDART_INF_F;
+            }
+        }
+        float m0 = mx0, m1 = mx1;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            m0 = fmaxf(m0, fmaxf(s[4 * j], s[4 * j + 1]));
+            m1 = fmaxf(m1, fmaxf(s[4 * j + 2], s[4 * j + 3]));
+        }
+#pragma unroll
+        for (int x = 1; x <= 2; x <<= 1) {
+            m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, x));
+            m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, x));
+        }
+        const float alpha0 = (mx0 == -CUDART_INF_F) ? 0.f : ex2_approx((mx0 - m0) * sl2);
+        const float alpha1 = (mx1 == -CUDART_INF_F) ? 0.f : ex2_approx((mx1 - m1) * sl2);
+        const float ms0 = (m0 == -CUDART_INF_F) ? 0.f : m0 * sl2;      // no valid key yet: every P below is 0
+        const float ms1 = (m1 == -CUDART_INF_F) ? 0.f : m1 * sl2;
+        mx0 = m0;
+        mx1 = m1;
+        uint32_t p[32];
+        float ps0 = 0.f, ps1 = 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const float e0 = ex2_approx(fmaf(s[4 * j], sl2, -ms0)), e1 = ex2_approx(fmaf(s[4 * j + 1], sl2, -ms0));
+            const float e2 = ex2_approx(fmaf(s[4 * j + 2], sl2, -ms1)), e3 = ex2_approx(fmaf(s[4 * j + 3], sl2, -ms1));
+            ps0 += e0 + e1;
+            ps1 += e2 + e3;
+            __half2 h01 = __floats2half2_rn(e0, e1), h23 = __floats2half2_rn(e2, e3);
+            p[2 * j] = *reinterpret_cast<uint32_t *>(&h01);
+            p[2 * j + 1] = *reinterpret_cast<uint32_t *>(&h23);
+        }
+        sum0 = fmaf(sum0, alpha0, ps0);
+        sum1 = fmaf(sum1, alpha1, ps1);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            o[4 * j] *= alpha0;
+            o[4 * j + 1] *= alpha0;
+            o[4 * j + 2] *= alpha1;
+            o[4 * j + 3] *= alpha1;
+        }
+        {
+            const uint64_t bv = wgmma_desc_sw128(smem_u32(sVt));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const uint32_t a[4] = {p[4 * k], p[4 * k + 1], p[4 * k + 2], p[4 * k + 3]};
+                wgmma_m64n64_f16_rs(o, a, bv + (k >> 2) * 512 + 2 * (k & 3), 1u);   // slab k / 4 is 8192 B on
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+        }
+        if (lane == 0) mbar_arrive(empty + st);
+    }
+
+#pragma unroll
+    for (int x = 1; x <= 2; x <<= 1) {
+        sum0 += __shfl_xor_sync(0xffffffffu, sum0, x);
+        sum1 += __shfl_xor_sync(0xffffffffu, sum1, x);
+    }
+    const float inv0 = (sum0 > 0.f) ? 1.f / sum0 : 0.f, inv1 = (sum1 > 0.f) ? 1.f / sum1 : 0.f;
+    const int q = q0 + 64 * g + r0;
+    __half *dst = ctx + (static_cast<int64_t>(row0) + q) * H + h * 64 + c2;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if (q < S) *reinterpret_cast<__half2 *>(dst + 8 * j) = __floats2half2_rn(o[4 * j] * inv0, o[4 * j + 1] * inv0);
+        if (q + 8 < S)
+            *reinterpret_cast<__half2 *>(dst + 8 * static_cast<int64_t>(H) + 8 * j) =
+                __floats2half2_rn(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+    }
+}
+
 // last layer, deferred flow: CLS rows of the attention context and of LN_pending(y) (two-pass statistics from the fp32 sums)
 __global__ void gather_cls_ln_kernel(const __half *__restrict__ ctx, const float *__restrict__ y, int B, int S, int H,
                                      const float *__restrict__ g, const float *__restrict__ b, float eps,
@@ -1285,23 +1472,26 @@ static int launch_cls_normalize(const float *x, int B, int S, int H, float *out,
     return AC_OK;
 }
 
-// Every attention variant the library runs, with the dynamic shared memory the kernel is allowed and launched with (rows in
-// the enum's order).  All take the same arguments up to their score term.
-struct AttVariant { const void *kernel; int smem; };
-enum { ATT_PLAIN64, ATT_PLAIN32, ATT_RELBIAS, ATTS_PLAIN64, ATTS_PLAIN32, ATTS_RELBIAS, ATTS_DISENT, ATT_VARIANTS };
+// Every attention variant the library runs, with the dynamic shared memory the kernel is allowed and launched with and its
+// block size (rows in the enum's order).  All take the same arguments up to their score term.
+struct AttVariant { const void *kernel; int smem, threads; };
+enum { ATT_PLAIN64, ATT_PLAIN32, ATT_RELBIAS, ATTS_PLAIN64, ATTS_PLAIN32, ATTS_RELBIAS, ATTS_DISENT, ATTL_PLAIN64, ATT_VARIANTS };
 static const AttVariant att_variants[ATT_VARIANTS] = {
-    {reinterpret_cast<const void *>(attention_kernel<64, ScorePlain>), ATT_SMEM<ScorePlain>},
-    {reinterpret_cast<const void *>(attention_kernel<32, ScorePlain>), ATT_SMEM<ScorePlain>},
-    {reinterpret_cast<const void *>(attention_kernel<64, ScoreRelBias>), ATT_SMEM<ScoreRelBias>},
-    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScorePlain>), ATTS_SMEM<ScorePlain>},
-    {reinterpret_cast<const void *>(attention_stream_kernel<32, ScorePlain>), ATTS_SMEM<ScorePlain>},
-    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScoreRelBias>), ATTS_SMEM<ScoreRelBias>},
-    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScoreDisent>), ATTS_SMEM<ScoreDisent>},
+    {reinterpret_cast<const void *>(attention_kernel<64, ScorePlain>), ATT_SMEM<ScorePlain>, ATT_THREADS},
+    {reinterpret_cast<const void *>(attention_kernel<32, ScorePlain>), ATT_SMEM<ScorePlain>, ATT_THREADS},
+    {reinterpret_cast<const void *>(attention_kernel<64, ScoreRelBias>), ATT_SMEM<ScoreRelBias>, ATT_THREADS},
+    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScorePlain>), ATTS_SMEM<ScorePlain>, ATT_THREADS},
+    {reinterpret_cast<const void *>(attention_stream_kernel<32, ScorePlain>), ATTS_SMEM<ScorePlain>, ATT_THREADS},
+    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScoreRelBias>), ATTS_SMEM<ScoreRelBias>, ATT_THREADS},
+    {reinterpret_cast<const void *>(attention_stream_kernel<64, ScoreDisent>), ATTS_SMEM<ScoreDisent>, ATT_THREADS},
+    {reinterpret_cast<const void *>(attention_long_kernel), ATTL_SMEM, ATTL_THREADS},
 };
 
 // softmax(Q K^T / sqrt(head_dim) [+ MPNet relative bias] + mask) V out of e->qk / e->vT into e->ctx; window = sliding
 // half-window, 0 = full attention.  S <= 128 runs attention_kernel, longer sequences attention_stream_kernel over 128-query
 // blocks; DeBERTa runs attention_stream_kernel<64, ScoreDisent> at every length, with layer `layer`'s c2p / p2c boxes.
+// Past AC_ENCODER_MAX_S every encoder but ModernBERT (in practice RoBERTa-arch ones with a long position table,
+// check_shape_map_vt) runs attention_long_kernel; ModernBERT keeps attention_stream_kernel at every length.
 // cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail), so only the first query block is computed.
 static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, int layer,
                             cudaStream_t s) {
@@ -1344,11 +1534,13 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, in
         bias.rel_bias = e->rel_bias;
         score = &bias;
         id = streamed ? ATTS_RELBIAS : ATT_RELBIAS;
+    } else if (S > AC_ENCODER_MAX_S && c.arch != AC_ARCH_MODERNBERT) {
+        id = ATTL_PLAIN64;                    // head_dim 64 (checked above), window 0 (only ModernBERT has bands)
     }
     const AttVariant &v = att_variants[id];
     void *args[] = {&e->m_qk_att, &e->m_vt_att, &mask, &B, &S, &heads, &H, &window, &e->ctx, score};
     // a launch error is the runtime's last error, which AC_LAUNCH_CHECK reads
-    cudaLaunchKernel(v.kernel, dim3(B * heads, streamed ? q_blocks : 1), dim3(ATT_THREADS), args, v.smem, s);
+    cudaLaunchKernel(v.kernel, dim3(B * heads, streamed ? q_blocks : 1), dim3(v.threads), args, v.smem, s);
     prof_end(slot, s);
     AC_LAUNCH_CHECK();
     return AC_OK;
@@ -1740,9 +1932,21 @@ static int check_shape_map_vt(ac_encoder *e, const char *who, int B, int S) {
         // RoPE has no position table: any S up to the encoder's max_pos (<= AC_MODERNBERT_MAX_S) runs
         AC_REQUIRE(S <= e->cfg.max_pos, "%s: S=%d exceeds this ModernBERT encoder's max_pos=%d (max_position_embeddings)", who,
                    S, e->cfg.max_pos);
-    } else if (S > 512) {
-        set_error("%s: S=%d > 512 is not supported (the reference truncates at max_length = 512)", who, S);
-        return AC_E_UNSUPPORTED;
+    } else if (S > AC_ENCODER_MAX_S) {
+        // RoBERTa positions run from pad_idx + 1: a table with more rows than AC_ENCODER_MAX_S of them (XLM-R's 8194) takes
+        // the sequences it has positions for, up to AC_MODERNBERT_MAX_S
+        const ac_encoder_config &c = e->cfg;
+        if (c.arch != AC_ARCH_ROBERTA || c.max_pos <= AC_ENCODER_MAX_S + c.pad_idx + 1) {
+            set_error("%s: S=%d > 512 is not supported (the reference truncates at max_length = 512)", who, S);
+            return AC_E_UNSUPPORTED;
+        }
+        const int s_max = std::min(AC_MODERNBERT_MAX_S, c.max_pos - c.pad_idx - 1);
+        if (S > s_max) {
+            set_error("%s: S=%d exceeds %d, the longest sequence this RoBERTa encoder has positions for "
+                      "(max_position_embeddings=%d, positions from pad_idx + 1 = %d, at most %d)",
+                      who, S, s_max, c.max_pos, c.pad_idx + 1, AC_MODERNBERT_MAX_S);
+            return AC_E_UNSUPPORTED;
+        }
     }
     AC_REQUIRE(static_cast<int64_t>(B) * S <= e->cfg.max_tokens, "%s: B*S=%lld exceeds max_tokens=%d", who,
                static_cast<long long>(B) * S, e->cfg.max_tokens);

@@ -88,6 +88,28 @@ def electra_small(seed: int = 1234):
     return m, cfg
 
 
+def bge_m3(seed: int = 1234):
+    """HF XLMRobertaModel of the BAAI/bge-m3 shape (XLM-RoBERTa-large with 8194 positions: 24 x 1024, 16 heads, I = 4096,
+    vocab 250002, pad id 1, one token type, LayerNorm eps 1e-5), random init under torch.manual_seed(seed).
+    Snowflake/snowflake-arctic-embed-l-v2.0 has the same shape."""
+    from transformers import XLMRobertaConfig, XLMRobertaModel
+    torch.manual_seed(seed)
+    cfg = XLMRobertaConfig(vocab_size=250002, hidden_size=1024, num_hidden_layers=24, num_attention_heads=16,
+                           intermediate_size=4096, max_position_embeddings=8194, type_vocab_size=1, layer_norm_eps=1e-5,
+                           pad_token_id=1, bos_token_id=0, eos_token_id=2)
+    m = XLMRobertaModel(cfg, add_pooling_layer=False)
+    m.eval()
+    return m, cfg
+
+
+def xlmr_ids(B: int, S: int, seed: int = 7, vocab: int = 250002) -> torch.Tensor:
+    """uniform in [5, vocab), <s>=0 first, </s>=2 last, never the pad id 1; int32 [B,S] on the host."""
+    g = torch.Generator().manual_seed(seed)
+    ids = torch.randint(5, vocab, (B, S), generator=g, dtype=torch.int64)
+    ids[:, 0], ids[:, -1] = 0, 2
+    return ids.to(torch.int32)
+
+
 def modernbert_ids(B: int, S: int, seed: int = 7) -> torch.Tensor:
     """uniform in [1000, 50000), [CLS]=50281 first, [SEP]=50282 last, never the pad id 50283; int32 [B,S] on the host."""
     g = torch.Generator().manual_seed(seed)

@@ -249,7 +249,9 @@ enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2,
        AC_ARCH_DEBERTA = 4 /* DeBERTa-v2/v3: post-LN BERT block, BERT positions, disentangled c2p + p2c attention
                               (pos_key, pos_query, pos_span, rel_index); head_dim 64 */ };
 #define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts for BERT / RoBERTa / DistilBERT (their
-                                  position tables stop at 512) */
+                                  position tables stop at 512).  An AC_ARCH_ROBERTA encoder whose table has more than
+                                  AC_ENCODER_MAX_S + pad_idx + 1 rows (XLM-R: bge-m3, arctic-embed-l-v2.0, 8194 rows) accepts
+                                  S <= min(AC_MODERNBERT_MAX_S, max_pos - pad_idx - 1) */
 #define AC_MODERNBERT_MAX_S 8192   /* largest max_pos of an AC_ARCH_MODERNBERT encoder (max_position_embeddings of the
                                       published checkpoints) */
 enum {
@@ -339,7 +341,9 @@ int ac_encoder_destroy(ac_encoder *enc);
 
 /* ids[B,S] int32 token ids, mask[B,S] int32 (1 keep / 0 pad; NULL = all ones), type_ids nullable (ignored by
  * AC_ARCH_MODERNBERT, whose RoPE positions are 0..S-1 for every sequence, padded or not).  S <= AC_ENCODER_MAX_S, or
- * S <= max_pos for AC_ARCH_MODERNBERT.
+ * S <= max_pos for AC_ARCH_MODERNBERT, or, for an AC_ARCH_ROBERTA encoder with max_pos > AC_ENCODER_MAX_S + pad_idx + 1,
+ * S <= min(AC_MODERNBERT_MAX_S, max_pos - pad_idx - 1) (its positions run from pad_idx + 1; head_dim 64 past
+ * AC_ENCODER_MAX_S).
  * out_unit_cls[B,H] = L2-normalised (eps 1e-12) CLS row of the last hidden state. */
 int ac_encoder_forward_cls(ac_encoder *enc, const int32_t *ids, const int32_t *mask,
                            const int32_t *type_ids, int B, int S, float *out_unit_cls,
