@@ -26,12 +26,12 @@ AC_ACT_LOGITS, AC_ACT_SOFTMAX, AC_ACT_SIGMOID = 0, 1, 2
 AC_LOSS_CE, AC_LOSS_BCE, AC_LOSS_CE_STRATEGIC = 0, 1, 2
 AC_COST_LINEAR, AC_COST_SEPARABLE = 0, 1
 AC_STRATEGIC_CANDIDATES = 50
-AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERTA = 0, 1, 2, 3, 4
+AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERTA, AC_ARCH_ROTARY = 0, 1, 2, 3, 4, 5
 AC_ENCODER_MAX_S = 512
 AC_MODERNBERT_MAX_S = 8192
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
-AC_FFN_GELU_ERF, AC_FFN_GELU_TANH = 0, 1
-# hidden_act of a post-LN (BERT-family) config -> ac_encoder_config.ffn_act
+AC_FFN_GELU_ERF, AC_FFN_GELU_TANH, AC_FFN_SWIGLU = 0, 1, 2
+# hidden_act of a post-LN (BERT-family) config -> ac_encoder_config.ffn_act (SwiGLU is NomicBERT's alone: nomic_bert_settings)
 FFN_ACTS = {"gelu": AC_FFN_GELU_ERF, "gelu_new": AC_FFN_GELU_TANH, "gelu_pytorch_tanh": AC_FFN_GELU_TANH}
 
 EXPORTS = [
@@ -523,14 +523,15 @@ def ewc_penalty(p, fisher, star, lam: float, batch_size: Optional[int], C_old: i
 
 
 def linear_tc(X, W, bias, residual=None, epi: int = 0, round_out: bool = False, out_half: bool = False) -> torch.Tensor:
-    """X, W fp32 -> tf32 path; X, W fp16 -> fp16 path (the encoder's); Y fp32 unless out_half."""
+    """X, W fp32 -> tf32 path; X, W fp16 -> fp16 path (the encoder's); Y fp32 unless out_half.  epi 4 (SwiGLU) takes W's
+    rows interleaved in 32-row groups (activated, multiplier) and returns Y [M, N / 2]."""
     L = load_library()
     assert X.is_cuda and W.is_cuda and X.dtype == W.dtype and X.dtype in (torch.float32, torch.float16)
     X, W = X.contiguous(), W.contiguous()
     prec = AC_PREC_F16 if X.dtype == torch.float16 else AC_PREC_TF32
     M, K = X.shape
     N = W.shape[0]
-    Y = torch.empty((M, N), dtype=torch.float16 if out_half else torch.float32, device=X.device)
+    Y = torch.empty((M, N // 2 if epi == 4 else N), dtype=torch.float16 if out_half else torch.float32, device=X.device)
     check(L.ac_linear_tc(X.data_ptr(), W.data_ptr(), ptr(bias), ptr(residual), Y.data_ptr(), M, N, K, epi,
                          1 if round_out else 0, prec, 1 if out_half else 0, stream_ptr()), "ac_linear_tc")
     return Y
@@ -841,12 +842,97 @@ def modernbert_settings(c) -> dict:
                 rope_theta=(theta["full_attention"], theta["sliding_attention"]))
 
 
+def _rotary_settings(c, family: str, acts) -> None:
+    """Refusals shared by NomicBERT and jina-embeddings-v3 (post-LN BERT blocks with RoPE on q and k), raised before any
+    device call with the setting's name."""
+    rp = getattr(c, "rope_parameters", None) or {}
+    if rp.get("rope_type", "default") != "default":
+        raise AdaptiveB200Error(f"{family} rope_type={rp.get('rope_type')!r} is not implemented in the CUDA path (only "
+                                "'default' RoPE; dynamic NTK, YaRN and linear scaling need a table per sequence length)")
+    H, heads = c.hidden_size, c.num_attention_heads
+    if H % 128 != 0 or H > 1024:
+        raise AdaptiveB200Error(f"{family} hidden_size={H} is not implemented in the CUDA path: the encoder takes hidden "
+                                "<= 1024 in multiples of 128")
+    head_dim = getattr(c, "head_dim", None) or (H // heads if heads > 0 else 0)
+    if heads <= 0 or head_dim != 64 or H != 64 * heads:
+        raise AdaptiveB200Error(f"{family} head_dim={head_dim} (hidden={H}, heads={heads}) is not implemented in the CUDA "
+                                "path: only head_dim 64")
+    if c.hidden_act not in acts:
+        raise AdaptiveB200Error(f"{family} hidden_act={c.hidden_act!r} is not implemented in the CUDA path (only "
+                                f"{', '.join(repr(a) for a in acts)})")
+
+
+def nomic_bert_settings(c) -> None:
+    """Raises AdaptiveB200Error naming any NomicBertConfig setting the CUDA path does not implement (no device call)."""
+    _rotary_settings(c, "NomicBERT", ("silu", "swish"))
+
+
+def jina_v3_settings(c) -> None:
+    """Raises AdaptiveB200Error naming any JinaEmbeddingsV3Config setting the CUDA path does not implement (no device
+    call)."""
+    _rotary_settings(c, "jina-embeddings-v3", tuple(FFN_ACTS))
+
+
+def _rotary_dims(c, ffn_act: int) -> dict:
+    """Encoder dims of a rotary config: max_pos = the RoPE table's rows and the longest S, max(512, min(max_position_embeddings,
+    AC_MODERNBERT_MAX_S)) (HF itself fails past max_position_embeddings when no token_type_ids are passed)"""
+    rp = getattr(c, "rope_parameters", None) or {}
+    return dict(layers=c.num_hidden_layers, hidden=c.hidden_size, heads=c.num_attention_heads,
+                intermediate=c.intermediate_size, vocab=c.vocab_size,
+                max_pos=max(AC_ENCODER_MAX_S, min(int(c.max_position_embeddings), AC_MODERNBERT_MAX_S)),
+                type_vocab=max(int(c.type_vocab_size), 1), ln_eps=c.layer_norm_eps, pad_idx=0, ffn_act=ffn_act,
+                rope_theta=float(rp.get("rope_theta", getattr(c, "default_theta", 10000.0))))
+
+
+def _rotary_to_bert_state_dict(sd: dict, c, ffn, ffn_act: int):
+    """the native names of a NomicBertModel / JinaEmbeddingsV3Model (layers.l.self_attn.*, post_*_layernorm, mlp.*) as the
+    BERT names Encoder consumes; ffn(sd, layer prefix) gives the FFN's BERT names -> (weight, bias or None).  Biases the checkpoint does
+    not have become zeros, so that ac_encoder_create never sees a NULL bias.  pooler.* is not used."""
+    out = {k: sd[k] for k in ("embeddings.word_embeddings.weight", "embeddings.token_type_embeddings.weight",
+                              "embeddings.LayerNorm.weight", "embeddings.LayerNorm.bias")}
+    ren = {"self_attn.q_proj": "attention.self.query", "self_attn.k_proj": "attention.self.key",
+           "self_attn.v_proj": "attention.self.value", "self_attn.o_proj": "attention.output.dense",
+           "post_attention_layernorm": "attention.output.LayerNorm", "post_mlp_layernorm": "output.LayerNorm"}
+    for l in range(c.num_hidden_layers):
+        src, dst = f"layers.{l}.", f"encoder.layer.{l}."
+        for a, b in ren.items():
+            w = sd[src + a + ".weight"]
+            out[dst + b + ".weight"] = w
+            out[dst + b + ".bias"] = sd.get(src + a + ".bias", torch.zeros(w.shape[0], dtype=torch.float32))
+        for b, (w, bias) in ffn(sd, src).items():
+            out[dst + b + ".weight"] = w
+            out[dst + b + ".bias"] = bias if bias is not None else torch.zeros(w.shape[0], dtype=torch.float32)
+    return out, _rotary_dims(c, ffn_act)
+
+
+def nomic_bert_to_bert_state_dict(sd: dict, c):
+    """NomicBERT (HF models/nomic_bert): RoPE (theta 1000 by default), no q/k/v/o biases, SwiGLU FFN
+    down(silu(gate_proj x) * up_proj x) without biases.  FFN1 is cat([gate_proj, up_proj]) [2I, H] (AC_FFN_SWIGLU's row
+    order).  Returns the BERT names and the Encoder dims (arch "rotary")."""
+    nomic_bert_settings(c)
+    ffn = lambda sd, p: {
+        "intermediate.dense": (torch.cat([sd[p + "mlp.gate_proj.weight"], sd[p + "mlp.up_proj.weight"]]), None),
+        "output.dense": (sd[p + "mlp.down_proj.weight"], None)}
+    return _rotary_to_bert_state_dict(sd, c, ffn, AC_FFN_SWIGLU)
+
+
+def jina_v3_to_bert_state_dict(sd: dict, c):
+    """jina-embeddings-v3 (HF models/jina_embeddings_v3): RoPE (theta 20000 by default) with q/k/v/o biases, FFN
+    fc2(GELU(fc1 x)) with biases.  Returns the BERT names and the Encoder dims (arch "rotary")."""
+    jina_v3_settings(c)
+    ffn = lambda sd, p: {"intermediate.dense": (sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"]),
+                         "output.dense": (sd[p + "mlp.fc2.weight"], sd[p + "mlp.fc2.bias"])}
+    return _rotary_to_bert_state_dict(sd, c, ffn, FFN_ACTS[c.hidden_act])
+
+
 class Encoder:
     """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors).  arch "mpnet"
     takes the BERT names (mpnet_to_bert_state_dict) and rel_bias, the [heads, 2 AC_ENCODER_MAX_S - 1] table of
     mpnet_relative_bias_table; arch "deberta" the BERT names and the pos_key / pos_query / pos_span / rel_index of
     deberta_to_bert_state_dict.  embedding_size (0 = hidden) and the "embeddings_project.*" tensors give factorized
     embeddings (albert_to_bert_state_dict, electra_to_bert_state_dict); ffn_act is AC_FFN_GELU_ERF or AC_FFN_GELU_TANH.
+    arch "rotary" takes the BERT names without a position table, RoPE with base rope_theta on q and k, and ffn_act
+    AC_FFN_SWIGLU too (nomic_bert_to_bert_state_dict, jina_v3_to_bert_state_dict).
     Names that refer to the same source tensor (ALBERT's shared layers) are copied and packed once."""
 
     def __init__(self, sd: dict, *, arch: str, layers: int, hidden: int, heads: int, intermediate: int, vocab: int,
@@ -897,7 +983,8 @@ class Encoder:
                                 ctypes.cast(ls, POINTER(ctypes.c_int32)), rope[0].data_ptr(), rope[1].data_ptr())
         else:
             w.word_emb = g("embeddings.word_embeddings.weight")
-            w.pos_emb = g("embeddings.position_embeddings.weight")
+            if arch != "rotary":
+                w.pos_emb = g("embeddings.position_embeddings.weight")
             w.type_emb = g("embeddings.token_type_embeddings.weight")
             w.emb_ln_w = g("embeddings.LayerNorm.weight")
             w.emb_ln_b = g("embeddings.LayerNorm.bias")
@@ -912,10 +999,15 @@ class Encoder:
             w.out_ln_w, w.out_ln_b = arr(p + "output.LayerNorm.weight"), arr(p + "output.LayerNorm.bias")
             if "embeddings_project.weight" in sd:      # factorized embeddings (ALBERT, ELECTRA)
                 w.emb_proj_w, w.emb_proj_b = g("embeddings_project.weight"), g("embeddings_project.bias")
-            code = {"bert": AC_ARCH_BERT, "roberta": AC_ARCH_ROBERTA, "mpnet": AC_ARCH_MPNET, "deberta": AC_ARCH_DEBERTA}[arch]
+            code = {"bert": AC_ARCH_BERT, "roberta": AC_ARCH_ROBERTA, "mpnet": AC_ARCH_MPNET, "deberta": AC_ARCH_DEBERTA,
+                    "rotary": AC_ARCH_ROTARY}[arch]
             cfg = EncoderConfig(code, layers, hidden, heads, intermediate, vocab, max_pos, type_vocab, pad_idx, ln_eps,
                                 AC_PREC_F16, max_tokens, 1 if cls_only else 0)
             cfg.embedding_size, cfg.ffn_act = embedding_size, ffn_act
+            if arch == "rotary":          # ac_encoder_create refuses a rotary encoder without its table
+                rope = modernbert_rope_table(float(rope_theta), max_pos).to(dev)
+                keep["rope"] = rope
+                cfg.rope_full = rope.data_ptr()
             if rel_bias is not None:      # ac_encoder_create refuses an MPNet encoder without it
                 rb = rel_bias.detach().to(device=dev, dtype=torch.float32).contiguous()
                 keep["rel_bias"] = rb
@@ -935,7 +1027,10 @@ class Encoder:
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
         """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel / DebertaV2Model / AlbertModel /
-        ElectraModel (post-LN blocks) or ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  head_dim 64 or 32 for BERT / RoBERTa /
+        ElectraModel / NomicBertModel / JinaEmbeddingsV3Model (post-LN blocks; the last two with RoPE, Nomic's FFN SwiGLU) or
+        ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  NomicBERT and jina-embeddings-v3 take sequences up
+        to max(512, min(max_position_embeddings, AC_MODERNBERT_MAX_S)), RoPE positions 0..S-1 whatever the padding; their
+        remote-code modules (trust_remote_code=True), whose parameter names differ, are refused.  head_dim 64 or 32 for BERT / RoBERTa /
         DistilBERT, 64 for MPNet, DeBERTa and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
         AC_MODERNBERT_MAX_S.  A RoBERTa / XLM-RoBERTa model with head_dim 64 whose position table has more than
         512 + pad_token_id + 1 rows (bge-m3, snowflake-arctic-embed-l-v2.0: 8194) takes sequences up to
@@ -967,6 +1062,16 @@ class Encoder:
         if mt == "electra":
             sd, dims = electra_to_bert_state_dict(dict(model.state_dict()), c)
             return cls(sd, arch="bert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
+        if mt in ("nomic_bert", "jina_embeddings_v3"):
+            from transformers import JinaEmbeddingsV3Model, NomicBertModel
+            native = NomicBertModel if mt == "nomic_bert" else JinaEmbeddingsV3Model
+            if not isinstance(model, native):
+                raise AdaptiveB200Error(f"model_type '{mt}' from {type(model).__module__}.{type(model).__name__} is not the "
+                                        f"native transformers {native.__name__}: remote-code modules (trust_remote_code=True) "
+                                        "are not implemented in the CUDA path; load the model without trust_remote_code")
+            to_bert = nomic_bert_to_bert_state_dict if mt == "nomic_bert" else jina_v3_to_bert_state_dict
+            sd, dims = to_bert(dict(model.state_dict()), c)
+            return cls(sd, arch="rotary", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
         if mt not in ("bert", "roberta", "xlm-roberta"):
             raise AdaptiveB200Error(f"encoder architecture '{mt}' is not implemented in the CUDA path yet")
         if getattr(c, "hidden_act", "gelu") not in FFN_ACTS or getattr(c, "position_embedding_type", "absolute") != "absolute":

@@ -3,8 +3,9 @@
 // Replaces `self.model(**inputs).last_hidden_state[:, 0, :]` + F.normalize at
 // /root/reference/src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel.forward:
 // embeddings modeling_bert.py:53-113, self-attention :143-207, output+LN :287-298, FFN :330-356;
-// HF ModernBertModel.forward in models/modernbert/modeling_modernbert.py).  One layer loop (forward_layers) runs both
-// block kinds; they differ in the LayerNorm left pending on the residual path and in compile-time epilogue choices.
+// HF ModernBertModel.forward in models/modernbert/modeling_modernbert.py; NomicBertModel / JinaEmbeddingsV3Model, the
+// post-LN block with RoPE and, for Nomic, a SwiGLU FFN).  One layer loop (forward_layers) runs both block kinds; they
+// differ in the LayerNorm left pending on the residual path and in compile-time epilogue choices.
 //
 // Precision: every tensor-core operand is fp16 (RNE from fp32), accumulation fp32 (wgmma), residual stream, LayerNorm,
 // softmax and GELU in fp32.  fp16 carries the same 10-bit mantissa as tf32, so the measured error is the tf32 one
@@ -70,6 +71,15 @@ __device__ __forceinline__ float gelu_tanh(float y) {
     constexpr float k3 = static_cast<float>(-2.0 * 0.79788456080286535588 * 1.4426950408889634074 * 0.044715);
     const float t = y * fmaf(k3, y * y, k1);
     return y * rcp_approx(1.f + ex2_approx(t));
+}
+// SiLU (NomicBERT's SwiGLU, HF "silu" / "swish"):  y sigma(y) = y / (1 + exp(-y)) = y / (1 + 2^t), t = y k, k = -log2(e)
+// rounded once from double.  2 MUFU + 3 FP32 ops.  Relative error: k and the product are 1/2 ulp each, |dt| <= 2 * 2^-24 |t|,
+// an exp error <= 2 ln2 |t| 2^-24 (<= 1.0e-5 for |t| <= 126; the inputs with |y| <= 20 have |t| <= 29: <= 2.4e-6), damped by
+// 2^t / (1 + 2^t) < 1 in the quotient; ex2.approx <= 2 ulp, the add 1/2 ulp, rcp.approx <= 1 ulp, the product 1/2 ulp
+// (< 5e-7 together).  For y < -88.7 (t > 128) 2^t = +inf and the result is y * 0 = -0, never NaN; for t < -126 it is y.
+__device__ __forceinline__ float silu(float y) {
+    constexpr float k = static_cast<float>(-1.4426950408889634074);
+    return y * rcp_approx(1.f + ex2_approx(y * k));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -162,12 +172,13 @@ struct EpiF32 : EpiBase {
 //   Act::GeGLU  (ModernBERT's mlp.Wi) pack_defer_kernel interleaved the weight rows in 32-row groups, so a warp's slice
 //               holds [input cols 32 g .. + 31 | gate cols 32 g .. + 31]; the gate chunk re-reads the input chunk from the
 //               accumulator tile and writes fp16(GELU_erf(input) * gate) to columns 32 g.. of Y (N = 2 I, ldy = I)
+//   Act::SwiGLU (NomicBERT's gate_proj | up_proj) GeGLU's layout and path with silu: fp16(silu(gate_proj) * up_proj)
 //   Act::Rope   (q and k of ModernBERT's Wqkv) rotated in fp32 before the fp16 rounding: the pair (d, d + 32) of a head is
 //               the two chunks of a warp's slice, the partner re-read from the accumulator tile; position = row % S
 // DEFER: the A operand was the UN-normalised residual sum y (fp16) and the weights were packed as fp16(gamma * W):
 //   LayerNorm(y) W^T + b = r (acc - mu c1) + c0  with the row statistics (mu, r) of y, c1 = rowsum(W'), and `bias`
 //   holding c0 = W beta + b  (producer side: EpiResidDefer)
-enum class Act { None, Gelu, GeGLU, Rope, GeluTanh };
+enum class Act { None, Gelu, GeGLU, Rope, GeluTanh, SwiGLU };
 // the activation an EpiF16 applies to every pre-activation (GeGLU and RoPE combine a chunk with its partner instead)
 template <Act ACT>
 __device__ __forceinline__ float act_elem(float y) {
@@ -199,7 +210,7 @@ struct EpiF16 : EpiBase {
                                          int lane, int, const float *acc) const {
         const int row_base = row - lane;                                     // first row of this warp's quarter
         if (row_base >= M || col0 >= N) return;                              // warp-uniform
-        constexpr bool GLU = ACT == Act::GeGLU, ROT = ACT == Act::Rope;
+        constexpr bool GLU = ACT == Act::GeGLU || ACT == Act::SwiGLU, ROT = ACT == Act::Rope;
         if (GLU && (col0 & 32) == 0) return;                                 // input chunk: consumed by its gate chunk
         const int ocol0 = GLU ? (col0 - 32) / 2 : col0, oN = GLU ? N / 2 : N;
         const int pofs = (col0 & 32) ? -32 : 32;                             // partner chunk (RoPE half / GeGLU input)
@@ -232,7 +243,8 @@ struct EpiF16 : EpiBase {
                 p[6] = pre(st, a1.z, pbb.z, pcb.z); p[7] = pre(st, a1.w, pbb.w, pcb.w);
                 if (GLU) {
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) y[k] = gelu_erf(p[k]) * y[k];          // y = gate, p = input
+                    for (int k = 0; k < 8; ++k)                                         // y = gate, p = input
+                        y[k] = (ACT == Act::SwiGLU ? silu(p[k]) : gelu_erf(p[k])) * y[k];
                 } else {
                     // HF apply_rotary_pos_emb: x cos + rotate_half(x) sin, rotate_half = (-x[32:], x[:32])
                     const float4 c0v = __ldg(reinterpret_cast<const float4 *>(rrow + 8 * j));
@@ -477,7 +489,7 @@ __global__ void fill_value_kernel(float *__restrict__ p, int n, float v) {
 //   Wp[n,k] = fp16(gamma[k] W[n,k]),  c1[n] = sum_k Wp[n,k] (fp32),  c0[n] = sum_k beta[k] W[n,k] + bias[n]
 // gamma / beta NULL = identity LayerNorm (layer 0 consumes the already normalised embeddings), bias NULL = 0.
 // glu != 0 (GeGLU weight [2I, H], N = 2I): packed row n takes source row (n / 64) 32 + n % 32 of the input half for
-// n % 64 < 32, the same row of the gate half otherwise -- the row order EpiF16<Act::GeGLU, ..> expects
+// n % 64 < 32, the same row of the gate half otherwise -- the row order EpiF16<Act::GeGLU / Act::SwiGLU, ..> expects
 __global__ void pack_defer_kernel(const float *__restrict__ W, const float *__restrict__ bias, const float *__restrict__ gamma,
                                   const float *__restrict__ beta, int N, int K, __half *__restrict__ Wp, float *__restrict__ c1,
                                   float *__restrict__ c0, int glu = 0) {
@@ -1454,7 +1466,7 @@ struct ac_encoder {
     // row statistics (ping-pong) and the per-GEMM_EPI_COLS-column partials the residual epilogues write
     float2 *stats_a = nullptr, *stats_b = nullptr, *stats_id = nullptr, *parts = nullptr;
     float *ones = nullptr, *zeros = nullptr;   // ones [H]; zeros [max(3H, 2I)]: beta / bias of the bias-free ModernBERT
-    float *rope[2] = {nullptr, nullptr};       // ModernBERT RoPE tables [max_pos, 64] (full, sliding layers)
+    float *rope[2] = {nullptr, nullptr};       // RoPE tables [max_pos, 64]: ModernBERT (full, sliding layers), rotary (full)
     float *rel_bias = nullptr;                 // MPNet relative position bias [heads, 2 AC_ENCODER_MAX_S - 1]; NULL otherwise
     // DeBERTa c2p / p2c operand boxes [layers, ATTS_POS_DELTAS, heads, 2 (c2p, p2c), 256, 64] fp16 (pos_gather_kernel) and
     // their 128-row-box map; NULL otherwise
@@ -1603,13 +1615,17 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
                        (cfg->layers == 1 || w->attn_norm_w)),
                "ac_encoder_create: ModernBERT needs %d <= max_pos <= %d (max_pos=%d), layer_sliding, sliding_window > 0, both "
                "RoPE tables, wqkv, wi, final_norm_w and attn_norm_w", AC_ENCODER_MAX_S, AC_MODERNBERT_MAX_S, cfg->max_pos);
+    const bool rot = cfg->arch == AC_ARCH_ROTARY;
+    AC_REQUIRE(!rot || (cfg->rope_full && cfg->max_pos >= AC_ENCODER_MAX_S && cfg->max_pos <= AC_MODERNBERT_MAX_S),
+               "ac_encoder_create: AC_ARCH_ROTARY needs rope_full and %d <= max_pos <= %d (max_pos=%d)", AC_ENCODER_MAX_S,
+               AC_MODERNBERT_MAX_S, cfg->max_pos);
     AC_REQUIRE(cfg->precision == AC_PREC_F16, "ac_encoder_create: only AC_PREC_F16 (fp16 operands, fp32 accumulate) is implemented");
     AC_REQUIRE(cfg->hidden % 128 == 0 && cfg->hidden <= 1024, "ac_encoder_create: hidden=%d must be a multiple of 128, <= 1024", cfg->hidden);
-    // the attention kernels take head_dim 64 or 32; ModernBERT's RoPE epilogue pairs (d, d + 32) inside a 64-column head
+    // the attention kernels take head_dim 64 or 32; the RoPE epilogue pairs (d, d + 32) inside a 64-column head
     AC_REQUIRE(cfg->heads > 0 && cfg->hidden % cfg->heads == 0 &&
-                   (cfg->hidden / cfg->heads == 64 || (!mb && cfg->hidden / cfg->heads == 32)),
-               "ac_encoder_create: head_dim must be %s (hidden=%d heads=%d)", mb ? "64 for ModernBERT" : "64 or 32", cfg->hidden,
-               cfg->heads);
+                   (cfg->hidden / cfg->heads == 64 || (!mb && !rot && cfg->hidden / cfg->heads == 32)),
+               "ac_encoder_create: head_dim must be %s (hidden=%d heads=%d)",
+               mb ? "64 for ModernBERT" : rot ? "64 for AC_ARCH_ROTARY" : "64 or 32", cfg->hidden, cfg->heads);
     const bool mp = cfg->arch == AC_ARCH_MPNET;
     AC_REQUIRE(!mp || (cfg->rel_bias && cfg->hidden == 64 * cfg->heads),
                "ac_encoder_create: MPNet needs rel_bias and head_dim 64 (hidden=%d heads=%d)", cfg->hidden, cfg->heads);
@@ -1619,8 +1635,11 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
                "ac_encoder_create: DeBERTa needs pos_key, pos_query, rel_index, pos_span > 0 (pos_span=%d) and head_dim 64 "
                "(hidden=%d heads=%d)", cfg->pos_span, cfg->hidden, cfg->heads);
     AC_REQUIRE(cfg->intermediate % 64 == 0 && cfg->layers > 0 && cfg->max_tokens > 0, "ac_encoder_create: bad dims");
-    AC_REQUIRE(cfg->ffn_act == AC_FFN_GELU_ERF || cfg->ffn_act == AC_FFN_GELU_TANH, "ac_encoder_create: unknown ffn_act=%d",
-               cfg->ffn_act);
+    AC_REQUIRE(cfg->ffn_act == AC_FFN_GELU_ERF || cfg->ffn_act == AC_FFN_GELU_TANH || cfg->ffn_act == AC_FFN_SWIGLU,
+               "ac_encoder_create: unknown ffn_act=%d", cfg->ffn_act);
+    const bool swiglu = cfg->ffn_act == AC_FFN_SWIGLU;
+    AC_REQUIRE(!swiglu || rot, "ac_encoder_create: ffn_act=%d (AC_FFN_SWIGLU) is implemented for AC_ARCH_ROTARY only (arch=%d)",
+               cfg->ffn_act, cfg->arch);
     const int E = cfg->embedding_size ? cfg->embedding_size : cfg->hidden;
     AC_REQUIRE(!mb || cfg->ffn_act == AC_FFN_GELU_ERF, "ac_encoder_create: ModernBERT takes no ffn_act=%d (its FFN is GeGLU)",
                cfg->ffn_act);
@@ -1638,6 +1657,7 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     e->cfg = *cfg;
     e->cfg.embedding_size = E;        // 0 resolved to hidden: forward_layers reads the width from here
     const int H = cfg->hidden, I = cfg->intermediate, L = cfg->layers;
+    const int n1 = (mb || swiglu) ? 2 * I : I;   // rows of the first FFN weight (GLU: activated rows + multiplier rows)
     const size_t T = static_cast<size_t>((cfg->max_tokens + 127) / 128 * 128);
     e->T = T;
 #define TRY(x) do { rc = (x); if (rc) { ac_encoder_destroy(e); return rc; } } while (0)
@@ -1680,7 +1700,13 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
         }
     } else {
         TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * E));
-        TRY(pack_f32(e, &e->pos, w->pos_emb, static_cast<size_t>(cfg->max_pos) * E));
+        if (rot) {
+            // no position table: RoPE on q and k (table rope[0]); the embedding kernel reads one zero row (forward_layers)
+            e->pos = e->zeros;
+            TRY(pack_f32(e, &e->rope[0], cfg->rope_full, static_cast<size_t>(cfg->max_pos) * 64));
+        } else {
+            TRY(pack_f32(e, &e->pos, w->pos_emb, static_cast<size_t>(cfg->max_pos) * E));
+        }
         TRY(pack_f32(e, &e->type, w->type_emb, static_cast<size_t>(cfg->type_vocab) * E));
         TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, E));
         TRY(pack_f32(e, &e->emb_ln_b, w->emb_ln_b, E));
@@ -1743,15 +1769,20 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
             if (const int j = earlier(l, ffn1_src); j >= 0) {
                 ly.w1 = e->layers[j].w1, ly.c1f = e->layers[j].c1f, ly.c0f = e->layers[j].c0f;
             } else {
-                TRY(pack_consumer(e, 1, &w->ff1_w[l], &w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], I, H, 0, &ly.w1, &ly.c1f,
-                                  &ly.c0f));
+                TRY(pack_consumer(e, 1, &w->ff1_w[l], &w->ff1_b[l], w->ao_ln_w[l], w->ao_ln_b[l], n1, H, swiglu, &ly.w1,
+                                  &ly.c1f, &ly.c0f));
             }
             TRY(copy_of(&Layer::w2, w->ff2_w, l, HI));
             TRY(copy_of(&Layer::b2, w->ff2_b, l, H));
             TRY(copy_of(&Layer::ln_out_w, w->out_ln_w, l, H));
             TRY(copy_of(&Layer::ln_out_b, w->out_ln_b, l, H));
         }
-        if (cfg->cls_only) {
+        if (cfg->cls_only && swiglu) {
+            // plain interleaved FFN1 of the last layer and its interleaved bias (c0 with no LayerNorm folded in)
+            float *c1;
+            TRY(pack_consumer(e, 1, &w->ff1_w[L - 1], &w->ff1_b[L - 1], nullptr, nullptr, n1, H, 1, &e->w1_last, &c1,
+                              &e->b1_last));
+        } else if (cfg->cls_only) {
             TRY(pack_f16(e, &e->w1_last, w->ff1_w[L - 1], HI));
             TRY(pack_f32(e, &e->b1_last, w->ff1_b[L - 1], I));
         }
@@ -1798,7 +1829,6 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
         TRY(make_tmap_2d(&e->m_emb, e->ctx, 2, T, E, static_cast<uint64_t>(E) * 2, GEMM_BLOCK_M, 64));
         TRY(make_tmap_2d(&e->m_emb_proj, e->emb_proj_w, 2, H, E, static_cast<uint64_t>(E) * 2, GEMM_BLOCK_N, 64));
     }
-    const int n1 = mb ? 2 * I : I;    // rows of the first FFN weight (ModernBERT: GeGLU input + gate)
     for (Layer &ly : e->layers) {
         TRY(make_tmap_2d(&ly.m_wqkv, ly.wqkv, 2, 3 * H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
         TRY(make_tmap_2d(&ly.m_wo, ly.wo, 2, H, H, static_cast<uint64_t>(H) * 2, GEMM_BLOCK_N, 64));
@@ -1826,16 +1856,20 @@ static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, in
 // deferred; the residual epilogues add LN_pending(y), carried as (row statistics, gamma, beta).  That pending LayerNorm is
 // the one decision the block kinds differ in: post-LN blocks leave LN1 / LN2 pending, pre-LN blocks keep the identity
 // (stats (0, 1), gamma 1, beta 0) pending throughout.  The rest is the epilogue type (RoPE, GeGLU) and data in e->layers.
-// FFN_ACT: GeGLU (pre-LN), or the post-LN encoder's GELU (ac_encoder_config.ffn_act: exact erf or tanh).
-template <bool PRE_LN, Act FFN_ACT>
+// ROPE: q and k rotated in the QKV epilogue (ModernBERT; post-LN AC_ARCH_ROTARY, which has no position table).
+// FFN_ACT: GeGLU (pre-LN), or the post-LN encoder's (ac_encoder_config.ffn_act: exact-erf or tanh GELU, SwiGLU).
+template <bool PRE_LN, bool ROPE, Act FFN_ACT>
 static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids, int B, int S,
                           float *out_unit_cls, cudaStream_t s) {
-    static_assert(PRE_LN == (FFN_ACT == Act::GeGLU), "GeGLU is the pre-LN block's FFN");
+    static_assert(PRE_LN == (FFN_ACT == Act::GeGLU) && (!PRE_LN || ROPE), "the pre-LN block is ModernBERT's: RoPE, GeGLU");
+    constexpr bool GLU = FFN_ACT == Act::GeGLU || FFN_ACT == Act::SwiGLU;
     using EpiFfn1 = EpiF16<FFN_ACT, true>;
     using EpiFfn1Rows = EpiF16<FFN_ACT, false>;                     // on materialised LayerNorm rows (CLS-only tail)
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden, I = c.intermediate, M = B * S;
-    const int N1 = PRE_LN ? 2 * I : I;                              // FFN1 accumulator columns (GeGLU: input + gate)
+    const int N1 = GLU ? 2 * I : I;                                 // FFN1 accumulator columns (GLU: activated + multiplier)
+    // a post-LN RoPE encoder's e->pos is one zero row: the embedding kernel's clamp to max_pos - 1 = 0 reads it
+    const int emb_pos = (ROPE && !PRE_LN) ? 1 : c.max_pos;
     const int S_pad = (S + 7) / 8 * 8;
     const int wpb = 8;
     const int row_blocks = (M + wpb - 1) / wpb;
@@ -1846,7 +1880,7 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
     if (!e->emb_proj_w) {
         embed_ln_kernel<true><<<row_blocks, wpb * 32, 0, s>>>(ids, PRE_LN ? nullptr : type_ids, e->word, e->pos, e->type,
                                                               e->emb_ln_w, e->emb_ln_b, c.ln_eps, B, S, H, c.arch, c.pad_idx,
-                                                              c.vocab, c.max_pos, c.type_vocab, e->x, e->xh);
+                                                              c.vocab, emb_pos, c.type_vocab, e->x, e->xh);
         AC_LAUNCH_CHECK();
     } else {
         // factorized embeddings: LayerNorm at width E into the ctx scratch (fp16), then y = LN(emb) Wp^T + bp at width H
@@ -1863,7 +1897,7 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
     const float *pg = e->ones, *pb = e->zeros;
     for (int l = 0; l < c.layers; ++l) {
         const Layer &ly = e->layers[l];
-        EpiQKV<PRE_LN> eq{.qk = {.bias = ly.c0qkv, .c1 = ly.c1qkv, .row_stats = st_qkv, .Y = e->qk, .M = M, .N = 3 * H,
+        EpiQKV<ROPE> eq{.qk = {.bias = ly.c0qkv, .c1 = ly.c1qkv, .row_stats = st_qkv, .Y = e->qk, .M = M, .N = 3 * H,
                                  .ldy = 2 * H, .S = S, .rope = e->rope[ly.window ? 1 : 0]},
                           .vT = e->vT, .vt_col0 = 2 * H, .S_pad = S_pad, .H = H};
         if ((rc = launch_linear(e->m_xh, ly.m_wqkv, M, 3 * H, H, eq, s))) return rc;
@@ -1932,6 +1966,9 @@ static int check_shape_map_vt(ac_encoder *e, const char *who, int B, int S) {
         // RoPE has no position table: any S up to the encoder's max_pos (<= AC_MODERNBERT_MAX_S) runs
         AC_REQUIRE(S <= e->cfg.max_pos, "%s: S=%d exceeds this ModernBERT encoder's max_pos=%d (max_position_embeddings)", who,
                    S, e->cfg.max_pos);
+    } else if (e->cfg.arch == AC_ARCH_ROTARY) {
+        AC_REQUIRE(S <= e->cfg.max_pos, "%s: S=%d exceeds this rotary encoder's max_pos=%d (min(max_position_embeddings, %d))",
+                   who, S, e->cfg.max_pos, AC_MODERNBERT_MAX_S);
     } else if (S > AC_ENCODER_MAX_S) {
         // RoBERTa positions run from pad_idx + 1: a table with more rows than AC_ENCODER_MAX_S of them (XLM-R's 8194) takes
         // the sequences it has positions for, up to AC_MODERNBERT_MAX_S
@@ -1969,10 +2006,18 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
     int rc = check_shape_map_vt(e, "ac_encoder_forward_cls", B, S);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (e->cfg.arch == AC_ARCH_MODERNBERT) return forward_layers<true, Act::GeGLU>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    if (e->cfg.arch == AC_ARCH_MODERNBERT)
+        return forward_layers<true, true, Act::GeGLU>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    if (e->cfg.arch == AC_ARCH_ROTARY) {
+        if (e->cfg.ffn_act == AC_FFN_SWIGLU)
+            return forward_layers<false, true, Act::SwiGLU>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+        if (e->cfg.ffn_act == AC_FFN_GELU_TANH)
+            return forward_layers<false, true, Act::GeluTanh>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+        return forward_layers<false, true, Act::Gelu>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    }
     if (e->cfg.ffn_act == AC_FFN_GELU_TANH)
-        return forward_layers<false, Act::GeluTanh>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-    return forward_layers<false, Act::Gelu>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+        return forward_layers<false, false, Act::GeluTanh>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    return forward_layers<false, false, Act::Gelu>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
 }
 
 // parity entry: the attention stage alone, through the handle's own buffers, V^T view and launch_attention
@@ -2017,6 +2062,7 @@ static int linear_tc(const CUtensorMap &ta, const CUtensorMap &tb, const float *
             __half *Yh = static_cast<__half *>(Y);
             if (epi == 0) return run(EpiF16<Act::None, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
             if (epi == 3) return run(EpiF16<Act::GeluTanh, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
+            if (epi == 4) return run(EpiF16<Act::SwiGLU, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N / 2});
             return run(EpiF16<Act::Gelu, false>{.bias = bias, .Y = Yh, .M = M, .N = N, .ldy = N});
         }
     }
@@ -2030,10 +2076,12 @@ static int linear_tc(const CUtensorMap &ta, const CUtensorMap &tb, const float *
 extern "C" int ac_linear_tc(const void *X, const void *W, const float *bias, const float *residual, void *Y, int M, int N,
                             int K, int epi, int round_out, int precision, int out_half, ac_stream_t stream) {
     AC_REQUIRE(X && W && Y && bias && M > 0 && N > 0 && K > 0, "ac_linear_tc: bad arguments (bias is required)");
-    AC_REQUIRE(epi >= 0 && epi <= 3 && (epi != 2 || residual), "ac_linear_tc: bad epilogue");
+    AC_REQUIRE(epi >= 0 && epi <= 4 && (epi != 2 || residual), "ac_linear_tc: bad epilogue");
     AC_REQUIRE(precision == AC_PREC_TF32 || precision == AC_PREC_F16, "ac_linear_tc: bad precision");
     AC_REQUIRE(!(out_half && epi == 2), "ac_linear_tc: the residual epilogue writes fp32");
     AC_REQUIRE(epi != 3 || (out_half && precision == AC_PREC_F16), "ac_linear_tc: the tanh-GELU epilogue writes fp16");
+    AC_REQUIRE(epi != 4 || (out_half && precision == AC_PREC_F16 && N % 64 == 0),
+               "ac_linear_tc: the SwiGLU epilogue writes fp16 and takes N %% 64 == 0 (interleaved weight rows)");
     const int es = precision == AC_PREC_F16 ? 2 : 4;
     AC_REQUIRE((K * es) % 16 == 0 && N % 8 == 0, "ac_linear_tc: rows must be 16-byte multiples and N %% 8 == 0");
     int rc = ac_device_check();

@@ -102,6 +102,30 @@ def bge_m3(seed: int = 1234):
     return m, cfg
 
 
+def nomic_v15(seed: int = 1234):
+    """HF NomicBertModel(NomicBertConfig()) == nomic-ai/nomic-embed-text-v1 / v1.5 architecture (12 x 768, 12 heads, SwiGLU
+    I = 3072 without biases, no q/k/v/o biases, RoPE theta 1000, 2048 positions, vocab 30528), random init under
+    torch.manual_seed(seed).  Token ids: synthetic_ids(B, S, vocab=30528)."""
+    from transformers import NomicBertConfig, NomicBertModel
+    torch.manual_seed(seed)
+    cfg = NomicBertConfig()
+    m = NomicBertModel(cfg)
+    m.eval()
+    return m, cfg
+
+
+def jina_v3(seed: int = 1234):
+    """HF JinaEmbeddingsV3Model(JinaEmbeddingsV3Config()) == jinaai/jina-embeddings-v3 architecture (24 x 1024, 16 heads,
+    GELU I = 4096 with biases, RoPE theta 20000, 8194 positions of which 8192 are used, vocab 250002, one token type), random
+    init under torch.manual_seed(seed), without the pooler.  Token ids: xlmr_ids."""
+    from transformers import JinaEmbeddingsV3Config, JinaEmbeddingsV3Model
+    torch.manual_seed(seed)
+    cfg = JinaEmbeddingsV3Config()
+    m = JinaEmbeddingsV3Model(cfg, add_pooling_layer=False)
+    m.eval()
+    return m, cfg
+
+
 def xlmr_ids(B: int, S: int, seed: int = 7, vocab: int = 250002) -> torch.Tensor:
     """uniform in [5, vocab), <s>=0 first, </s>=2 last, never the pad id 1; int32 [B,S] on the host."""
     g = torch.Generator().manual_seed(seed)

@@ -242,12 +242,16 @@ int ac_head_train_strategic(const float *X, const int64_t *targets, const int64_
 
 /* ------------------------------------------------------------------------------------------
  * Stage E -- encoder.  Replaces `self.model(**inputs).last_hidden_state[:,0,:]` + F.normalize at
- *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel / ModernBertModel forward).
+ *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel / ModernBertModel / NomicBertModel /
+ *   JinaEmbeddingsV3Model forward).
  * ------------------------------------------------------------------------------------------ */
 enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2,
        AC_ARCH_MPNET = 3 /* post-LN BERT block, RoBERTa positions, relative position bias (rel_bias); head_dim 64 */,
        AC_ARCH_DEBERTA = 4 /* DeBERTa-v2/v3: post-LN BERT block, BERT positions, disentangled c2p + p2c attention
-                              (pos_key, pos_query, pos_span, rel_index); head_dim 64 */ };
+                              (pos_key, pos_query, pos_span, rel_index); head_dim 64 */,
+       AC_ARCH_ROTARY = 5 /* NomicBERT, jina-embeddings-v3: post-LN BERT block, RoPE on q and k (rope_full, positions
+                             0..S-1 for every sequence, padded or not), embeddings LayerNorm(word + type) with no position
+                             table (pos_emb is not read); head_dim 64, no embedding projection */ };
 #define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts for BERT / RoBERTa / DistilBERT (their
                                   position tables stop at 512).  An AC_ARCH_ROBERTA encoder whose table has more than
                                   AC_ENCODER_MAX_S + pad_idx + 1 rows (XLM-R: bge-m3, arctic-embed-l-v2.0, 8194 rows) accepts
@@ -263,7 +267,8 @@ enum {
 typedef struct {
     int arch;            /* AC_ARCH_* */
     int layers, hidden, heads, intermediate;   /* hidden % 128 == 0; head_dim = hidden / heads is 64 or 32
-                                                  (64 only for AC_ARCH_MODERNBERT, AC_ARCH_MPNET and AC_ARCH_DEBERTA) */
+                                                  (64 only for AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERTA and
+                                                  AC_ARCH_ROTARY) */
     int vocab, max_pos, type_vocab;
     int pad_idx;         /* roberta, mpnet: position ids start at pad_idx+1 */
     float ln_eps;
@@ -271,13 +276,16 @@ typedef struct {
     int max_tokens;      /* workspace is sized for B*S <= max_tokens */
     int cls_only;        /* != 0: the last layer's output projection / FFN / LayerNorms run on the CLS rows only
                             (classifier.py:1272 uses nothing else); 0 keeps the full last hidden state */
-    /* AC_ARCH_MODERNBERT only (ignored otherwise).  AC_ENCODER_MAX_S <= max_pos <= AC_MODERNBERT_MAX_S: the longest
-       sequence the encoder accepts and the rows of both RoPE tables (RoPE has no position parameters). */
+    /* AC_ARCH_MODERNBERT only (ignored otherwise), except rope_full, which AC_ARCH_ROTARY reads too.  For both,
+       AC_ENCODER_MAX_S <= max_pos <= AC_MODERNBERT_MAX_S is the longest sequence the encoder accepts and the rows of its
+       RoPE tables (RoPE has no position parameters). */
     int sliding_window;          /* half-window w = local_attention / 2: a sliding layer's query i sees keys |i - j| <= w */
     const int32_t *layer_sliding;  /* HOST array [layers]: 1 = sliding_attention, 0 = full_attention (config.layer_types) */
-    const float *rope_full;      /* DEVICE [max_pos, 64] fp32 RoPE table of the full-attention layers:              */
+    const float *rope_full;      /* DEVICE [max_pos, 64] fp32 RoPE table of the full-attention layers (every layer of
+                                    AC_ARCH_ROTARY):                                                                   */
     const float *rope_sliding;   /*   row = position, [0, 32) cos, [32, 64) sin of the 32 frequencies (HF
-                                       ModernBertRotaryEmbedding's formula, built by the caller); the sliding layers' table */
+                                       ModernBertRotaryEmbedding's formula = LlamaRotaryEmbedding's, default rope type,
+                                       built by the caller); the sliding layers' table */
     /* AC_ARCH_MPNET only (ignored otherwise), copied by ac_encoder_create.  DEVICE [heads, 2 AC_ENCODER_MAX_S - 1] fp32:
        entry (h, AC_ENCODER_MAX_S - 1 + key - query) is the bias every layer adds to head h's scaled score of (query, key)
        (HF MPNetEncoder.compute_position_bias: relative_attention_bias.weight[bucket(key - query), h], built by the caller) */
@@ -295,12 +303,15 @@ typedef struct {
     /* factorized embeddings (ALBERT, ELECTRA): width E of the embedding tables and their LayerNorm; 0 means hidden.  An E
        other than hidden needs the projection ac_encoder_weights.emb_proj_w; with a projection E % 128 == 0, E <= hidden. */
     int embedding_size;
-    int ffn_act;                 /* AC_FFN_*: the FFN activation of a post-LN encoder; AC_ARCH_MODERNBERT (GeGLU) takes 0 */
+    int ffn_act;                 /* AC_FFN_*: the FFN activation of a post-LN encoder; AC_ARCH_MODERNBERT (GeGLU) takes 0,
+                                    AC_FFN_SWIGLU is AC_ARCH_ROTARY's only */
 } ac_encoder_config;
 
 enum {
     AC_FFN_GELU_ERF = 0,         /* exact-erf GELU (HF "gelu") */
-    AC_FFN_GELU_TANH = 1         /* tanh-approximated GELU (HF "gelu_new", "gelu_pytorch_tanh"; ALBERT v2) */
+    AC_FFN_GELU_TANH = 1,        /* tanh-approximated GELU (HF "gelu_new", "gelu_pytorch_tanh"; ALBERT v2) */
+    AC_FFN_SWIGLU = 2            /* down(silu(gate_proj x) * up_proj x) (NomicBERT): ff1_w[l] is [2I, H], the activated rows
+                                    (gate_proj) then the multiplier rows (up_proj); ff1_b[l] is [2I] */
 };
 
 /* device pointers to the HF state_dict tensors (fp32, HF layout [out,in]).
@@ -309,6 +320,9 @@ enum {
  *   ao_w       layers.l.attn.Wo               ao_ln_w   layers.l.mlp_norm
  *   ff2_w      layers.l.mlp.Wo
  * and the fields after out_ln_b; every other pointer may be NULL.
+ * AC_ARCH_ROTARY takes the BERT fields but pos_emb, every bias present (pass zeros where the checkpoint has none): q/k/v/ao
+ * self_attn.{q,k,v,o}_proj, ao_ln post_attention_layernorm, ff1 mlp.fc1 or (AC_FFN_SWIGLU) cat(mlp.gate_proj, mlp.up_proj),
+ * ff2 mlp.fc2 / mlp.down_proj, out_ln post_mlp_layernorm.
  * Shared layers (ALBERT's cross-layer parameter sharing): a packed operand whose source pointers -- weights, biases and the
  * LayerNorm folded into it -- equal an earlier layer's reuses that layer's packed copy, so pass the same pointer for every
  * layer that shares a tensor.  Sharing is by pointer identity only: equal values at different addresses are packed twice. */
@@ -341,7 +355,7 @@ int ac_encoder_destroy(ac_encoder *enc);
 
 /* ids[B,S] int32 token ids, mask[B,S] int32 (1 keep / 0 pad; NULL = all ones), type_ids nullable (ignored by
  * AC_ARCH_MODERNBERT, whose RoPE positions are 0..S-1 for every sequence, padded or not).  S <= AC_ENCODER_MAX_S, or
- * S <= max_pos for AC_ARCH_MODERNBERT, or, for an AC_ARCH_ROBERTA encoder with max_pos > AC_ENCODER_MAX_S + pad_idx + 1,
+ * S <= max_pos for AC_ARCH_MODERNBERT and AC_ARCH_ROTARY, or, for an AC_ARCH_ROBERTA encoder with max_pos > AC_ENCODER_MAX_S + pad_idx + 1,
  * S <= min(AC_MODERNBERT_MAX_S, max_pos - pad_idx - 1) (its positions run from pad_idx + 1; head_dim 64 past
  * AC_ENCODER_MAX_S).
  * out_unit_cls[B,H] = L2-normalised (eps 1e-12) CLS row of the last hidden state. */
@@ -366,7 +380,9 @@ int ac_encoder_attention(ac_encoder *enc, const void *qk, const void *vT, const 
 
 /* generic tensor-core linear (the encoder's GEMM with its fused epilogues), exposed for parity tests and roofline
  * measurement: Y[M,N] = epi(X[M,K] W[N,K]^T + bias) (+ residual).  epi: 0 bias, 1 bias+GELU(erf), 2 bias+fp32 residual,
- * 3 bias+GELU(tanh) (AC_PREC_F16 with out_half != 0 only).
+ * 3 bias+GELU(tanh) (AC_PREC_F16 with out_half != 0 only), 4 SwiGLU (AC_PREC_F16 with out_half != 0, N % 64 == 0): W's
+ * rows interleaved in 32-row groups (rows 64 g .. + 31 activated, 64 g + 32 .. + 63 their multipliers), Y [M, N / 2] with
+ * Y[m, 32 g + j] = silu(p[m, 64 g + j]) * p[m, 64 g + 32 + j], p = X W^T + bias.
  * precision AC_PREC_TF32: X, W, Y fp32 (operands used as stored; round_out != 0 rounds Y to tf32);
  * precision AC_PREC_F16 : X, W fp16, Y fp32 or (out_half != 0, epi != 2) fp16. */
 int ac_linear_tc(const void *X, const void *W, const float *bias, const float *residual, void *Y,
