@@ -27,6 +27,7 @@ AC_LOSS_CE, AC_LOSS_BCE, AC_LOSS_CE_STRATEGIC = 0, 1, 2
 AC_COST_LINEAR, AC_COST_SEPARABLE = 0, 1
 AC_STRATEGIC_CANDIDATES = 50
 AC_ARCH_BERT, AC_ARCH_ROBERTA, AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERTA, AC_ARCH_ROTARY = 0, 1, 2, 3, 4, 5
+AC_ARCH_EUROBERT = 6
 AC_ENCODER_MAX_S = 512
 AC_MODERNBERT_MAX_S = 8192
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
@@ -925,6 +926,65 @@ def jina_v3_to_bert_state_dict(sd: dict, c):
     return _rotary_to_bert_state_dict(sd, c, ffn, FFN_ACTS[c.hidden_act])
 
 
+def eurobert_settings(c) -> dict:
+    """Encoder dims of a EuroBertConfig; raises AdaptiveB200Error naming any setting the CUDA path does not implement (checked
+    before any device call).  The sequence limit and the RoPE table's rows are max(512, min(max_position_embeddings,
+    AC_MODERNBERT_MAX_S))."""
+    rp = getattr(c, "rope_parameters", None) or {}
+    if rp.get("rope_type", "default") != "default":
+        raise AdaptiveB200Error(f"EuroBERT rope_type={rp.get('rope_type')!r} is not implemented in the CUDA path (only "
+                                "'default' RoPE; llama3, YaRN, dynamic NTK and linear scaling change the table)")
+    for flag in ("attention_bias", "mlp_bias"):
+        if getattr(c, flag, False):
+            raise AdaptiveB200Error(f"EuroBERT {flag}=True is not implemented in the CUDA path (the published checkpoints "
+                                    "have no biases)")
+    H, heads = c.hidden_size, c.num_attention_heads
+    if H % 128 != 0 or H > 1024:
+        raise AdaptiveB200Error(f"EuroBERT hidden_size={H} is not implemented in the CUDA path: the encoder takes hidden "
+                                "<= 1024 in multiples of 128")
+    head_dim = getattr(c, "head_dim", None) or (H // heads if heads > 0 else 0)
+    if heads <= 0 or head_dim != 64 or H != 64 * heads:
+        raise AdaptiveB200Error(f"EuroBERT head_dim={head_dim} (hidden={H}, heads={heads}) is not implemented in the CUDA "
+                                "path: only head_dim 64")
+    if c.hidden_act not in ("silu", "swish"):
+        raise AdaptiveB200Error(f"EuroBERT hidden_act={c.hidden_act!r} is not implemented in the CUDA path (only 'silu', "
+                                "'swish')")
+    kv = c.num_key_value_heads if c.num_key_value_heads is not None else heads
+    if kv <= 0 or heads % kv != 0:
+        raise AdaptiveB200Error(f"EuroBERT num_key_value_heads={kv} does not divide num_attention_heads={heads}")
+    return dict(layers=c.num_hidden_layers, hidden=H, heads=heads, intermediate=c.intermediate_size, vocab=c.vocab_size,
+                max_pos=max(AC_ENCODER_MAX_S, min(int(c.max_position_embeddings), AC_MODERNBERT_MAX_S)),
+                ln_eps=c.rms_norm_eps, pad_idx=(c.pad_token_id if c.pad_token_id is not None else 0),
+                rope_theta=float(rp.get("rope_theta", 10000.0)))
+
+
+def eurobert_to_modernbert_names(sd: dict, c):
+    """EuroBertModel's parameters under the ModernBERT names the "eurobert" Encoder reads (include/adaptive_b200.h,
+    AC_ARCH_EUROBERT): input_layernorm -> attn_norm (layer 0's too), post_attention_layernorm -> mlp_norm, o_proj -> attn.Wo,
+    cat(q, k, v) -> attn.Wqkv, cat(gate_proj, up_proj) -> mlp.Wi, down_proj -> mlp.Wo, norm -> final_norm.  Grouped-query
+    attention: k_proj / v_proj rows are expanded to every query head in HF repeat_kv's order (query head h reads kv head
+    h // (heads / num_key_value_heads)) before the concatenation, so no kernel sees kv heads.  Returns the names and the
+    Encoder dims (eurobert_settings)."""
+    dims = eurobert_settings(c)
+    heads, L = dims["heads"], dims["layers"]
+    kv = c.num_key_value_heads if c.num_key_value_heads is not None else heads
+
+    def expand(w):            # [kv 64, H] -> [heads 64, H]
+        return w.view(kv, 1, 64, -1).expand(kv, heads // kv, 64, w.shape[-1]).reshape(heads * 64, -1)
+
+    out = {"embeddings.tok_embeddings.weight": sd["embed_tokens.weight"], "final_norm.weight": sd["norm.weight"]}
+    for l in range(L):
+        p = f"layers.{l}."
+        out[p + "attn_norm.weight"] = sd[p + "input_layernorm.weight"]
+        out[p + "mlp_norm.weight"] = sd[p + "post_attention_layernorm.weight"]
+        out[p + "attn.Wqkv.weight"] = torch.cat([sd[p + "self_attn.q_proj.weight"], expand(sd[p + "self_attn.k_proj.weight"]),
+                                                 expand(sd[p + "self_attn.v_proj.weight"])])
+        out[p + "attn.Wo.weight"] = sd[p + "self_attn.o_proj.weight"]
+        out[p + "mlp.Wi.weight"] = torch.cat([sd[p + "mlp.gate_proj.weight"], sd[p + "mlp.up_proj.weight"]])
+        out[p + "mlp.Wo.weight"] = sd[p + "mlp.down_proj.weight"]
+    return out, dims
+
+
 class Encoder:
     """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors).  arch "mpnet"
     takes the BERT names (mpnet_to_bert_state_dict) and rel_bias, the [heads, 2 AC_ENCODER_MAX_S - 1] table of
@@ -932,7 +992,8 @@ class Encoder:
     deberta_to_bert_state_dict.  embedding_size (0 = hidden) and the "embeddings_project.*" tensors give factorized
     embeddings (albert_to_bert_state_dict, electra_to_bert_state_dict); ffn_act is AC_FFN_GELU_ERF or AC_FFN_GELU_TANH.
     arch "rotary" takes the BERT names without a position table, RoPE with base rope_theta on q and k, and ffn_act
-    AC_FFN_SWIGLU too (nomic_bert_to_bert_state_dict, jina_v3_to_bert_state_dict).
+    AC_FFN_SWIGLU too (nomic_bert_to_bert_state_dict, jina_v3_to_bert_state_dict).  arch "eurobert" takes the ModernBERT
+    names of eurobert_to_modernbert_names (RMSNorms, layer 0's attn_norm used, no embedding norm) and one rope_theta.
     Names that refer to the same source tensor (ALBERT's shared layers) are copied and packed once."""
 
     def __init__(self, sd: dict, *, arch: str, layers: int, hidden: int, heads: int, intermediate: int, vocab: int,
@@ -965,22 +1026,27 @@ class Encoder:
             return ctypes.cast(a, _PP)
 
         w = EncoderWeights()
-        if arch == "modernbert":
+        if arch in ("modernbert", "eurobert"):
             # HF ModernBertModel names; mlp_norm travels in ao_ln_w, attn.Wo in ao_w, mlp.Wo in ff2_w (include/adaptive_b200.h)
+            eb = arch == "eurobert"
             w.word_emb = g("embeddings.tok_embeddings.weight")
-            w.emb_ln_w = g("embeddings.norm.weight")
+            if not eb:                          # EuroBERT has no embedding norm
+                w.emb_ln_w = g("embeddings.norm.weight")
             w.final_norm_w = g("final_norm.weight")
             p = "layers.{}."
             w.ao_w, w.ao_ln_w, w.ff2_w = arr(p + "attn.Wo.weight"), arr(p + "mlp_norm.weight"), arr(p + "mlp.Wo.weight")
             w.wqkv, w.wi = arr(p + "attn.Wqkv.weight"), arr(p + "mlp.Wi.weight")
-            an = (c_void_p * layers)(None, *[g(f"layers.{l}.attn_norm.weight") for l in range(1, layers)])  # layer 0: Identity
-            ls = (ctypes.c_int32 * layers)(*layer_sliding)
-            rope = [modernbert_rope_table(t, max_pos).to(dev) for t in rope_theta]
+            # ModernBERT's layer-0 attn_norm is Identity; EuroBERT's input_layernorm of layer 0 is a real RMSNorm
+            an = (c_void_p * layers)(*[g(f"layers.{l}.attn_norm.weight") if (l or eb) else None for l in range(layers)])
+            ls = (ctypes.c_int32 * layers)(*(layer_sliding or [0] * layers))
+            rope = [modernbert_rope_table(t, max_pos).to(dev) for t in ((rope_theta,) if eb else rope_theta)]
             keep.update(an=an, ls=ls, rope=rope)
             w.attn_norm_w = ctypes.cast(an, _PP)
-            cfg = EncoderConfig(AC_ARCH_MODERNBERT, layers, hidden, heads, intermediate, vocab, max_pos, 1, pad_idx,
-                                ln_eps, AC_PREC_F16, max_tokens, 1 if cls_only else 0, sliding_window,
-                                ctypes.cast(ls, POINTER(ctypes.c_int32)), rope[0].data_ptr(), rope[1].data_ptr())
+            cfg = EncoderConfig(AC_ARCH_EUROBERT if eb else AC_ARCH_MODERNBERT, layers, hidden, heads, intermediate, vocab,
+                                max_pos, 1, pad_idx, ln_eps, AC_PREC_F16, max_tokens, 1 if cls_only else 0, sliding_window,
+                                ctypes.cast(ls, POINTER(ctypes.c_int32)), rope[0].data_ptr(), rope[-1].data_ptr())
+            if eb:
+                cfg.rope_sliding, cfg.ffn_act = None, AC_FFN_SWIGLU
         else:
             w.word_emb = g("embeddings.word_embeddings.weight")
             if arch != "rotary":
@@ -1027,8 +1093,10 @@ class Encoder:
     @classmethod
     def from_hf(cls, model, max_tokens: int = 65536, device="cuda", cls_only: bool = True):
         """Build from an in-memory HF BertModel / RobertaModel / DistilBertModel / MPNetModel / DebertaV2Model / AlbertModel /
-        ElectraModel / NomicBertModel / JinaEmbeddingsV3Model (post-LN blocks; the last two with RoPE, Nomic's FFN SwiGLU) or
-        ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers).  NomicBERT and jina-embeddings-v3 take sequences up
+        ElectraModel / NomicBertModel / JinaEmbeddingsV3Model (post-LN blocks; the last two with RoPE, Nomic's FFN SwiGLU),
+        ModernBertModel (pre-LN, RoPE, GeGLU, sliding-window layers) or EuroBertModel (pre-norm with RMSNorm, RoPE, SwiGLU,
+        grouped-query attention expanded to every head; sequences up to max(512, min(max_position_embeddings,
+        AC_MODERNBERT_MAX_S))).  NomicBERT and jina-embeddings-v3 take sequences up
         to max(512, min(max_position_embeddings, AC_MODERNBERT_MAX_S)), RoPE positions 0..S-1 whatever the padding; their
         remote-code modules (trust_remote_code=True), whose parameter names differ, are refused.  head_dim 64 or 32 for BERT / RoBERTa /
         DistilBERT, 64 for MPNet, DeBERTa and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
@@ -1062,6 +1130,14 @@ class Encoder:
         if mt == "electra":
             sd, dims = electra_to_bert_state_dict(dict(model.state_dict()), c)
             return cls(sd, arch="bert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
+        if mt == "eurobert":
+            from transformers import EuroBertModel
+            if not isinstance(model, EuroBertModel):
+                raise AdaptiveB200Error(f"model_type 'eurobert' from {type(model).__module__}.{type(model).__name__} is not the "
+                                        "native transformers EuroBertModel: remote-code modules (trust_remote_code=True) are "
+                                        "not implemented in the CUDA path; load the model without trust_remote_code")
+            sd, dims = eurobert_to_modernbert_names(dict(model.state_dict()), c)
+            return cls(sd, arch="eurobert", max_tokens=max_tokens, device=device, cls_only=cls_only, **dims)
         if mt in ("nomic_bert", "jina_embeddings_v3"):
             from transformers import JinaEmbeddingsV3Model, NomicBertModel
             native = NomicBertModel if mt == "nomic_bert" else JinaEmbeddingsV3Model

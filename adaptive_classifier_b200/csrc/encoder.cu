@@ -4,7 +4,7 @@
 // /root/reference/src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel.forward:
 // embeddings modeling_bert.py:53-113, self-attention :143-207, output+LN :287-298, FFN :330-356;
 // HF ModernBertModel.forward in models/modernbert/modeling_modernbert.py; NomicBertModel / JinaEmbeddingsV3Model, the
-// post-LN block with RoPE and, for Nomic, a SwiGLU FFN).  One layer loop (forward_layers) runs both block kinds; they
+// post-LN block with RoPE and, for Nomic, a SwiGLU FFN; EuroBertModel, ModernBERT's pre-norm block with RMSNorm and SwiGLU).  One layer loop (forward_layers) runs both block kinds; they
 // differ in the LayerNorm left pending on the residual path and in compile-time epilogue choices.
 //
 // Precision: every tensor-core operand is fp16 (RNE from fp32), accumulation fp32 (wgmma), residual stream, LayerNorm,
@@ -458,9 +458,16 @@ struct EpiEmbProj : EpiBase {
     }
 };
 
-// (sum, sumsq) partials of every GEMM_EPI_COLS-column part -> (mu, 1/sqrt(var + eps)) per row; parts are added in a fixed order.
+// The norm a block applies to its residual sums: LayerNorm (BERT family, ModernBERT) or RMSNorm (EuroBERT: weight * y /
+// sqrt(mean(y^2) + eps), no mean subtraction, no bias).  A deferred RMSNorm is the deferred LayerNorm with row statistics
+// (0, 1/sqrt(mean(y^2) + eps)) and beta 0, so every deferred-norm epilogue serves both.
+enum class Norm { Layer, Rms };
+
+// (sum, sumsq) partials of every GEMM_EPI_COLS-column part -> (mu, 1/sqrt(var + eps)) per row (RMS: (0, 1/sqrt(sumsq/H + eps)));
+// parts are added in a fixed order.
 // Kept as a kernel of its own: folding these loads + rsqrt into the consuming epilogues puts them at the head of every tile's
 // epilogue, which is the critical path of the HBM-bound residual GEMMs.
+template <Norm NORM>
 __global__ void ln_stats_kernel(const float2 *__restrict__ parts, int nparts, int64_t part_stride, int rows, int H, float eps,
                                 float2 *__restrict__ stats) {
     const int row = blockIdx.x * blockDim.x + threadIdx.x;
@@ -470,6 +477,10 @@ __global__ void ln_stats_kernel(const float2 *__restrict__ parts, int nparts, in
         const float2 v = parts[static_cast<int64_t>(p) * part_stride + row];
         s += v.x;
         q += v.y;
+    }
+    if constexpr (NORM == Norm::Rms) {
+        stats[row] = make_float2(0.f, 1.f / sqrtf(q / static_cast<float>(H) + eps));
+        return;
     }
     const float mu = s / static_cast<float>(H);
     const float var = fmaxf(q / static_cast<float>(H) - mu * mu, 0.f);
@@ -518,9 +529,34 @@ __global__ void pack_defer_kernel(const float *__restrict__ W, const float *__re
 // ------------------------------------------------------------------------------------------------
 constexpr int LN_MAXV = 8;
 
+// RMS: weight * (x / sqrt(mean(x^2) + eps)) (EuroBertRMSNorm, fp32); b is not read
+template <Norm NORM = Norm::Layer>
 __device__ __forceinline__ void ln_row(float4 (&x)[LN_MAXV], int nv, int H, const float *__restrict__ w,
                                        const float *__restrict__ b, float eps, int lane, float *out_full,
                                        __half *out_half) {
+    if constexpr (NORM == Norm::Rms) {
+        float q = 0.f;
+#pragma unroll
+        for (int i = 0; i < LN_MAXV; ++i)
+            if (i < nv) q += (x[i].x * x[i].x + x[i].y * x[i].y) + (x[i].z * x[i].z + x[i].w * x[i].w);
+        const float r = 1.f / sqrtf(warp_sum(q) / static_cast<float>(H) + eps);
+#pragma unroll
+        for (int i = 0; i < LN_MAXV; ++i)
+            if (i < nv) {
+                const int col = (lane + 32 * i) * 4;
+                const float4 w4 = __ldg(reinterpret_cast<const float4 *>(w + col));
+                const float4 o = make_float4(x[i].x * r * w4.x, x[i].y * r * w4.y, x[i].z * r * w4.z, x[i].w * r * w4.w);
+                if (out_full) *reinterpret_cast<float4 *>(out_full + col) = o;
+                if (out_half) {
+                    __half2 h0 = __floats2half2_rn(o.x, o.y), h1 = __floats2half2_rn(o.z, o.w);
+                    uint2 pk;
+                    pk.x = *reinterpret_cast<uint32_t *>(&h0);
+                    pk.y = *reinterpret_cast<uint32_t *>(&h1);
+                    *reinterpret_cast<uint2 *>(out_half + col) = pk;
+                }
+            }
+        return;
+    }
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < LN_MAXV; ++i)
@@ -557,6 +593,7 @@ __device__ __forceinline__ void ln_row(float4 (&x)[LN_MAXV], int nv, int H, cons
         }
 }
 
+template <Norm NORM>
 __global__ void layernorm_kernel(const float *__restrict__ in, const float *__restrict__ w, const float *__restrict__ b,
                                  float eps, int rows, int H, float *__restrict__ out_full, __half *__restrict__ out_half) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -568,8 +605,8 @@ __global__ void layernorm_kernel(const float *__restrict__ in, const float *__re
 #pragma unroll
     for (int i = 0; i < LN_MAXV; ++i)
         if (i < nv) x[i] = *reinterpret_cast<const float4 *>(src + (lane + 32 * i) * 4);
-    ln_row(x, nv, H, w, b, eps, lane, out_full ? out_full + static_cast<int64_t>(row) * H : nullptr,
-           out_half ? out_half + static_cast<int64_t>(row) * H : nullptr);
+    ln_row<NORM>(x, nv, H, w, b, eps, lane, out_full ? out_full + static_cast<int64_t>(row) * H : nullptr,
+                 out_half ? out_half + static_cast<int64_t>(row) * H : nullptr);
 }
 
 // modeling_bert.py:53-113 / modeling_roberta.py:146-159: (word + type) + position -> LayerNorm
@@ -577,13 +614,16 @@ __global__ void layernorm_kernel(const float *__restrict__ in, const float *__re
 // modeling_modernbert.py ModernBertEmbeddings: pos = type = NULL, LayerNorm(word) (b = zeros: norm_bias=False)
 // modeling_albert.py AlbertEmbeddings, modeling_electra.py ElectraEmbeddings: BERT's rule at width H = embedding_size;
 // F32_OUT = false writes the fp16 rows only (the A operand of the embedding projection, EpiEmbProj)
-template <bool F32_OUT>
+// RAW_RMS (modeling_eurobert.py EuroBertModel: embed_tokens(ids), no norm, no position table; pos = NULL): the raw word row
+// is the residual stream (out_full, out_half) and rms_stats[row] = (0, 1/sqrt(mean(x^2) + eps)) are the statistics of
+// layer 0's deferred input_layernorm; w, b are not read
+template <bool F32_OUT, bool RAW_RMS = false>
 __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *__restrict__ type_ids,
                                 const float *__restrict__ word, const float *__restrict__ pos,
                                 const float *__restrict__ type, const float *__restrict__ w,
                                 const float *__restrict__ b, float eps, int B, int S, int H, int arch, int pad_idx,
                                 int vocab, int max_pos, int type_vocab, float *__restrict__ out_full,
-                                __half *__restrict__ out_half) {
+                                __half *__restrict__ out_half, float2 *__restrict__ rms_stats = nullptr) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= B * S) return;
@@ -620,6 +660,24 @@ __global__ void embed_ln_kernel(const int32_t *__restrict__ ids, const int32_t *
             x[i].z = (a.z + t.z) + q.z;
             x[i].w = (a.w + t.w) + q.w;
         }
+    if constexpr (RAW_RMS) {
+        float q = 0.f;
+#pragma unroll
+        for (int i = 0; i < LN_MAXV; ++i)
+            if (i < nv) {
+                const int col = (lane + 32 * i) * 4;
+                *reinterpret_cast<float4 *>(out_full + static_cast<int64_t>(row) * H + col) = x[i];
+                const __half2 h0 = __floats2half2_rn(x[i].x, x[i].y), h1 = __floats2half2_rn(x[i].z, x[i].w);
+                uint2 pk;
+                pk.x = *reinterpret_cast<const uint32_t *>(&h0);
+                pk.y = *reinterpret_cast<const uint32_t *>(&h1);
+                *reinterpret_cast<uint2 *>(out_half + static_cast<int64_t>(row) * H + col) = pk;
+                q += (x[i].x * x[i].x + x[i].y * x[i].y) + (x[i].z * x[i].z + x[i].w * x[i].w);
+            }
+        q = warp_sum(q);
+        if (lane == 0) rms_stats[row] = make_float2(0.f, 1.f / sqrtf(q / static_cast<float>(H) + eps));
+        return;
+    }
     ln_row(x, nv, H, w, b, eps, lane, F32_OUT ? out_full + static_cast<int64_t>(row) * H : nullptr,
            out_half + static_cast<int64_t>(row) * H);
 }
@@ -1619,13 +1677,21 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     AC_REQUIRE(!rot || (cfg->rope_full && cfg->max_pos >= AC_ENCODER_MAX_S && cfg->max_pos <= AC_MODERNBERT_MAX_S),
                "ac_encoder_create: AC_ARCH_ROTARY needs rope_full and %d <= max_pos <= %d (max_pos=%d)", AC_ENCODER_MAX_S,
                AC_MODERNBERT_MAX_S, cfg->max_pos);
+    const bool eb = cfg->arch == AC_ARCH_EUROBERT;
+    AC_REQUIRE(!eb || (cfg->rope_full && cfg->max_pos >= AC_ENCODER_MAX_S && cfg->max_pos <= AC_MODERNBERT_MAX_S),
+               "ac_encoder_create: AC_ARCH_EUROBERT needs rope_full and %d <= max_pos <= %d (max_pos=%d)", AC_ENCODER_MAX_S,
+               AC_MODERNBERT_MAX_S, cfg->max_pos);
+    AC_REQUIRE(!eb || (w->wqkv && w->wi && w->attn_norm_w && w->final_norm_w),
+               "ac_encoder_create: AC_ARCH_EUROBERT needs wqkv, wi, attn_norm_w (every layer's, layer 0's included) and "
+               "final_norm_w");
     AC_REQUIRE(cfg->precision == AC_PREC_F16, "ac_encoder_create: only AC_PREC_F16 (fp16 operands, fp32 accumulate) is implemented");
     AC_REQUIRE(cfg->hidden % 128 == 0 && cfg->hidden <= 1024, "ac_encoder_create: hidden=%d must be a multiple of 128, <= 1024", cfg->hidden);
     // the attention kernels take head_dim 64 or 32; the RoPE epilogue pairs (d, d + 32) inside a 64-column head
     AC_REQUIRE(cfg->heads > 0 && cfg->hidden % cfg->heads == 0 &&
-                   (cfg->hidden / cfg->heads == 64 || (!mb && !rot && cfg->hidden / cfg->heads == 32)),
+                   (cfg->hidden / cfg->heads == 64 || (!mb && !rot && !eb && cfg->hidden / cfg->heads == 32)),
                "ac_encoder_create: head_dim must be %s (hidden=%d heads=%d)",
-               mb ? "64 for ModernBERT" : rot ? "64 for AC_ARCH_ROTARY" : "64 or 32", cfg->hidden, cfg->heads);
+               mb ? "64 for ModernBERT" : rot ? "64 for AC_ARCH_ROTARY" : eb ? "64 for AC_ARCH_EUROBERT" : "64 or 32",
+               cfg->hidden, cfg->heads);
     const bool mp = cfg->arch == AC_ARCH_MPNET;
     AC_REQUIRE(!mp || (cfg->rel_bias && cfg->hidden == 64 * cfg->heads),
                "ac_encoder_create: MPNet needs rel_bias and head_dim 64 (hidden=%d heads=%d)", cfg->hidden, cfg->heads);
@@ -1638,8 +1704,11 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     AC_REQUIRE(cfg->ffn_act == AC_FFN_GELU_ERF || cfg->ffn_act == AC_FFN_GELU_TANH || cfg->ffn_act == AC_FFN_SWIGLU,
                "ac_encoder_create: unknown ffn_act=%d", cfg->ffn_act);
     const bool swiglu = cfg->ffn_act == AC_FFN_SWIGLU;
-    AC_REQUIRE(!swiglu || rot, "ac_encoder_create: ffn_act=%d (AC_FFN_SWIGLU) is implemented for AC_ARCH_ROTARY only (arch=%d)",
+    AC_REQUIRE(!swiglu || rot || eb,
+               "ac_encoder_create: ffn_act=%d (AC_FFN_SWIGLU) is implemented for AC_ARCH_ROTARY / AC_ARCH_EUROBERT only (arch=%d)",
                cfg->ffn_act, cfg->arch);
+    AC_REQUIRE(!eb || swiglu, "ac_encoder_create: AC_ARCH_EUROBERT takes ffn_act=%d (AC_FFN_SWIGLU) only (ffn_act=%d)",
+               AC_FFN_SWIGLU, cfg->ffn_act);
     const int E = cfg->embedding_size ? cfg->embedding_size : cfg->hidden;
     AC_REQUIRE(!mb || cfg->ffn_act == AC_FFN_GELU_ERF, "ac_encoder_create: ModernBERT takes no ffn_act=%d (its FFN is GeGLU)",
                cfg->ffn_act);
@@ -1672,22 +1741,25 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
     TRY(dev_alloc(e, &e->zeros, nzeros));
     e->layers.resize(L);
     const size_t HH = static_cast<size_t>(H) * H, HI = static_cast<size_t>(H) * I;
-    if (mb) {
+    if (mb || eb) {
         // ModernBERT (modeling_modernbert.py): no biases or LayerNorm betas.  Wqkv consumes the sums pending attn_norm
-        // (Identity in layer 0), Wi the sums pending mlp_norm
+        // (Identity in layer 0), Wi the sums pending mlp_norm.
+        // EuroBERT (modeling_eurobert.py) the same pre-norm block with RMSNorms: no embedding norm, so layer 0's Wqkv
+        // consumes the raw embeddings pending input_layernorm (attn_norm_w[0]); full attention in every layer; Wi is
+        // cat(gate_proj, up_proj), the same interleaved row order for SwiGLU
         Layer &last = e->layers[L - 1];
         TRY(pack_f32(e, &e->word, w->word_emb, static_cast<size_t>(cfg->vocab) * H));
-        TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
+        if (mb) TRY(pack_f32(e, &e->emb_ln_w, w->emb_ln_w, H));
         TRY(pack_f32(e, &last.ln_out_w, w->final_norm_w, H));
         TRY(pack_f32(e, &e->rope[0], cfg->rope_full, static_cast<size_t>(cfg->max_pos) * 64));
-        TRY(pack_f32(e, &e->rope[1], cfg->rope_sliding, static_cast<size_t>(cfg->max_pos) * 64));
+        if (mb) TRY(pack_f32(e, &e->rope[1], cfg->rope_sliding, static_cast<size_t>(cfg->max_pos) * 64));
         e->emb_ln_b = e->b1_last = last.ln_out_b = e->zeros;
         for (int l = 0; l < L; ++l) {
             Layer &ly = e->layers[l];
-            ly.window = cfg->layer_sliding[l] ? cfg->sliding_window : 0;
+            ly.window = mb && cfg->layer_sliding[l] ? cfg->sliding_window : 0;
             ly.bo = ly.b2 = ly.ln_ffn_b = e->zeros;
-            TRY(pack_consumer(e, 1, &w->wqkv[l], nullptr, l ? w->attn_norm_w[l] : nullptr, nullptr, 3 * H, H, 0, &ly.wqkv,
-                              &ly.c1qkv, &ly.c0qkv));
+            TRY(pack_consumer(e, 1, &w->wqkv[l], nullptr, (l || eb) ? w->attn_norm_w[l] : nullptr, nullptr, 3 * H, H, 0,
+                              &ly.wqkv, &ly.c1qkv, &ly.c0qkv));
             TRY(pack_f16(e, &ly.wo, w->ao_w[l], HH));
             TRY(pack_f32(e, &ly.ln_ffn_w, w->ao_ln_w[l], H));
             TRY(pack_consumer(e, 1, &w->wi[l], nullptr, w->ao_ln_w[l], nullptr, 2 * I, H, 1, &ly.w1, &ly.c1f, &ly.c0f));
@@ -1849,19 +1921,25 @@ static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, in
 }
 
 // The layer stack, for post-LN (BERT / RoBERTa / DistilBERT, modeling_bert.py) or pre-LN (ModernBERT,
-// modeling_modernbert.py ModernBertModel.forward) blocks:
+// modeling_modernbert.py ModernBertModel.forward; EuroBERT, modeling_eurobert.py, with RMSNorm and SwiGLU) blocks:
 //     post-LN   y = LN1(y + attn(y))               y = LN2(y + GELU-FFN(y))               out = y
 //     pre-LN    y = y + attn(attn_norm(y))         y = y + GeGLU-FFN(mlp_norm(y))         out = final_norm(y)
 // e->x holds the un-normalised residual sums y, e->xh their fp16 copy.  QKV and FFN1 apply the LayerNorm they consume
 // deferred; the residual epilogues add LN_pending(y), carried as (row statistics, gamma, beta).  That pending LayerNorm is
 // the one decision the block kinds differ in: post-LN blocks leave LN1 / LN2 pending, pre-LN blocks keep the identity
 // (stats (0, 1), gamma 1, beta 0) pending throughout.  The rest is the epilogue type (RoPE, GeGLU) and data in e->layers.
-// ROPE: q and k rotated in the QKV epilogue (ModernBERT; post-LN AC_ARCH_ROTARY, which has no position table).
-// FFN_ACT: GeGLU (pre-LN), or the post-LN encoder's (ac_encoder_config.ffn_act: exact-erf or tanh GELU, SwiGLU).
-template <bool PRE_LN, bool ROPE, Act FFN_ACT>
+// ROPE: q and k rotated in the QKV epilogue (ModernBERT, EuroBERT; post-LN AC_ARCH_ROTARY, which has no position table).
+// FFN_ACT: GeGLU (ModernBERT), SwiGLU (EuroBERT), or the post-LN encoder's (ac_encoder_config.ffn_act: exact-erf or tanh
+// GELU, SwiGLU).
+// NORM: RMSNorm for EuroBERT's pre-norm block (input_layernorm, post_attention_layernorm, norm).  Its residual stream starts
+// as the raw embedding rows, so layer 0's QKV consumes them with their RMS statistics instead of the identity.
+template <bool PRE_LN, bool ROPE, Act FFN_ACT, Norm NORM>
 static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask, const int32_t *type_ids, int B, int S,
                           float *out_unit_cls, cudaStream_t s) {
-    static_assert(PRE_LN == (FFN_ACT == Act::GeGLU) && (!PRE_LN || ROPE), "the pre-LN block is ModernBERT's: RoPE, GeGLU");
+    static_assert(PRE_LN ? ROPE && FFN_ACT == (NORM == Norm::Layer ? Act::GeGLU : Act::SwiGLU)
+                         : NORM == Norm::Layer && FFN_ACT != Act::GeGLU,
+                  "pre-LN blocks are ModernBERT's (LayerNorm, RoPE, GeGLU) and EuroBERT's (RMSNorm, RoPE, SwiGLU); post-LN "
+                  "blocks use LayerNorm");
     constexpr bool GLU = FFN_ACT == Act::GeGLU || FFN_ACT == Act::SwiGLU;
     using EpiFfn1 = EpiF16<FFN_ACT, true>;
     using EpiFfn1Rows = EpiF16<FFN_ACT, false>;                     // on materialised LayerNorm rows (CLS-only tail)
@@ -1877,7 +1955,16 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
     const int64_t pstride = static_cast<int64_t>(e->T);
     const bool cls_tail = c.cls_only && static_cast<size_t>(B) <= e->Bc;
     int rc;
-    if (!e->emb_proj_w) {
+    // the embeddings arrive normalised (or projected): identity LayerNorm pending, and identity statistics for layer 0's QKV;
+    // EuroBERT's arrive raw, with the RMS statistics of layer 0's input_layernorm in stats_a
+    const float2 *pst = e->stats_id, *st_qkv = e->stats_id;
+    if constexpr (NORM == Norm::Rms) {
+        embed_ln_kernel<true, true><<<row_blocks, wpb * 32, 0, s>>>(ids, nullptr, e->word, nullptr, nullptr, nullptr, nullptr,
+                                                                    c.ln_eps, B, S, H, c.arch, c.pad_idx, c.vocab, c.max_pos,
+                                                                    c.type_vocab, e->x, e->xh, e->stats_a);
+        AC_LAUNCH_CHECK();
+        st_qkv = e->stats_a;
+    } else if (!e->emb_proj_w) {
         embed_ln_kernel<true><<<row_blocks, wpb * 32, 0, s>>>(ids, PRE_LN ? nullptr : type_ids, e->word, e->pos, e->type,
                                                               e->emb_ln_w, e->emb_ln_b, c.ln_eps, B, S, H, c.arch, c.pad_idx,
                                                               c.vocab, emb_pos, c.type_vocab, e->x, e->xh);
@@ -1892,8 +1979,6 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
         EpiEmbProj ep{.bias = e->emb_proj_b, .y = e->x, .yh = e->xh, .M = M, .N = H, .ld = H};
         if ((rc = launch_linear(e->m_emb, e->m_emb_proj, M, H, E, ep, s))) return rc;
     }
-    // the embeddings arrive normalised (or projected): identity LayerNorm pending, and identity statistics for layer 0's QKV
-    const float2 *pst = e->stats_id, *st_qkv = e->stats_id;
     const float *pg = e->ones, *pb = e->zeros;
     for (int l = 0; l < c.layers; ++l) {
         const Layer &ly = e->layers[l];
@@ -1907,7 +1992,7 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
         EpiResidDefer eo{.bias = ly.bo, .y = e->x, .yh = e->xh, .stats_prev = pst, .gamma = pg, .beta = pb, .parts = e->parts,
                          .part_stride = pstride, .M = M, .N = H, .ld = H};
         if ((rc = launch_linear(e->m_ctx, ly.m_wo, M, H, H, eo, s))) return rc;
-        ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
+        ln_stats_kernel<NORM><<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
         AC_LAUNCH_CHECK();
         EpiFfn1 e1{.bias = ly.c0f, .c1 = ly.c1f, .row_stats = e->stats_b, .Y = e->ffn, .M = M, .N = N1, .ldy = I};
         if ((rc = launch_linear(e->m_xh, ly.m_w1, M, N1, H, e1, s))) return rc;
@@ -1916,7 +2001,7 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
         EpiResidDefer e2{.bias = ly.b2, .y = e->x, .yh = e->xh, .stats_prev = pst, .gamma = pg, .beta = pb, .parts = e->parts,
                          .part_stride = pstride, .M = M, .N = H, .ld = H};
         if ((rc = launch_linear(e->m_ffn, ly.m_w2, M, H, I, e2, s))) return rc;
-        ln_stats_kernel<<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_a);
+        ln_stats_kernel<NORM><<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_a);
         AC_LAUNCH_CHECK();
         st_qkv = e->stats_a;
         if constexpr (!PRE_LN) { pst = e->stats_a; pg = ly.ln_out_w; pb = ly.ln_out_b; }
@@ -1935,19 +2020,19 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
         AC_LAUNCH_CHECK();
         EpiF32<false, true> eo{.bias = last.bo, .residual = e->x_cls, .Y = e->tmp_cls, .M = B, .N = H, .ldy = H};
         if ((rc = launch_linear(e->m_ctx_cls, last.m_wo, B, H, H, eo, s))) return rc;
-        layernorm_kernel<<<cb, wpb * 32, 0, s>>>(e->tmp_cls, last.ln_ffn_w, last.ln_ffn_b, c.ln_eps, B, H, PRE_LN ? nullptr : res,
+        layernorm_kernel<NORM><<<cb, wpb * 32, 0, s>>>(e->tmp_cls, last.ln_ffn_w, last.ln_ffn_b, c.ln_eps, B, H, PRE_LN ? nullptr : res,
                                                  e->xh_cls);
         AC_LAUNCH_CHECK();
         EpiFfn1Rows e1{.bias = e->b1_last, .Y = e->ffn_cls, .M = B, .N = N1, .ldy = I};
         if ((rc = launch_linear(e->m_xh_cls, e->p_w1_last, B, N1, H, e1, s))) return rc;
         EpiF32<false, true> e2{.bias = last.b2, .residual = res, .Y = sum, .M = B, .N = H, .ldy = H};
         if ((rc = launch_linear(e->m_ffn_cls, last.m_w2, B, H, I, e2, s))) return rc;
-        layernorm_kernel<<<cb, wpb * 32, 0, s>>>(sum, last.ln_out_w, last.ln_out_b, c.ln_eps, B, H, res, nullptr);
+        layernorm_kernel<NORM><<<cb, wpb * 32, 0, s>>>(sum, last.ln_out_w, last.ln_out_b, c.ln_eps, B, H, res, nullptr);
         AC_LAUNCH_CHECK();
         if ((rc = launch_cls_normalize(res, B, 1, H, out_unit_cls, s))) return rc;
     } else {
         // full hidden state requested (cls_only = 0, or B > Bc): materialise the output LayerNorm for every row
-        layernorm_kernel<<<row_blocks, wpb * 32, 0, s>>>(e->x, last.ln_out_w, last.ln_out_b, c.ln_eps, M, H, e->tmp, nullptr);
+        layernorm_kernel<NORM><<<row_blocks, wpb * 32, 0, s>>>(e->x, last.ln_out_w, last.ln_out_b, c.ln_eps, M, H, e->tmp, nullptr);
         AC_LAUNCH_CHECK();
         if ((rc = launch_cls_normalize(e->tmp, B, S, H, out_unit_cls, s))) return rc;
     }
@@ -1968,6 +2053,9 @@ static int check_shape_map_vt(ac_encoder *e, const char *who, int B, int S) {
                    S, e->cfg.max_pos);
     } else if (e->cfg.arch == AC_ARCH_ROTARY) {
         AC_REQUIRE(S <= e->cfg.max_pos, "%s: S=%d exceeds this rotary encoder's max_pos=%d (min(max_position_embeddings, %d))",
+                   who, S, e->cfg.max_pos, AC_MODERNBERT_MAX_S);
+    } else if (e->cfg.arch == AC_ARCH_EUROBERT) {
+        AC_REQUIRE(S <= e->cfg.max_pos, "%s: S=%d exceeds this EuroBERT encoder's max_pos=%d (min(max_position_embeddings, %d))",
                    who, S, e->cfg.max_pos, AC_MODERNBERT_MAX_S);
     } else if (S > AC_ENCODER_MAX_S) {
         // RoBERTa positions run from pad_idx + 1: a table with more rows than AC_ENCODER_MAX_S of them (XLM-R's 8194) takes
@@ -2006,18 +2094,21 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
     int rc = check_shape_map_vt(e, "ac_encoder_forward_cls", B, S);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    constexpr Norm LN = Norm::Layer;
     if (e->cfg.arch == AC_ARCH_MODERNBERT)
-        return forward_layers<true, true, Act::GeGLU>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+        return forward_layers<true, true, Act::GeGLU, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    if (e->cfg.arch == AC_ARCH_EUROBERT)
+        return forward_layers<true, true, Act::SwiGLU, Norm::Rms>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
     if (e->cfg.arch == AC_ARCH_ROTARY) {
         if (e->cfg.ffn_act == AC_FFN_SWIGLU)
-            return forward_layers<false, true, Act::SwiGLU>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+            return forward_layers<false, true, Act::SwiGLU, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
         if (e->cfg.ffn_act == AC_FFN_GELU_TANH)
-            return forward_layers<false, true, Act::GeluTanh>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-        return forward_layers<false, true, Act::Gelu>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+            return forward_layers<false, true, Act::GeluTanh, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+        return forward_layers<false, true, Act::Gelu, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
     }
     if (e->cfg.ffn_act == AC_FFN_GELU_TANH)
-        return forward_layers<false, false, Act::GeluTanh>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-    return forward_layers<false, false, Act::Gelu>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+        return forward_layers<false, false, Act::GeluTanh, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    return forward_layers<false, false, Act::Gelu, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
 }
 
 // parity entry: the attention stage alone, through the handle's own buffers, V^T view and launch_attention

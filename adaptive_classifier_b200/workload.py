@@ -126,6 +126,22 @@ def jina_v3(seed: int = 1234):
     return m, cfg
 
 
+def eurobert_210m(seed: int = 1234):
+    """EuroBERT/EuroBERT-210m architecture as HF EuroBertModel (12 x 768, 12 heads of 64 with as many kv heads, SwiGLU
+    I = 3072 without biases, RMSNorm eps 1e-5, RoPE theta 250000, 8192 positions, vocab 128256), random init under
+    torch.manual_seed(seed).  The hub config cannot be read offline: the dims are those of the EuroBERT paper
+    (arXiv:2503.05500) and the model card, and EuroBertConfig()'s defaults for the rest.  Token ids: synthetic_ids(B, S,
+    vocab=128256)."""
+    from transformers import EuroBertConfig, EuroBertModel
+    torch.manual_seed(seed)
+    cfg = EuroBertConfig(vocab_size=128256, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
+                         num_attention_heads=12, num_key_value_heads=12, max_position_embeddings=8192,
+                         rope_parameters={"rope_type": "default", "rope_theta": 250000.0})
+    m = EuroBertModel(cfg)
+    m.eval()
+    return m, cfg
+
+
 def xlmr_ids(B: int, S: int, seed: int = 7, vocab: int = 250002) -> torch.Tensor:
     """uniform in [5, vocab), <s>=0 first, </s>=2 last, never the pad id 1; int32 [B,S] on the host."""
     g = torch.Generator().manual_seed(seed)

@@ -243,7 +243,7 @@ int ac_head_train_strategic(const float *X, const int64_t *targets, const int64_
 /* ------------------------------------------------------------------------------------------
  * Stage E -- encoder.  Replaces `self.model(**inputs).last_hidden_state[:,0,:]` + F.normalize at
  *   src/adaptive_classifier/classifier.py:1271-1275 (HF BertModel / RobertaModel / ModernBertModel / NomicBertModel /
- *   JinaEmbeddingsV3Model forward).
+ *   JinaEmbeddingsV3Model / EuroBertModel forward).
  * ------------------------------------------------------------------------------------------ */
 enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2,
        AC_ARCH_MPNET = 3 /* post-LN BERT block, RoBERTa positions, relative position bias (rel_bias); head_dim 64 */,
@@ -251,7 +251,11 @@ enum { AC_ARCH_BERT = 0, AC_ARCH_ROBERTA = 1, AC_ARCH_MODERNBERT = 2,
                               (pos_key, pos_query, pos_span, rel_index); head_dim 64 */,
        AC_ARCH_ROTARY = 5 /* NomicBERT, jina-embeddings-v3: post-LN BERT block, RoPE on q and k (rope_full, positions
                              0..S-1 for every sequence, padded or not), embeddings LayerNorm(word + type) with no position
-                             table (pos_emb is not read); head_dim 64, no embedding projection */ };
+                             table (pos_emb is not read); head_dim 64, no embedding projection */,
+       AC_ARCH_EUROBERT = 6 /* EuroBERT: ModernBERT's pre-norm block with RMSNorm (ln_eps = rms_norm_eps), no embedding norm
+                               (the residual stream starts as the raw embed_tokens rows), RoPE on q and k (rope_full, positions
+                               0..S-1 for every sequence, padded or not), full attention in every layer, no biases,
+                               ffn_act = AC_FFN_SWIGLU; head_dim 64, no embedding projection.  Weights: see ac_encoder_weights */ };
 #define AC_ENCODER_MAX_S 512   /* longest sequence ac_encoder_forward_cls accepts for BERT / RoBERTa / DistilBERT (their
                                   position tables stop at 512).  An AC_ARCH_ROBERTA encoder whose table has more than
                                   AC_ENCODER_MAX_S + pad_idx + 1 rows (XLM-R: bge-m3, arctic-embed-l-v2.0, 8194 rows) accepts
@@ -267,8 +271,8 @@ enum {
 typedef struct {
     int arch;            /* AC_ARCH_* */
     int layers, hidden, heads, intermediate;   /* hidden % 128 == 0; head_dim = hidden / heads is 64 or 32
-                                                  (64 only for AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERTA and
-                                                  AC_ARCH_ROTARY) */
+                                                  (64 only for AC_ARCH_MODERNBERT, AC_ARCH_MPNET, AC_ARCH_DEBERTA,
+                                                  AC_ARCH_ROTARY and AC_ARCH_EUROBERT) */
     int vocab, max_pos, type_vocab;
     int pad_idx;         /* roberta, mpnet: position ids start at pad_idx+1 */
     float ln_eps;
@@ -276,13 +280,14 @@ typedef struct {
     int max_tokens;      /* workspace is sized for B*S <= max_tokens */
     int cls_only;        /* != 0: the last layer's output projection / FFN / LayerNorms run on the CLS rows only
                             (classifier.py:1272 uses nothing else); 0 keeps the full last hidden state */
-    /* AC_ARCH_MODERNBERT only (ignored otherwise), except rope_full, which AC_ARCH_ROTARY reads too.  For both,
+    /* AC_ARCH_MODERNBERT only (ignored otherwise), except rope_full, which AC_ARCH_ROTARY and AC_ARCH_EUROBERT read too.
+       For all three,
        AC_ENCODER_MAX_S <= max_pos <= AC_MODERNBERT_MAX_S is the longest sequence the encoder accepts and the rows of its
        RoPE tables (RoPE has no position parameters). */
     int sliding_window;          /* half-window w = local_attention / 2: a sliding layer's query i sees keys |i - j| <= w */
     const int32_t *layer_sliding;  /* HOST array [layers]: 1 = sliding_attention, 0 = full_attention (config.layer_types) */
     const float *rope_full;      /* DEVICE [max_pos, 64] fp32 RoPE table of the full-attention layers (every layer of
-                                    AC_ARCH_ROTARY):                                                                   */
+                                    AC_ARCH_ROTARY and AC_ARCH_EUROBERT):                                              */
     const float *rope_sliding;   /*   row = position, [0, 32) cos, [32, 64) sin of the 32 frequencies (HF
                                        ModernBertRotaryEmbedding's formula = LlamaRotaryEmbedding's, default rope type,
                                        built by the caller); the sliding layers' table */
@@ -304,7 +309,7 @@ typedef struct {
        other than hidden needs the projection ac_encoder_weights.emb_proj_w; with a projection E % 128 == 0, E <= hidden. */
     int embedding_size;
     int ffn_act;                 /* AC_FFN_*: the FFN activation of a post-LN encoder; AC_ARCH_MODERNBERT (GeGLU) takes 0,
-                                    AC_FFN_SWIGLU is AC_ARCH_ROTARY's only */
+                                    AC_ARCH_EUROBERT AC_FFN_SWIGLU; among the others AC_FFN_SWIGLU is AC_ARCH_ROTARY's only */
 } ac_encoder_config;
 
 enum {
@@ -323,6 +328,14 @@ enum {
  * AC_ARCH_ROTARY takes the BERT fields but pos_emb, every bias present (pass zeros where the checkpoint has none): q/k/v/ao
  * self_attn.{q,k,v,o}_proj, ao_ln post_attention_layernorm, ff1 mlp.fc1 or (AC_FFN_SWIGLU) cat(mlp.gate_proj, mlp.up_proj),
  * ff2 mlp.fc2 / mlp.down_proj, out_ln post_mlp_layernorm.
+ * AC_ARCH_EUROBERT (models/eurobert/modeling_eurobert.py, no biases) uses the AC_ARCH_MODERNBERT fields, every other pointer
+ * may be NULL (emb_ln_w is not read: there is no embedding norm):
+ *   word_emb        embed_tokens                      attn_norm_w[l]  layers.l.input_layernorm (entry 0 USED)
+ *   wqkv[l]         cat(q_proj, k_proj, v_proj) [3H, H], k_proj / v_proj expanded to every query head (grouped-query
+ *                   attention: query head h reads kv head h / (heads / num_key_value_heads), HF repeat_kv's order)
+ *   ao_w[l]         layers.l.self_attn.o_proj         ao_ln_w[l]      layers.l.post_attention_layernorm
+ *   wi[l]           cat(mlp.gate_proj, mlp.up_proj) [2I, H]
+ *   ff2_w[l]        layers.l.mlp.down_proj            final_norm_w    norm
  * Shared layers (ALBERT's cross-layer parameter sharing): a packed operand whose source pointers -- weights, biases and the
  * LayerNorm folded into it -- equal an earlier layer's reuses that layer's packed copy, so pass the same pointer for every
  * layer that shares a tensor.  Sharing is by pointer identity only: equal values at different addresses are packed twice. */
@@ -334,8 +347,9 @@ typedef struct {
     const float *const *ao_w, *const *ao_b, *const *ao_ln_w, *const *ao_ln_b;
     const float *const *ff1_w, *const *ff1_b, *const *ff2_w, *const *ff2_b;
     const float *const *out_ln_w, *const *out_ln_b;
-    /* AC_ARCH_MODERNBERT */
-    const float *const *attn_norm_w;  /* [layers] layers.l.attn_norm (entry 0 unused: layer 0's attn_norm is Identity) */
+    /* AC_ARCH_MODERNBERT (and AC_ARCH_EUROBERT, as listed above) */
+    const float *const *attn_norm_w;  /* [layers] layers.l.attn_norm (ModernBERT: entry 0 unused, layer 0's attn_norm is
+                                         Identity) */
     const float *final_norm_w;        /* final_norm */
     const float *const *wqkv;         /* [layers] layers.l.attn.Wqkv [3H, H], q, k, v thirds */
     const float *const *wi;           /* [layers] layers.l.mlp.Wi [2I, H], input rows then gate rows */
@@ -355,7 +369,7 @@ int ac_encoder_destroy(ac_encoder *enc);
 
 /* ids[B,S] int32 token ids, mask[B,S] int32 (1 keep / 0 pad; NULL = all ones), type_ids nullable (ignored by
  * AC_ARCH_MODERNBERT, whose RoPE positions are 0..S-1 for every sequence, padded or not).  S <= AC_ENCODER_MAX_S, or
- * S <= max_pos for AC_ARCH_MODERNBERT and AC_ARCH_ROTARY, or, for an AC_ARCH_ROBERTA encoder with max_pos > AC_ENCODER_MAX_S + pad_idx + 1,
+ * S <= max_pos for AC_ARCH_MODERNBERT, AC_ARCH_ROTARY and AC_ARCH_EUROBERT, or, for an AC_ARCH_ROBERTA encoder with max_pos > AC_ENCODER_MAX_S + pad_idx + 1,
  * S <= min(AC_MODERNBERT_MAX_S, max_pos - pad_idx - 1) (its positions run from pad_idx + 1; head_dim 64 past
  * AC_ENCODER_MAX_S).
  * out_unit_cls[B,H] = L2-normalised (eps 1e-12) CLS row of the last hidden state. */
