@@ -294,13 +294,16 @@ static int plan_training(int batch, const ac_head_params *p, int n_steps, bool u
     if (a.items < G) G = a.items;               // tiny heads: no idle CTAs spinning in the barriers
     pl.G = G;
     plan_args(a, batch, p, G);
-    // AdamW moments resident in shared memory if at least three ring stages still fit; then as many stages (<= 8) as there is room for
+    // AdamW moments resident in shared memory if at least three ring stages still fit; then as many stages (<= 8) as there is room
+    // for, but no more than the longest product has chunks plus one: a deeper ring is never filled and only takes shared memory
     const size_t limit = 220 * 1024;
     pl.smem_bytes = ~size_t(0);
     constexpr int res_min_nst = 3;      // resident moments must leave room for at least three ring stages; otherwise they stay in L2
+    const int nst_useful = (a.kmax + ht::HT_KC - 1) / ht::HT_KC + 1;
+    const int nst_max = nst_useful < res_min_nst ? res_min_nst : (nst_useful > 8 ? 8 : nst_useful);
     for (int res = update ? 1 : 0; res >= 0; --res) {
         a.res_mv = res;
-        for (a.nst = 8; a.nst >= (res ? res_min_nst : 2); --a.nst) {
+        for (a.nst = nst_max; a.nst >= (res ? res_min_nst : 2); --a.nst) {
             const size_t bytes = static_cast<size_t>(ht::ht_smem_layout(a).total) * sizeof(float);
             if (bytes <= limit) { pl.smem_bytes = bytes; break; }
         }

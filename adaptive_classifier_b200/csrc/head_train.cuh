@@ -347,7 +347,9 @@ __device__ __forceinline__ void ht_rows_dot(float *out, float *As, float *red, f
         }
         HT_DSTAMP(2);
     }
-    // combine the 8 column parts in order
+    // combine the 8 column parts in order.  `red` shares its floats with the ring (ht_smem_layout): every copy has landed (the
+    // last wait covered the last chunk) and the barrier orders the last chunk's reads before the partials overwrite it
+    __syncthreads();
 #pragma unroll
     for (int bi = 0; bi < 2; ++bi)
         if (bi < nb) {
@@ -417,6 +419,9 @@ __device__ __forceinline__ void ht_outer_acc(float *g, float *As, int nst, const
 // shared-memory carve-up (floats), identical on host and device.  Per slot s: parameter rows th + s * 8 * kmax, gradient rows
 // g + s * 8 * kmax, moments mv + s * 16 * kmax (m then v; only with res_mv), biases bs + 8 s, bias gradients gb + 8 s, relu' * mask
 // factors (later the input gradients of the own rows) fac + s * batch * 8, bias moments bm + 16 s (m then v).
+// The column-part partials `red` of ht_rows_dot are only written after a product's last chunk has been consumed, so they
+// share their floats with the streamed-operand ring As (sized for the larger of the two): 16 KB that lets a 1024-wide head
+// with two slots train at batch 32.
 struct Smem {
     int th, g, mv, bs, gb, bm, fac;
     int dA, out, As, Wt, red, rsum, ridx /* int64 */, bc, scal, total;
@@ -434,9 +439,10 @@ __host__ __device__ inline Smem ht_smem_layout(const Args &a) {
     s.fac = take(a.slots * a.batch * HT_RB);
     s.dA = take(a.batch * HT_RB);
     s.out = take(a.batch * HT_RB);
-    s.As = take(a.nst * a.batch * HT_AS);
+    const int ring = a.nst * a.batch * HT_AS, red = HT_KPARTS * HT_MAXB * HT_RB;
+    s.As = take(ring > red ? ring : red);
+    s.red = s.As;
     s.Wt = take(a.nst * HT_RB * HT_KC);
-    s.red = take(HT_KPARTS * HT_MAXB * HT_RB);
     s.rsum = take(HT_THREADS);
     s.ridx = take(2 * HT_MAXB);
     s.bc = take(2 * HT_BCW);
@@ -659,14 +665,17 @@ __global__ void __launch_bounds__(HT_THREADS, 1) head_train_kernel(const Args a)
                 if (lane == 0) a.rowloss[b] = (y >= 0 && y < C) ? (STRAT ? invB * (lse - zy) : (lse - zy)) : 0.f;
             } else {
                 const float *yr = static_cast<const float *>(a.targets) + ridx[b] * C;
-                const float inv = 1.f / (static_cast<float>(Bt) * static_cast<float>(C));
+                const float numel = static_cast<float>(Bt) * static_cast<float>(C);
                 float l = 0.f;
                 for (int j = lane; j < ldz; j += 32) {
                     if (j < C) {
                         const float s = 1.f / (1.f + expf(-HT_LDCG(zr + j)));
                         const float y = yr[j];
                         l -= y * fmaxf(logf(s), -100.f) + (1.f - y) * fmaxf(logf(1.f - s), -100.f);   // nn.BCELoss clamps log at -100
-                        dr[j] = (s - y) * inv;
+                        // ATen's BCE backward (s - y) / max(s (1 - s), 1e-12) / (B C), then sigmoid's backward times (1 - s) s:
+                        // not (s - y) / (B C), which differs where s rounds to 1 (z > 16.6) or s (1 - s) < 1e-12 (z < -27.6)
+                        const float sp = (1.f - s) * s;
+                        dr[j] = (s - y) / fmaxf(sp, 1e-12f) / numel * (1.f - s) * s;
                     } else {
                         dr[j] = 0.f;
                     }

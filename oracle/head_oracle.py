@@ -63,7 +63,8 @@ def head_grads(X: Tensor, y: Tensor, p: Dict[str, Tensor], masks: Optional[Tuple
         s = torch.sigmoid(z)
         C = z.shape[1]
         loss = -(y * torch.log(s).clamp_min(-100) + (1 - y) * torch.log(1 - s).clamp_min(-100)).mean()
-        dz = (s - y) / (B * C)
+        # ATen's BCE backward, then sigmoid's backward: the gradient vanishes where s rounds to 1 or s (1 - s) < 1e-12
+        dz = (s - y) / ((1 - s) * s).clamp_min(1e-12) / (B * C) * (1 - s) * s
     g = {}
     g["W2"] = dz.t() @ h1d
     g["b2"] = dz.sum(0)

@@ -3,7 +3,8 @@
 // grid barriers are real barriers and the scheduler shuffles the thread order between barriers, so a missing barrier or a
 // wrong ownership index changes the result.  The kernel header is compiled as is (it is plain SIMT C++); the result of
 // several optimizer steps is compared with a straightforward restatement of the same arithmetic (natural loop order) below.
-//   usage: head_train_emul D H0 H1 C n batch G loss(0 ce|1 bce) dropout_p ewc(0|1) update(0|1) seed
+//   usage: head_train_emul D H0 H1 C n batch G loss(0 ce|1 bce) dropout_p ewc(0|1) update(0|1) seed [z_shift]
+//   z_shift: the output biases are moved to +z_shift / -z_shift (even / odd classes) -- saturated logits
 #include "cuda_shim.h"
 #define AC_CPU_SHIM 1
 static inline uint8_t *shim_dyn_smem() { return shim::g_cur->blk->dyn_smem; }
@@ -68,7 +69,7 @@ static float ref_step(RefState &S, const std::vector<float> &X, const std::vecto
             for (int c = 0; c < C; ++c) {
                 const float s = 1.f / (1.f + expf(-z[b * C + c])), y = yf[rows[b] * C + c];
                 l -= y * fmaxf(logf(s), -100.f) + (1.f - y) * fmaxf(logf(1.f - s), -100.f);
-                dz[b * C + c] = (s - y) / (static_cast<float>(B) * C);
+                dz[b * C + c] = (s - y) / fmaxf((1.f - s) * s, 1e-12f) / (static_cast<float>(B) * C) * (1.f - s) * s;
             }
             loss += l / C;
         }
@@ -176,6 +177,7 @@ int main(int argc, char **argv) {
     const float p_drop = static_cast<float>(atof(argv[9]));
     const bool ewc = atoi(argv[10]) != 0, update = atoi(argv[11]) != 0;
     const unsigned seed = static_cast<unsigned>(atoi(argv[12]));
+    const float z_shift = argc > 13 ? static_cast<float>(atof(argv[13])) : 0.f;
     std::mt19937 rng(seed);
     Host T{D, H0, H1, C, {}, {}}, F = T, St = T;
     const int rows[3] = {H0, H1, C}, K[3] = {D, H0, H1};
@@ -188,6 +190,7 @@ int main(int argc, char **argv) {
         for (auto &x : St.W[l]) x += 0.05f;
         for (auto &x : St.b[l]) x -= 0.03f;
     }
+    for (int c = 0; c < C; ++c) T.b[2][c] += (c % 2 ? -z_shift : z_shift);
     std::vector<float> X, yf;
     fill(X, size_t(n) * D, rng, 1.f);
     std::vector<int64_t> yi(n), perm(n);

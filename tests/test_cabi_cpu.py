@@ -79,7 +79,7 @@ def test_head_training_kernel_on_the_cpu_emulation():
     r = subprocess.run(["g++", "-std=c++17", "-O1", "-I/usr/local/cuda/include", os.path.join(shim, "head_train_emul.cpp"),
                         os.path.join(shim, "cuda_shim.cpp"), "-o", exe], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-2000:]
-    #        D   H0  H1  C    n  batch G loss dropout ewc update seed
+    #        D   H0  H1  C    n  batch G loss dropout ewc update seed [z_shift]
     cases = ["40 40 20 5 50 20 3 0 0.1 0 1 1",          # CE, dropout, last batch partial
              "40 40 20 5 50 20 2 1 0.1 0 1 2",          # BCE; 2 CTAs -> several ownership blocks per CTA
              "264 136 68 11 70 32 4 0 0.1 1 1 3",       # K not a multiple of the chunk width; EWC with a grown head
@@ -90,7 +90,9 @@ def test_head_training_kernel_on_the_cpu_emulation():
              "40 40 20 5 50 20 9 0 0.1 1 1 9",
              "264 136 68 11 70 32 28 0 0.1 1 1 10",
              "520 264 68 11 30 30 4 0 0.0 0 0 6",       # several 256-column chunks per product
-             "128 128 64 130 64 32 5 0 0.2 1 1 11"]     # CE with more than 128 classes (logit tail re-read)    # one ownership block per CTA
+             "128 128 64 130 64 32 5 0 0.2 1 1 11",     # CE with more than 128 classes (logit tail re-read)
+             "520 264 68 11 40 3 4 0 0.1 0 0 12",       # partials of the row products larger than the ring they share (batch 3)
+             "40 40 20 6 24 12 3 1 0.0 0 0 13 30"]      # BCE at saturated logits (z ~ +-30): ATen's vanishing gradient
     for c in cases:
         out = subprocess.run([exe] + c.split(), capture_output=True, text=True, timeout=600)
         assert out.returncode == 0 and "MATCH" in out.stdout, (c, out.stdout[-600:], out.stderr[-300:])
