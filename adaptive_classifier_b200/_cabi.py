@@ -82,7 +82,7 @@ class EncoderConfig(Structure):
                 ("sliding_window", c_int), ("layer_sliding", POINTER(ctypes.c_int32)),
                 ("rope_full", c_void_p), ("rope_sliding", c_void_p), ("rel_bias", c_void_p),
                 ("pos_key", c_void_p), ("pos_query", c_void_p), ("pos_span", c_int), ("rel_index", c_void_p),
-                ("embedding_size", c_int), ("ffn_act", c_int)]
+                ("embedding_size", c_int), ("ffn_act", c_int), ("rel_radius", c_int)]
 
 
 _PP = POINTER(c_void_p)
@@ -611,12 +611,14 @@ def mpnet_to_bert_state_dict(sd: dict, c):
     return out, dims
 
 
-def deberta_rel_index(position_buckets: int, max_relative_positions: int) -> Tuple[torch.Tensor, int]:
-    """(rel_index, span) of ac_encoder_config: int32 [2 AC_ENCODER_MAX_S - 1] with entry AC_ENCODER_MAX_S - 1 + r =
+def deberta_rel_index(position_buckets: int, max_relative_positions: int,
+                      radius: int = AC_ENCODER_MAX_S) -> Tuple[torch.Tensor, int]:
+    """(rel_index, span) of ac_encoder_config: int32 [2 radius - 1] with entry radius - 1 + r =
     c(r) = clamp(bucket(r) + span, 0, 2 span - 1) for r = query - key, with HF build_relative_position's arithmetic
     (make_log_bucket_position: identity below span / 2, log-spaced up to max_relative_positions; no buckets when either
-    setting is < 1), span = position_buckets, or max_relative_positions without buckets."""
-    r = torch.arange(-(AC_ENCODER_MAX_S - 1), AC_ENCODER_MAX_S, dtype=torch.long)
+    setting is < 1), span = position_buckets, or max_relative_positions without buckets.  radius is the table's
+    ac_encoder_config.rel_radius (AC_ENCODER_MAX_S: rel_radius 0)."""
+    r = torch.arange(-(radius - 1), radius, dtype=torch.long)
     if position_buckets > 0 and max_relative_positions > 0:
         sign = torch.sign(r)
         mid = position_buckets // 2
@@ -659,7 +661,9 @@ def deberta_to_bert_state_dict(sd: dict, c):
     tables where the checkpoint has none (position_biased_input off, type_vocab_size 0), and build the per-layer fp32
     position tables pos_key / pos_query [layers, 2 span, H] (from the encoder's rel_embeddings, LayerNorm-ed under
     norm_rel_ebd = layer_norm, through key_proj / query_proj or pos_key_proj / pos_query_proj) and rel_index
-    (deberta_rel_index).  Raises AdaptiveB200Error naming any setting the CUDA path does not implement."""
+    (deberta_rel_index).  Without absolute positions (position_biased_input False: deberta-v3-*, mdeberta-v3-base) dims
+    also carry rel_index_long, the radius-AC_MODERNBERT_MAX_S index, with which the encoder takes sequences up to
+    AC_MODERNBERT_MAX_S tokens.  Raises AdaptiveB200Error naming any setting the CUDA path does not implement."""
     deberta_settings(c)
     H, L = c.hidden_size, c.num_hidden_layers
     f32 = lambda t: t.detach().to(device="cpu", dtype=torch.float32)
@@ -683,6 +687,11 @@ def deberta_to_bert_state_dict(sd: dict, c):
     if max_rel < 1:
         max_rel = c.max_position_embeddings
     rel_index, span = deberta_rel_index(buckets, max_rel)
+    # without absolute positions nothing in the model depends on the length: the long index lets S run to
+    # AC_MODERNBERT_MAX_S (Encoder's rel_index_long); with them, max_position_embeddings <= 512 bounds S
+    extra = {}
+    if not getattr(c, "position_biased_input", True):
+        extra["rel_index_long"] = deberta_rel_index(buckets, max_rel, AC_MODERNBERT_MAX_S)[0]
     rel = f32(sd["encoder.rel_embeddings.weight"])
     norm = [x.strip() for x in getattr(c, "norm_rel_ebd", "none").lower().split("|")]
     if "layer_norm" in norm:
@@ -698,7 +707,7 @@ def deberta_to_bert_state_dict(sd: dict, c):
         pq.append(torch.nn.functional.linear(rel, f32(sd[p + qname + ".weight"]), f32(sd[p + qname + ".bias"])))
     dims = dict(layers=L, hidden=H, heads=c.num_attention_heads, intermediate=c.intermediate_size, vocab=c.vocab_size,
                 max_pos=c.max_position_embeddings, type_vocab=max(c.type_vocab_size, 1), ln_eps=c.layer_norm_eps,
-                pad_idx=0, pos_key=torch.stack(pk), pos_query=torch.stack(pq), pos_span=span, rel_index=rel_index)
+                pad_idx=0, pos_key=torch.stack(pk), pos_query=torch.stack(pq), pos_span=span, rel_index=rel_index, **extra)
     return out, dims
 
 
@@ -989,8 +998,10 @@ class Encoder:
     """Owner of an ac_encoder handle built from an HF BERT/RoBERTa/ModernBERT state_dict (CUDA fp32 tensors).  arch "mpnet"
     takes the BERT names (mpnet_to_bert_state_dict) and rel_bias, the [heads, 2 AC_ENCODER_MAX_S - 1] table of
     mpnet_relative_bias_table; arch "deberta" the BERT names and the pos_key / pos_query / pos_span / rel_index of
-    deberta_to_bert_state_dict.  embedding_size (0 = hidden) and the "embeddings_project.*" tensors give factorized
-    embeddings (albert_to_bert_state_dict, electra_to_bert_state_dict); ffn_act is AC_FFN_GELU_ERF or AC_FFN_GELU_TANH.
+    deberta_to_bert_state_dict, and with rel_index_long (position-free configs) that index in place of rel_index, passed
+    with rel_radius AC_MODERNBERT_MAX_S so that sequences run up to that length.  embedding_size (0 = hidden) and the
+    "embeddings_project.*" tensors give factorized embeddings (albert_to_bert_state_dict, electra_to_bert_state_dict);
+    ffn_act is AC_FFN_GELU_ERF or AC_FFN_GELU_TANH.
     arch "rotary" takes the BERT names without a position table, RoPE with base rope_theta on q and k, and ffn_act
     AC_FFN_SWIGLU too (nomic_bert_to_bert_state_dict, jina_v3_to_bert_state_dict).  arch "eurobert" takes the ModernBERT
     names of eurobert_to_modernbert_names (RMSNorms, layer 0's attn_norm used, no embedding norm) and one rope_theta.
@@ -1001,7 +1012,8 @@ class Encoder:
                  max_tokens: int = 65536, device="cuda", cls_only: bool = True, sliding_window: int = 0,
                  layer_sliding=None, rope_theta=None, rel_bias: Optional[torch.Tensor] = None,
                  pos_key: Optional[torch.Tensor] = None, pos_query: Optional[torch.Tensor] = None, pos_span: int = 0,
-                 rel_index: Optional[torch.Tensor] = None, embedding_size: int = 0, ffn_act: int = AC_FFN_GELU_ERF):
+                 rel_index: Optional[torch.Tensor] = None, rel_index_long: Optional[torch.Tensor] = None,
+                 embedding_size: int = 0, ffn_act: int = AC_FFN_GELU_ERF):
         L = load_library()
         self._L = L
         self.hidden = hidden
@@ -1079,6 +1091,9 @@ class Encoder:
                 keep["rel_bias"] = rb
                 cfg.rel_bias = rb.data_ptr()
             if arch == "deberta":         # ac_encoder_create refuses a DeBERTa encoder without its tables
+                if rel_index_long is not None:
+                    rel_index = rel_index_long
+                    cfg.rel_radius = (rel_index.numel() + 1) // 2
                 pos = [t.detach().to(device=dev, dtype=dt).contiguous() if t is not None else None
                        for t, dt in ((pos_key, torch.float32), (pos_query, torch.float32), (rel_index, torch.int32))]
                 keep["pos"] = pos
@@ -1100,7 +1115,9 @@ class Encoder:
         to max(512, min(max_position_embeddings, AC_MODERNBERT_MAX_S)), RoPE positions 0..S-1 whatever the padding; their
         remote-code modules (trust_remote_code=True), whose parameter names differ, are refused.  head_dim 64 or 32 for BERT / RoBERTa /
         DistilBERT, 64 for MPNet, DeBERTa and ModernBERT.  Sequences up to 512 tokens, or for ModernBERT up to max(512, max_position_embeddings) <=
-        AC_MODERNBERT_MAX_S.  A RoBERTa / XLM-RoBERTa model with head_dim 64 whose position table has more than
+        AC_MODERNBERT_MAX_S.  DeBERTa-v2 / v3 without absolute positions (position_biased_input False: deberta-v3-*,
+        mdeberta-v3-base) takes sequences up to AC_MODERNBERT_MAX_S, as HF does; with absolute positions the 512 limit
+        stays.  A RoBERTa / XLM-RoBERTa model with head_dim 64 whose position table has more than
         512 + pad_token_id + 1 rows (bge-m3, snowflake-arctic-embed-l-v2.0: 8194) takes sequences up to
         min(AC_MODERNBERT_MAX_S, max_position_embeddings - pad_token_id - 1), which run the long full-attention kernel
         past 512 tokens; BERT-arch models keep the 512 limit."""

@@ -1033,9 +1033,10 @@ constexpr int ATTS_SMEM = ATTS_OFF_TERM + Score::SMEM_STREAM + 1024 /*align*/;
 // Each product is 2 x 2 wgmma m64n128k64 (query / key rows 0-63, 64-127 by G rows 0-127, 128-255) whose fragments are
 // added straight into the fp32 score tile: every fragment element lands on at most one score and every score receives
 // exactly one element per term, so a pass needs no atomics (the two passes are separated by a barrier).  Row 255 of a box
-// is zero and never lands.  delta = 128 (blockIdx.y - key block) is one of 7 values for S <= 512.
+// is zero and never lands.  delta = 128 (blockIdx.y - key block); c(r) is monotone and saturates, so past some radius
+// D every row of a box is the saturated one and the handle keeps only the boxes of blockIdx.y - key block in [-D, D]
+// (n = 2 D + 1 of them, ac_encoder_create), a larger offset reading the box at +-D.  That bounds the boxes at any S.
 // smem: the c2p box has its own 32 KB; the p2c box goes through the P slabs, free between PV and the next softmax.
-constexpr int ATTS_POS_DELTAS = 2 * (AC_ENCODER_MAX_S / 128) - 1;
 
 // C = A G^T of one relative term over the 128 A rows (sA: Q or this key block's K) and the 256-row box sG, added into the
 // score tile: c2p (P2C false) at (row, row - n + 127), p2c at (row - n + 127, row); n = the box row of the product column
@@ -1071,6 +1072,7 @@ __device__ __forceinline__ void att_rel_term(const uint8_t *sA, const uint8_t *s
 struct ScoreDisent : ScorePlain {
     CUtensorMap tmap_pos;                         // 128-row boxes over ac_encoder::pos_g
     int pos_row0;                                 // first row of the layer's boxes
+    int pos_d;                                    // D: the boxes cover block offsets -D .. D
     static constexpr int MIN_DH = 64;
     static constexpr bool ONE_BLOCK = false;
     static constexpr int SCALE_TERMS = 3;
@@ -1079,8 +1081,8 @@ struct ScoreDisent : ScorePlain {
     static constexpr int SMEM_STREAM = OFF_G + 2 * ATTS_STAGE_BYTES;
     // the c2p (term 0) / p2c (term 1) box of visit i -> its own 32 KB / the P slabs; window 0, so visit i is key block i
     __device__ __forceinline__ void issue_pos(const AttCta &cta, int i, int term) const {
-        const int row =
-            pos_row0 + (((static_cast<int>(blockIdx.y) - i + ATTS_POS_DELTAS / 2) * cta.heads + cta.h) * 2 + term) * 256;
+        const int d = min(max(static_cast<int>(blockIdx.y) - i, -pos_d), pos_d) + pos_d;
+        const int row = pos_row0 + ((d * cta.heads + cta.h) * 2 + term) * 256;
         uint64_t *bar = reinterpret_cast<uint64_t *>(cta.term) + term;
         uint8_t *dst = term ? cta.smem + ATTS_OFF_P : cta.term + OFF_G;
         mbar_arrive_expect_tx(bar, 2 * ATTS_STAGE_BYTES);
@@ -1447,24 +1449,26 @@ __global__ void gather_cls_ln_kernel(const __half *__restrict__ ctx, const float
     ln_row(x, nv, H, g, b, eps, lane, x_cls + dst, nullptr);
 }
 
-// DeBERTa operand boxes of attention_stream_kernel<64, ScoreDisent> (see att_rel_term): row ((((l ATTS_POS_DELTAS + d) heads
-// + h) 2 + term) 256 + t) = fp16 (RNE) of PosK (term 0) / PosQ (term 1) [l, c(r), 64 h .. 64 h + 63] with delta = 128 (d - 3),
-// r = delta + t - 127 (c2p) or delta + 127 - t (p2c), c(r) = rel_index[AC_ENCODER_MAX_S - 1 + r]; row t = 255 is zero.
+// DeBERTa operand boxes of attention_stream_kernel<64, ScoreDisent> (see att_rel_term): row ((((l n + d) heads + h) 2 + term)
+// 256 + t) = fp16 (RNE) of PosK (term 0) / PosQ (term 1) [l, c(r), 64 h .. 64 h + 63] with delta = 128 (d - n / 2),
+// r = delta + t - 127 (c2p) or delta + 127 - t (p2c), c(r) = rel_index[radius - 1 + r]; row t = 255 is zero.  rel_index
+// covers |r| < radius; a box row past it (|r| >= radius: no query-key pair of an accepted S) reads the nearest entry.
 // pos_key / pos_query [layers, 2 span, H] fp32.  64 threads per row, 4 rows per block.
 __global__ void pos_gather_kernel(const float *__restrict__ pos_key, const float *__restrict__ pos_query,
-                                  const int32_t *__restrict__ rel_index, int span, int heads, int H, __half *__restrict__ out) {
+                                  const int32_t *__restrict__ rel_index, int radius, int n, int span, int heads, int H,
+                                  __half *__restrict__ out) {
     const int64_t row = static_cast<int64_t>(blockIdx.x) * 4 + (threadIdx.x >> 6);
     const int col = threadIdx.x & 63;
     const int t = static_cast<int>(row % 256), term = static_cast<int>((row / 256) % 2);
     const int h = static_cast<int>((row / 512) % heads);
-    const int64_t ld = row / (512 * static_cast<int64_t>(heads));          // l ATTS_POS_DELTAS + d
-    const int d = static_cast<int>(ld % ATTS_POS_DELTAS);
-    const int64_t l = ld / ATTS_POS_DELTAS;
+    const int64_t ld = row / (512 * static_cast<int64_t>(heads));          // l n + d
+    const int d = static_cast<int>(ld % n);
+    const int64_t l = ld / n;
     float v = 0.f;
     if (t < 255) {
-        const int delta = 128 * (d - ATTS_POS_DELTAS / 2);
-        const int r = term ? delta + 127 - t : delta + t - 127;
-        const int c = min(max(rel_index[AC_ENCODER_MAX_S - 1 + r], 0), 2 * span - 1);
+        const int delta = 128 * (d - n / 2);
+        const int r = min(max(term ? delta + 127 - t : delta + t - 127, 1 - radius), radius - 1);
+        const int c = min(max(rel_index[radius - 1 + r], 0), 2 * span - 1);
         v = (term ? pos_query : pos_key)[(l * 2 * span + c) * H + 64 * h + col];
     }
     out[row * 64 + col] = __float2half_rn(v);
@@ -1526,10 +1530,11 @@ struct ac_encoder {
     float *ones = nullptr, *zeros = nullptr;   // ones [H]; zeros [max(3H, 2I)]: beta / bias of the bias-free ModernBERT
     float *rope[2] = {nullptr, nullptr};       // RoPE tables [max_pos, 64]: ModernBERT (full, sliding layers), rotary (full)
     float *rel_bias = nullptr;                 // MPNet relative position bias [heads, 2 AC_ENCODER_MAX_S - 1]; NULL otherwise
-    // DeBERTa c2p / p2c operand boxes [layers, ATTS_POS_DELTAS, heads, 2 (c2p, p2c), 256, 64] fp16 (pos_gather_kernel) and
+    // DeBERTa c2p / p2c operand boxes [layers, 2 pos_d + 1, heads, 2 (c2p, p2c), 256, 64] fp16 (pos_gather_kernel) and
     // their 128-row-box map; NULL otherwise
     __half *pos_g = nullptr;
     CUtensorMap m_pos;
+    int pos_d = 0;                        // the boxes' block offsets -pos_d .. pos_d (deberta_box_radius)
     std::vector<void *> allocs;
     int last_B = 0, last_S = 0;           // shape of the previous forward; its full hidden state (cls_only = 0) is in tmp
     bool last_cls_only = false;
@@ -1560,7 +1565,7 @@ static const AttVariant att_variants[ATT_VARIANTS] = {
 // softmax(Q K^T / sqrt(head_dim) [+ MPNet relative bias] + mask) V out of e->qk / e->vT into e->ctx; window = sliding
 // half-window, 0 = full attention.  S <= 128 runs attention_kernel, longer sequences attention_stream_kernel over 128-query
 // blocks; DeBERTa runs attention_stream_kernel<64, ScoreDisent> at every length, with layer `layer`'s c2p / p2c boxes.
-// Past AC_ENCODER_MAX_S every encoder but ModernBERT (in practice RoBERTa-arch ones with a long position table,
+// Past AC_ENCODER_MAX_S every encoder but ModernBERT and DeBERTa (in practice RoBERTa-arch ones with a long position table,
 // check_shape_map_vt) runs attention_long_kernel; ModernBERT keeps attention_stream_kernel at every length.
 // cls_rows: only row 0 of every sequence is read afterwards (the CLS-only tail), so only the first query block is computed.
 static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, int window, bool cls_rows, int layer,
@@ -1597,7 +1602,8 @@ static int launch_attention(ac_encoder *e, const int32_t *mask, int B, int S, in
     int id = dh == 32 ? (streamed ? ATTS_PLAIN32 : ATT_PLAIN32) : (streamed ? ATTS_PLAIN64 : ATT_PLAIN64);
     if (e->pos_g) {
         disent.tmap_pos = e->m_pos;
-        disent.pos_row0 = layer * ATTS_POS_DELTAS * heads * 2 * 256;
+        disent.pos_row0 = layer * (2 * e->pos_d + 1) * heads * 2 * 256;
+        disent.pos_d = e->pos_d;
         score = &disent;
         id = ATTS_DISENT;
     } else if (e->rel_bias) {
@@ -1665,6 +1671,25 @@ static int pack_consumer(ac_encoder *e, int n, const float *const *W, const floa
     return AC_OK;
 }
 
+// D of a DeBERTa handle's operand boxes, from its index table idx (entry radius - 1 + r = c(r), |r| < radius): the least d
+// for which c is constant for r >= 128 d - 127 and for r <= 127 - 128 d, so that the boxes at +-d, and every box farther
+// out, hold one row throughout (pos_gather_kernel) and a larger block offset may read the box at +-d.  At most
+// (radius - 1) / 128, the largest block offset of a sequence of S <= radius.  Published v3 settings give 5.
+static int deberta_box_radius(const std::vector<int32_t> &idx, int radius) {
+    const int cap = (radius - 1) / 128;
+    const auto c = [&](int r) { return idx[radius - 1 + r]; };
+    const auto saturated = [&](int d) {
+        for (int r = 128 * d - 127; r < radius; ++r)
+            if (c(r) != c(radius - 1)) return false;
+        for (int r = 127 - 128 * d; r > -radius; --r)
+            if (c(r) != c(1 - radius)) return false;
+        return true;
+    };
+    int d = 0;
+    while (d < cap && !saturated(d)) ++d;
+    return d;
+}
+
 extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_weights *w, ac_encoder **out) {
     AC_REQUIRE(cfg && w && out, "ac_encoder_create: null argument");
     const bool mb = cfg->arch == AC_ARCH_MODERNBERT;
@@ -1700,6 +1725,10 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
                        cfg->hidden == 64 * cfg->heads),
                "ac_encoder_create: DeBERTa needs pos_key, pos_query, rel_index, pos_span > 0 (pos_span=%d) and head_dim 64 "
                "(hidden=%d heads=%d)", cfg->pos_span, cfg->hidden, cfg->heads);
+    AC_REQUIRE(cfg->rel_radius == 0 ||
+                   (db && cfg->rel_radius > AC_ENCODER_MAX_S && cfg->rel_radius <= AC_MODERNBERT_MAX_S),
+               "ac_encoder_create: rel_radius=%d must be 0 (AC_ENCODER_MAX_S), or %d < rel_radius <= %d on an "
+               "AC_ARCH_DEBERTA encoder (arch=%d)", cfg->rel_radius, AC_ENCODER_MAX_S, AC_MODERNBERT_MAX_S, cfg->arch);
     AC_REQUIRE(cfg->intermediate % 64 == 0 && cfg->layers > 0 && cfg->max_tokens > 0, "ac_encoder_create: bad dims");
     AC_REQUIRE(cfg->ffn_act == AC_FFN_GELU_ERF || cfg->ffn_act == AC_FFN_GELU_TANH || cfg->ffn_act == AC_FFN_SWIGLU,
                "ac_encoder_create: unknown ffn_act=%d", cfg->ffn_act);
@@ -1788,9 +1817,28 @@ extern "C" int ac_encoder_create(const ac_encoder_config *cfg, const ac_encoder_
         }
         if (mp) TRY(pack_f32(e, &e->rel_bias, cfg->rel_bias, static_cast<size_t>(cfg->heads) * (2 * AC_ENCODER_MAX_S - 1)));
         if (db) {
-            const size_t rows = static_cast<size_t>(L) * ATTS_POS_DELTAS * cfg->heads * 2 * 256;
+            const int R = e->cfg.rel_radius = cfg->rel_radius ? cfg->rel_radius : AC_ENCODER_MAX_S;
+            if (R > AC_ENCODER_MAX_S) {
+                // past max_pos the embedding kernel re-reads the table's last row: only a table of zeros (no absolute
+                // positions, position_biased_input = False) is position-free
+                std::vector<float> pos(static_cast<size_t>(cfg->max_pos) * E);
+                TRY(check_cuda(cudaMemcpy(pos.data(), e->pos, pos.size() * sizeof(float), cudaMemcpyDeviceToHost),
+                               "copy pos_emb"));
+                if (std::any_of(pos.begin(), pos.end(), [](float v) { return v != 0.f; })) {
+                    set_error("ac_encoder_create: rel_radius=%d needs an all-zero pos_emb (a DeBERTa encoder without "
+                              "absolute positions, position_biased_input = False)", R);
+                    ac_encoder_destroy(e);
+                    return AC_E_INVALID;
+                }
+            }
+            std::vector<int32_t> idx(2 * R - 1);
+            TRY(check_cuda(cudaMemcpy(idx.data(), cfg->rel_index, idx.size() * sizeof(int32_t), cudaMemcpyDeviceToHost),
+                           "copy rel_index"));
+            e->pos_d = deberta_box_radius(idx, R);
+            const int n = 2 * e->pos_d + 1;
+            const size_t rows = static_cast<size_t>(L) * n * cfg->heads * 2 * 256;
             TRY(dev_alloc(e, &e->pos_g, rows * 64));
-            pos_gather_kernel<<<static_cast<unsigned>(rows / 4), 256>>>(cfg->pos_key, cfg->pos_query, cfg->rel_index,
+            pos_gather_kernel<<<static_cast<unsigned>(rows / 4), 256>>>(cfg->pos_key, cfg->pos_query, cfg->rel_index, R, n,
                                                                         cfg->pos_span, cfg->heads, H, e->pos_g);
             TRY(check_cuda(cudaGetLastError(), "pos_gather_kernel"));
             TRY(make_tmap_2d(&e->m_pos, e->pos_g, 2, rows, 64, 128, 128, 64));
@@ -2057,6 +2105,13 @@ static int check_shape_map_vt(ac_encoder *e, const char *who, int B, int S) {
     } else if (e->cfg.arch == AC_ARCH_EUROBERT) {
         AC_REQUIRE(S <= e->cfg.max_pos, "%s: S=%d exceeds this EuroBERT encoder's max_pos=%d (min(max_position_embeddings, %d))",
                    who, S, e->cfg.max_pos, AC_MODERNBERT_MAX_S);
+    } else if (e->cfg.arch == AC_ARCH_DEBERTA && e->cfg.rel_radius > AC_ENCODER_MAX_S) {
+        // relative positions only (ac_encoder_create checked that pos_emb is zeros): rel_index bounds S, max_pos does not
+        if (S > e->cfg.rel_radius) {
+            set_error("%s: S=%d exceeds %d, the rel_radius of this DeBERTa encoder's relative position index", who, S,
+                      e->cfg.rel_radius);
+            return AC_E_UNSUPPORTED;
+        }
     } else if (S > AC_ENCODER_MAX_S) {
         // RoBERTa positions run from pad_idx + 1: a table with more rows than AC_ENCODER_MAX_S of them (XLM-R's 8194) takes
         // the sequences it has positions for, up to AC_MODERNBERT_MAX_S
@@ -2075,7 +2130,7 @@ static int check_shape_map_vt(ac_encoder *e, const char *who, int B, int S) {
     }
     AC_REQUIRE(static_cast<int64_t>(B) * S <= e->cfg.max_tokens, "%s: B*S=%lld exceeds max_tokens=%d", who,
                static_cast<long long>(B) * S, e->cfg.max_tokens);
-    AC_REQUIRE(S <= e->cfg.max_pos, "%s: S exceeds max_position_embeddings", who);
+    AC_REQUIRE(S <= e->cfg.max_pos || e->cfg.rel_radius > AC_ENCODER_MAX_S, "%s: S exceeds max_position_embeddings", who);
     const int H = e->cfg.hidden;
     const int S_pad = (S + 7) / 8 * 8;
     AC_REQUIRE(static_cast<size_t>(B) * H * S_pad <= e->vt_elems,

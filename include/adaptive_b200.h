@@ -303,13 +303,20 @@ typedef struct {
                                     rel = rel_embeddings (LayerNorm-ed when norm_rel_ebd = layer_norm), biases included */
     const float *pos_query;      /* [layers, 2 pos_span, H] fp32: query_proj(rel) or pos_query_proj(rel) */
     int pos_span;                /* position_buckets, or max_relative_positions without buckets */
-    const int32_t *rel_index;    /* [2 AC_ENCODER_MAX_S - 1] int32: entry AC_ENCODER_MAX_S - 1 + r is
-                                    c(r) = clamp(bucket(r) + pos_span, 0, 2 pos_span - 1) (HF build_relative_position) */
+    const int32_t *rel_index;    /* [2 R - 1] int32, R = rel_radius or AC_ENCODER_MAX_S when it is 0: entry R - 1 + r is
+                                    c(r) = clamp(bucket(r) + pos_span, 0, 2 pos_span - 1) (HF build_relative_position)
+                                    for -R < r < R */
     /* factorized embeddings (ALBERT, ELECTRA): width E of the embedding tables and their LayerNorm; 0 means hidden.  An E
        other than hidden needs the projection ac_encoder_weights.emb_proj_w; with a projection E % 128 == 0, E <= hidden. */
     int embedding_size;
     int ffn_act;                 /* AC_FFN_*: the FFN activation of a post-LN encoder; AC_ARCH_MODERNBERT (GeGLU) takes 0,
                                     AC_ARCH_EUROBERT AC_FFN_SWIGLU; among the others AC_FFN_SWIGLU is AC_ARCH_ROTARY's only */
+    int rel_radius;              /* AC_ARCH_DEBERTA: the radius R of rel_index.  0 = AC_ENCODER_MAX_S, with S <= max_pos.
+                                    AC_ENCODER_MAX_S < R <= AC_MODERNBERT_MAX_S: S <= R, for an encoder without absolute
+                                    positions only (position_biased_input = False: pos_emb all zeros, which
+                                    ac_encoder_create checks).  Must be 0 for every other arch.  The handle keeps
+                                    layers x (2 D + 1) x heads x 64 KiB of relative operands, D <= 5 for the published
+                                    settings (D = the block offset past which c(r) is saturated, derived from rel_index). */
 } ac_encoder_config;
 
 enum {
@@ -371,7 +378,7 @@ int ac_encoder_destroy(ac_encoder *enc);
  * AC_ARCH_MODERNBERT, whose RoPE positions are 0..S-1 for every sequence, padded or not).  S <= AC_ENCODER_MAX_S, or
  * S <= max_pos for AC_ARCH_MODERNBERT, AC_ARCH_ROTARY and AC_ARCH_EUROBERT, or, for an AC_ARCH_ROBERTA encoder with max_pos > AC_ENCODER_MAX_S + pad_idx + 1,
  * S <= min(AC_MODERNBERT_MAX_S, max_pos - pad_idx - 1) (its positions run from pad_idx + 1; head_dim 64 past
- * AC_ENCODER_MAX_S).
+ * AC_ENCODER_MAX_S), or, for an AC_ARCH_DEBERTA encoder created with rel_radius > AC_ENCODER_MAX_S, S <= rel_radius.
  * out_unit_cls[B,H] = L2-normalised (eps 1e-12) CLS row of the last hidden state. */
 int ac_encoder_forward_cls(ac_encoder *enc, const int32_t *ids, const int32_t *mask,
                            const int32_t *type_ids, int B, int S, float *out_unit_cls,

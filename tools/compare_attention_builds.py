@@ -14,6 +14,10 @@ a process of its own, and compares the outputs with torch.equal.  One encoder pe
 Per case: `Encoder.forward_cls` (unit CLS rows, fp32) and `Encoder.attention` on seeded q, k, v (the stage alone, fp16; with
 the sliding half-window on ModernBERT).  Prints one line per case and exits 1 if any bit differs.  Writes only to a
 temporary directory.
+
+A library that sits in a built source tree (next to its own _cabi.py, as adaptive_classifier_b200/libadaptive_b200.so
+does) is driven by that tree's bindings, so builds whose C ABI or table layouts differ are each called as their own
+Python calls them.
 """
 import argparse
 import os
@@ -57,6 +61,9 @@ def model(name):
 
 
 def emit(lib, out_path):
+    pkg = os.path.dirname(os.path.abspath(lib))
+    if os.path.exists(os.path.join(pkg, "_cabi.py")):
+        sys.path.insert(0, os.path.dirname(pkg))
     from adaptive_classifier_b200 import _cabi
     _cabi.LIB_PATH = lib
     _cabi.load_library()
