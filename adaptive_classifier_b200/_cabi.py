@@ -47,6 +47,7 @@ EXPORTS = [
     "ac_pipeline_create", "ac_pipeline_destroy", "ac_pipeline_predict_device", "ac_pipeline_predict_host",
     "ac_pipeline_encode", "ac_pipeline_embeddings", "ac_pipeline_search_shard", "ac_pipeline_finish_sharded",
     "ac_pipeline_debug_copy", "ac_pipeline_knn_stats", "ac_launch_count", "ac_profile_enable", "ac_profile_read",
+    "ac_tokenizer_create", "ac_tokenizer_destroy", "ac_tokenize_workspace_bytes", "ac_tokenize", "ac_tokenize_pack",
 ]
 
 
@@ -86,6 +87,14 @@ class EncoderConfig(Structure):
 
 
 _PP = POINTER(c_void_p)
+
+
+class TokenizerSpec(Structure):
+    _fields_ = [("norm", c_void_p), ("cls", c_void_p), ("pool", c_void_p), ("pool_len", c_int64),
+                ("vocab_bytes", c_void_p), ("vocab_offsets", c_void_p), ("vocab_ids", c_void_p), ("n_vocab", c_int),
+                ("added_bytes", c_void_p), ("added_offsets", c_void_p), ("added_ids", c_void_p), ("n_added", c_int),
+                ("prefix", c_char_p), ("prefix_len", c_int),
+                ("cls_id", c_int), ("sep_id", c_int), ("pad_id", c_int), ("unk_id", c_int), ("max_input_chars", c_int)]
 
 
 class EncoderWeights(Structure):
@@ -167,6 +176,12 @@ def load_library() -> ctypes.CDLL:
     L.ac_pipeline_predict_host.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]
     L.ac_pipeline_debug_copy.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     L.ac_profile_enable.argtypes = [c_int]
+    L.ac_tokenizer_create.argtypes = [POINTER(TokenizerSpec), POINTER(c_void_p)]
+    L.ac_tokenizer_destroy.argtypes = [c_void_p]
+    L.ac_tokenize_workspace_bytes.argtypes = [c_void_p, c_int, POINTER(c_size_t)]
+    L.ac_tokenize.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                              c_void_p]
+    L.ac_tokenize_pack.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     L.ac_pipeline_knn_stats.argtypes = [c_void_p, c_void_p, c_int, c_void_p]
     L.ac_profile_read.argtypes = [c_int, POINTER(ctypes.c_double), POINTER(ctypes.c_double), POINTER(ctypes.c_double),
                                   POINTER(ctypes.c_longlong)]
@@ -1220,6 +1235,104 @@ class Encoder:
     def close(self):
         if getattr(self, "handle", None):
             self._L.ac_encoder_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def tokenizer_spec_struct(spec: dict):
+    """(TokenizerSpec, arrays it points into) from tokenizer.wordpiece_spec's dict and the Unicode tables of its flags"""
+    import numpy as np
+    from .tokenizer import pack_strings, unicode_tables
+    norm, cls, pool = unicode_tables(*spec["flags"])
+    pool = pool if pool.size else np.zeros(1, dtype=np.uint32)
+    words = list(spec["vocab"])
+    vb, vo = pack_strings(words)
+    vi = np.asarray([spec["vocab"][w] for w in words], dtype=np.int32)
+    ab, ao = pack_strings([a for a, _ in spec["added"]])
+    ai = np.asarray([i for _, i in spec["added"]] or [0], dtype=np.int32)
+    keep = [norm, cls, pool, vb, vo, vi, ab, ao, ai]
+    p = [a.ctypes.data for a in keep]
+    st = TokenizerSpec(p[0], p[1], p[2], len(pool), p[3], p[4], p[5], len(words), p[6], p[7], p[8], len(spec["added"]),
+                       spec["prefix"], len(spec["prefix"]), spec["cls_id"], spec["sep_id"], spec["pad_id"], spec["unk_id"],
+                       spec["max_input_chars"])
+    return st, keep
+
+
+class WordPieceTokenizer:
+    """Owner of an ac_tokenizer handle: `tokenizer(texts, max_length=..., truncation=True, padding=True)` of a WordPiece
+    tokenizer of the BERT shape (tokenizer.wordpiece_spec), computed on the device with identical ids."""
+
+    def __init__(self, spec: dict, device="cuda"):
+        L = load_library()
+        self._L = L
+        self.device = torch.device(device)
+        self.type_ids = spec["type_ids"]
+        st, keep = tokenizer_spec_struct(spec)
+        h = c_void_p()
+        with torch.cuda.device(self.device):
+            check(L.ac_tokenizer_create(ctypes.byref(st), ctypes.byref(h)), "ac_tokenizer_create")
+        self.handle = h
+        del keep
+        self._host = torch.empty(0, dtype=torch.uint8).pin_memory()
+        self._dev = torch.empty(0, dtype=torch.uint8, device=self.device)
+        self._max_len_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+
+    @classmethod
+    def from_hf(cls, tokenizer, device="cuda"):
+        """(WordPieceTokenizer, "") for a supported tokenizer, else (None, the reason)"""
+        from .tokenizer import wordpiece_spec
+        spec, why = wordpiece_spec(tokenizer)
+        if spec is None:
+            return None, why
+        return cls(spec, device), ""
+
+    def __call__(self, texts, max_length: int):
+        """ids, mask, type_ids (None when the tokenizer emits none) [B, S] int32 on the device, S = the batch's longest; None
+        when a text has no UTF-8 form (a lone surrogate), which the caller leaves to the host tokenizer."""
+        try:
+            enc = [t.encode("utf-8") for t in texts]
+        except UnicodeEncodeError:
+            return None
+        B = len(enc)
+        lens = [len(e) for e in enc]
+        n_text = sum(lens)
+        head = (8 * (B + 1) + 255) // 256 * 256            # int64 offsets, then the bytes, in one pinned buffer / one H2D copy
+        total = head + n_text
+        if self._host.numel() < total:
+            self._host = torch.empty(int(total * 1.25) + 4096, dtype=torch.uint8).pin_memory()
+            self._dev = torch.empty(self._host.numel(), dtype=torch.uint8, device=self.device)
+        off = self._host[: 8 * (B + 1)].view(torch.int64)
+        off[0] = 0
+        torch.cumsum(torch.tensor(lens, dtype=torch.int64), 0, out=off[1:])
+        mv = memoryview(self._host.numpy())
+        mv[head:total] = b"".join(enc)
+        with torch.cuda.device(self.device):
+            self._dev[:total].copy_(self._host[:total], non_blocking=True)
+            tokens = torch.empty((B, max_length), dtype=torch.int32, device=self.device)
+            lengths = torch.empty(B + 1, dtype=torch.int32, device=self.device)
+            nb = c_size_t()
+            check(self._L.ac_tokenize_workspace_bytes(self.handle, B, ctypes.byref(nb)), "ac_tokenize_workspace_bytes")
+            ws = _workspace(nb.value, self.device)
+            check(self._L.ac_tokenize(self.handle, self._dev.data_ptr() + head, self._dev.data_ptr(), B, max_length,
+                                      tokens.data_ptr(), lengths.data_ptr(), lengths.data_ptr() + 4 * B, ws.data_ptr(),
+                                      ws.numel(), stream_ptr()), "ac_tokenize")
+            self._max_len_host.copy_(lengths[B:], non_blocking=False)     # the one readback: the encoder needs S at launch
+            S = int(self._max_len_host[0])
+            ids = torch.empty((B, S), dtype=torch.int32, device=self.device)
+            mask = torch.empty_like(ids)
+            tt = torch.empty_like(ids) if self.type_ids else None
+            check(self._L.ac_tokenize_pack(self.handle, tokens.data_ptr(), lengths.data_ptr(), B, max_length, S, ids.data_ptr(),
+                                           mask.data_ptr(), ptr(tt), stream_ptr()), "ac_tokenize_pack")
+        return ids, mask, tt
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self._L.ac_tokenizer_destroy(self.handle)
             self.handle = None
 
     def __del__(self):

@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libadaptive_b200.so")
-SOURCES = ["api.cu", "knn_exact.cu", "knn_tc.cu", "head.cu", "encoder.cu", "predict.cu", "strategic.cu"]
+SOURCES = ["api.cu", "knn_exact.cu", "knn_tc.cu", "head.cu", "encoder.cu", "predict.cu", "strategic.cu", "tokenizer.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

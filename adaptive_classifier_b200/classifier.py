@@ -73,6 +73,14 @@ class AdaptiveClassifier:
         self._max_tokens = int(self.config.config.get("b200_max_tokens", 65536))
         with torch.cuda.device(torch.device(self.device)):
             self.encoder = _cabi.Encoder.from_hf(hf, max_tokens=self._max_tokens, device=self.device)
+            # WordPiece tokenizers of the BERT shape run on the device with identical ids; every other one stays on the host,
+            # and so does one whose tables or handle cannot be built
+            try:
+                self.device_tokenizer, why = _cabi.WordPieceTokenizer.from_hf(self.tokenizer, device=self.device)
+            except (_cabi.AdaptiveB200Error, ValueError) as e:
+                self.device_tokenizer, why = None, f"building the device tokenizer failed: {e}"
+        if self.device_tokenizer is None:
+            logger.debug(f"tokenization stays on the host: {why}")
 
         self.embedding_dim = getattr(self.model.config, "hidden_size", None) or self.model.config.dim
         self.memory = PrototypeMemory(self.embedding_dim, config=self.config)
@@ -144,6 +152,12 @@ class AdaptiveClassifier:
             return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
 
     def _embed_device(self, texts: List[str]) -> torch.Tensor:
+        tok = getattr(self, "device_tokenizer", None)
+        if tok is not None and texts and self.config.max_length >= 2:
+            with self._device_lock, torch.cuda.device(torch.device(self.device)):
+                out = tok(texts, self.config.max_length)
+            if out is not None:
+                return self._embed_ids_device(*out)
         ids, mask, tt = self._tokenize(texts)
         return self._embed_ids_device(ids, mask, tt)
 

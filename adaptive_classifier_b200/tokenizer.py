@@ -1,0 +1,257 @@
+"""Which Hugging Face tokenizers the device WordPiece tokenizer (csrc/tokenizer.cu) reproduces, and the Unicode tables it runs on.
+
+The tables are derived by probing the installed `tokenizers` library (`normalize_str`, `pre_tokenize_str`), not from Python's
+`unicodedata`: the Rust crates behind `tokenizers` carry their own Unicode version, and what must match is the library the host
+path runs.  Needs no GPU.
+"""
+from __future__ import annotations
+
+import hashlib
+import json
+import logging
+import os
+import tempfile
+import unicodedata
+from typing import Optional, Tuple
+
+import numpy as np
+
+logger = logging.getLogger(__name__)
+
+N_CODEPOINTS = 0x110000
+IDENTITY, BLOCKER = 0x80000000, 0x40000000
+OTHER, SPACE, PUNCT = 0, 1, 2
+_SEP = "#"            # probe separator: a starter every BertNormalizer flag combination keeps, and no other expansion holds
+_ORDER_A, _ORDER_B = "\U0001D16D", "\U0001D165"   # non-spacing-mark-free combining marks, combining class 226 > 216
+
+_CACHE = {}
+
+
+def probe_codepoints() -> np.ndarray:
+    return np.concatenate([np.arange(0xD800), np.arange(0xE000, N_CODEPOINTS)])
+
+
+def pretokenizer_classes() -> np.ndarray:
+    """uint8 [N_CODEPOINTS]: the class BertPreTokenizer gives each codepoint (SPACE: split and dropped, PUNCT: a word of its
+    own, OTHER: part of a word).  Probed as one string of every codepoint: whitespace leaves its position uncovered by every
+    piece, and the one-char pieces (punctuation, or a word char between two splits) are probed again between letters."""
+    key = ("pre",)
+    if key in _CACHE:
+        return _CACHE[key]
+    from tokenizers import pre_tokenizers
+    pt = pre_tokenizers.BertPreTokenizer()
+    cps = probe_codepoints()
+    chars = list(map(chr, cps.tolist()))
+    covered = np.zeros(len(chars), dtype=np.uint8)
+    single = []
+    for _, (a, b) in pt.pre_tokenize_str("".join(chars)):
+        covered[a:b] = 1
+        if b - a == 1:
+            single.append(a)
+    for _, (a, b) in pt.pre_tokenize_str("a" + "a".join(chars[i] for i in single) + "a"):
+        if b - a == 1 and a % 2 == 1:
+            covered[single[a // 2]] = 2
+    cls = np.zeros(N_CODEPOINTS, dtype=np.uint8)
+    cls[cps] = np.where(covered == 0, SPACE, np.where(covered == 2, PUNCT, OTHER))
+    _CACHE[key] = cls
+    return cls
+
+
+def _normalize_each(normalizer, chars) -> list:
+    """normalizer.normalize_str of every string of `chars` on its own, in one library call"""
+    seps = [i for i, c in enumerate(chars) if _SEP in c]
+    rest = [c for c in chars if _SEP not in c]
+    out = normalizer.normalize_str(_SEP + _SEP.join(rest) + _SEP).split(_SEP)
+    assert len(out) == len(rest) + 2, "probe separator split"
+    out = out[1:-1]
+    for i in seps:
+        out.insert(i, normalizer.normalize_str(chars[i]))
+    return out
+
+
+def _reorder_ranks(nz, marks) -> dict:
+    """{mark: rank} for the codepoints of `marks` the library reorders against another one: the ranks 1, 2, ... order them
+    as the library's combining classes do, read from how many marks each one moves behind.  A candidate it never reorders against any other, in either
+    direction, is a starter to it and is left out (rank 0)."""
+    n = len(marks)
+    if n < 2:
+        return {}
+    pairs = [chr(a) + chr(b) for a in marks for b in marks]
+    swapped = np.array([o == p[::-1] != p for o, p in zip(_normalize_each(nz, pairs), pairs)], dtype=bool).reshape(n, n)
+    moved = swapped.any(axis=1) | swapped.any(axis=0)
+    below = swapped.sum(axis=1)                     # monotone in the class: equal classes move behind the same marks
+    dense = {v: r + 1 for r, v in enumerate(sorted(set(below[moved].tolist())))}
+    return {a: dense[int(below[i])] for i, a in enumerate(marks) if moved[i]}
+
+
+def _disk_cache_path(key) -> str:
+    """file of the tables for `key` under the user's cache directory; the name carries the tokenizers version, the flags and a
+    hash of this module, so a changed library or a changed probe never reads an old file"""
+    with open(__file__, "rb") as f:
+        src = hashlib.sha256(f.read()).hexdigest()[:16]
+    root = os.environ.get("XDG_CACHE_HOME") or os.path.join(os.path.expanduser("~"), ".cache")
+    name = "wordpiece-tables-" + "-".join(str(k) for k in key) + f"-{src}.npz"
+    return os.path.join(root, "adaptive_classifier_b200", name)
+
+
+def unicode_tables(clean_text: bool, handle_chinese_chars: bool, strip_accents: bool, lowercase: bool):
+    """(norm uint32 [N_CODEPOINTS], cls uint8 [N_CODEPOINTS], pool uint32 [*]) in the layout of ac_tokenizer_spec, for the
+    BertNormalizer with these flags (strip_accents resolved: None means lowercase).  Probing takes seconds, so the result is
+    kept per flags in the process and, when the user's cache directory is writable, on disk."""
+    import tokenizers
+    key = (tokenizers.__version__, clean_text, handle_chinese_chars, strip_accents, lowercase)
+    if key in _CACHE:
+        return _CACHE[key]
+    path = _disk_cache_path(key)
+    try:
+        with np.load(path) as z:
+            res = (z["norm"], z["cls"], z["pool"])
+    except (OSError, KeyError, ValueError):
+        res = _probe_tables(*key[1:])
+        try:
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+            fd, tmp = tempfile.mkstemp(dir=os.path.dirname(path), suffix=".npz")
+            with os.fdopen(fd, "wb") as f:
+                np.savez(f, norm=res[0], cls=res[1], pool=res[2])
+            os.replace(tmp, path)                      # whole files only: concurrent processes may build the same tables
+        except OSError as e:
+            logger.debug(f"tokenizer tables not cached on disk: {e}")
+    _CACHE[key] = res
+    return res
+
+
+def _probe_tables(clean_text: bool, handle_chinese_chars: bool, strip_accents: bool, lowercase: bool):
+    from tokenizers import normalizers
+    nz = normalizers.BertNormalizer(clean_text=clean_text, handle_chinese_chars=handle_chinese_chars,
+                                    strip_accents=strip_accents, lowercase=lowercase)
+    cps = probe_codepoints()
+    chars = list(map(chr, cps.tolist()))
+    exp = _normalize_each(nz, chars)
+    norm = np.zeros(N_CODEPOINTS, dtype=np.uint32)
+    same = np.fromiter((e == c for e, c in zip(exp, chars)), dtype=bool, count=len(chars))
+    norm[cps[same]] = IDENTITY
+    pool, empty = [], []
+    for c, e in zip(cps[~same].tolist(), [e for e, s in zip(exp, same) if not s]):
+        if len(e) >= 32:
+            raise ValueError(f"U+{c:04X} expands to {len(e)} codepoints")
+        norm[c] = (len(pool) << 5) | len(e)
+        pool.extend(map(ord, e))
+        if not e:
+            empty.append(c)
+    cls = pretokenizer_classes().copy()
+    if strip_accents:
+        # canonical ordering: NFD sorts each run of marks by combining class before the non-spacing marks are removed.  The
+        # classes are the library's (its Unicode version need not be Python's), read from how it orders pairs of surviving
+        # codepoints; unicodedata only proposes the candidates
+        survivors = set(cps[same].tolist())
+        if any(unicodedata.combining(chr(c)) for c in set(pool) - survivors):
+            raise ValueError("a mark that only occurs inside expansions cannot be ordered by probing")
+        marks = sorted(c for c in survivors if unicodedata.combining(chr(c)))
+        ranks = _reorder_ranks(nz, marks)
+        if ranks:
+            # codepoints Python does not know yet may be marks to the library: probe them against its lowest- and
+            # highest-ranked marks (one of the two pairs reorders for any nonzero class)
+            lo = min(ranks, key=ranks.get)
+            hi = max(ranks, key=ranks.get)
+            kept = cps[same]
+            kept = kept[(kept < 0x40000) | ((kept >= 0xE0000) & (kept < 0xF0000))].tolist()
+            new = [c for c in kept if unicodedata.category(chr(c)) == "Cn"]
+            probes = _normalize_each(nz, [chr(hi) + chr(c) for c in new] + [chr(c) + chr(lo) for c in new])
+            found = [c for i, c in enumerate(new) if probes[i] == chr(c) + chr(hi) or probes[len(new) + i] == chr(lo) + chr(c)]
+            logger.debug(f"{len(found)} marks unknown to unicodedata")
+            if found:
+                ranks = _reorder_ranks(nz, sorted(set(marks) | set(found)))
+        for a, rank in ranks.items():
+            if rank > 63:
+                raise ValueError("more than 63 canonical-ordering ranks")
+            cls[a] |= rank << 2
+        # a removed codepoint between two marks either lets them reorder (removed before NFD, or a mark of nonzero class)
+        # or blocks them (a removed mark of class 0).  Control, format and private-use codepoints are removed by clean_text
+        # before NFD runs, so only the others are probed
+        empty = [c for c in empty if unicodedata.category(chr(c)) not in ("Cc", "Cf", "Co")] if clean_text else empty
+        if empty and _normalize_each(nz, [_ORDER_A + _ORDER_B]) == [_ORDER_B + _ORDER_A]:
+            probes = _normalize_each(nz, [_ORDER_A + chr(c) + _ORDER_B for c in empty])
+            norm[[c for c, o in zip(empty, probes) if o != _ORDER_B + _ORDER_A]] |= BLOCKER
+    return norm, cls, np.asarray(pool, dtype=np.uint32)
+
+
+_REPRESENTATIVE = ["Hello World", "  déjà vu, NAÏVE café!  ", "中文字符 and 𠀀", "İstanbul ΣΟΦΟΣ", "a\tb\nc d　e",
+                   "tab\x00null�", "emoji 👩‍👩‍👧 $5+<3>", "x" * 120]
+
+
+def wordpiece_spec(tokenizer) -> Tuple[Optional[dict], str]:
+    """(spec, "") when the tokenizer is one the device kernel reproduces id for id, else (None, reason).  The decision is read
+    from `backend_tokenizer.to_str()`, the pipeline that actually runs, and accepts nothing looser than:
+    WordPiece model, BertNormalizer, BertPreTokenizer, a single-sequence post-processor "[special] A [special]" with type id 0,
+    right truncation and padding, added tokens with normalized = false and single_word = false, and a Python wrapper that
+    passes the text through unchanged."""
+    bt = getattr(tokenizer, "backend_tokenizer", None)
+    if bt is None:
+        return None, "no Rust `tokenizers` backend (slow tokenizer)"
+    j = json.loads(bt.to_str())
+    model, nrm, pre, post = j.get("model") or {}, j.get("normalizer") or {}, j.get("pre_tokenizer") or {}, j.get("post_processor") or {}
+    if model.get("type") != "WordPiece":
+        return None, f"model {model.get('type')!r} is not WordPiece"
+    if nrm.get("type") != "BertNormalizer":
+        return None, f"normalizer {nrm.get('type')!r} is not BertNormalizer"
+    if pre.get("type") != "BertPreTokenizer":
+        return None, f"pre_tokenizer {pre.get('type')!r} is not BertPreTokenizer"
+    vocab = model["vocab"]
+    pt = post.get("type")
+    if pt == "TemplateProcessing":
+        single = post.get("single") or []
+        kinds = [next(iter(x)) for x in single]
+        if kinds != ["SpecialToken", "Sequence", "SpecialToken"] or any(next(iter(x.values())).get("type_id", 0) for x in single):
+            return None, "post-processor template is not '[special] A [special]' with type id 0"
+        ids = []
+        for x in (single[0], single[2]):
+            st = post["special_tokens"].get(x["SpecialToken"]["id"], {})
+            if len(st.get("ids", [])) != 1:
+                return None, "post-processor special token with more than one id"
+            ids.append(st["ids"][0])
+        cls_id, sep_id = ids
+    elif pt in ("BertProcessing", "RobertaProcessing"):
+        cls_id, sep_id = post["cls"][1], post["sep"][1]
+    else:
+        return None, f"post_processor {pt!r} is not TemplateProcessing / BertProcessing / RobertaProcessing"
+    if getattr(tokenizer, "truncation_side", "right") != "right" or getattr(tokenizer, "padding_side", "right") != "right":
+        return None, "left truncation or left padding"
+    added = j.get("added_tokens") or []
+    for a in added:
+        if a.get("normalized", True) or a.get("single_word", False):
+            return None, f"added token {a.get('content')!r} with normalized={a.get('normalized')} single_word={a.get('single_word')}"
+    if "" in vocab:
+        return None, "the vocab has an empty entry"
+    unk = model.get("unk_token")
+    if unk not in vocab:
+        return None, f"unk_token {unk!r} is not in the vocab"
+    prefix = model.get("continuing_subword_prefix", "##").encode("utf-8")
+    if len(prefix) > 16:
+        return None, "continuing_subword_prefix longer than 16 bytes"
+    if tokenizer.pad_token_id is None:
+        return None, "no pad token"
+    try:
+        # the transformers wrapper must hand the text to the backend unchanged
+        wrapped = tokenizer(_REPRESENTATIVE)["input_ids"]
+        backend = [e.ids for e in bt.encode_batch(_REPRESENTATIVE)]
+    except Exception as e:                       # noqa: BLE001 -- any failure means: not a shape we reproduce
+        return None, f"probe encoding failed: {e}"
+    if wrapped != backend:
+        return None, "the Python wrapper changes the text before the backend sees it"
+    strip = nrm.get("strip_accents")
+    lower = bool(nrm.get("lowercase", True))
+    spec = dict(vocab=vocab, added=[(a["content"], a["id"]) for a in added], prefix=prefix,
+                cls_id=int(cls_id), sep_id=int(sep_id), pad_id=int(tokenizer.pad_token_id), unk_id=int(vocab[unk]),
+                max_input_chars=int(model.get("max_input_chars_per_word", 100)),
+                flags=(bool(nrm.get("clean_text", True)), bool(nrm.get("handle_chinese_chars", True)),
+                       lower if strip is None else bool(strip), lower),
+                type_ids="token_type_ids" in getattr(tokenizer, "model_input_names", ()))
+    return spec, ""
+
+
+def pack_strings(strings) -> Tuple[np.ndarray, np.ndarray]:
+    """UTF-8 bytes of the strings back to back, and int64 offsets [n + 1]"""
+    enc = [s.encode("utf-8") for s in strings]
+    off = np.zeros(len(enc) + 1, dtype=np.int64)
+    np.cumsum([len(e) for e in enc], out=off[1:])
+    return np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8), off

@@ -410,6 +410,58 @@ int ac_linear_tc(const void *X, const void *W, const float *bias, const float *r
                  int M, int N, int K, int epi, int round_out, int precision, int out_half, ac_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Stage T -- tokenization.  Replaces `self.tokenizer(texts, max_length=..., truncation=True, padding=True)` at
+ *   src/adaptive_classifier/classifier.py:1259-1265 for WordPiece tokenizers of the BERT shape: BertNormalizer,
+ *   BertPreTokenizer, WordPiece, post-processor "[special] A [special]", right truncation and padding, added tokens with
+ *   normalized = false and single_word = false.  Which tokenizers qualify, and the tables below, are decided and built by
+ *   adaptive_classifier_b200/tokenizer.py from the installed `tokenizers` library.
+ * ------------------------------------------------------------------------------------------ */
+#define AC_TOKENIZER_CODEPOINTS 0x110000
+
+typedef struct {
+    /* HOST tables over every codepoint c < AC_TOKENIZER_CODEPOINTS:
+       norm[c]: bit 31 set = c normalizes to itself; else bits 5..29 = offset into pool and bits 0..4 = length of its normalized
+                expansion (bit 30 on an empty expansion: canonical ordering does not cross it);
+       cls[c]:  bits 0-1 the pre-tokenizer class of c as a normalized char (0 other, 1 whitespace, 2 punctuation), bits 2-7 its
+                rank in canonical ordering (0 for starters; marks of lower rank move before marks of higher rank) */
+    const uint32_t *norm;
+    const uint8_t *cls;
+    const uint32_t *pool;
+    int64_t pool_len;
+    /* vocab entry v: the bytes vocab_bytes[vocab_offsets[v] .. vocab_offsets[v + 1]) with id vocab_ids[v] */
+    const uint8_t *vocab_bytes;
+    const int64_t *vocab_offsets;
+    const int32_t *vocab_ids;
+    int n_vocab;
+    /* added tokens matched on the raw text (leftmost, then longest), same layout */
+    const uint8_t *added_bytes;
+    const int64_t *added_offsets;
+    const int32_t *added_ids;
+    int n_added;
+    const char *prefix;          /* continuing_subword_prefix, <= 16 bytes, not NUL-terminated */
+    int prefix_len;
+    int cls_id, sep_id, pad_id, unk_id;   /* first and last special token of the template, padding, WordPiece unk_token */
+    int max_input_chars;         /* WordPiece max_input_chars_per_word: longer words (in chars) are unk_id */
+} ac_tokenizer_spec;
+
+typedef struct ac_tokenizer ac_tokenizer;
+/* copies the tables and builds the vocab's hash table on the device */
+int ac_tokenizer_create(const ac_tokenizer_spec *spec, ac_tokenizer **out);
+int ac_tokenizer_destroy(ac_tokenizer *tok);
+/* bytes of workspace ac_tokenize needs for B texts */
+int ac_tokenize_workspace_bytes(const ac_tokenizer *tok, int B, size_t *bytes);
+/* text: UTF-8 bytes of B >= 1 texts, text i = text[offsets[i] .. offsets[i + 1]) (offsets int64[B + 1], nondecreasing, within
+ * the buffer).  Ids equal the library's for valid UTF-8; an invalid byte is read as U+FFFD, and no text is read past its end.
+ * tokens[B, max_length]: row i starts with the lengths[i] ids of text i, [CLS] pieces [SEP] truncated to max_length >= 2; *max_len = max lengths[i].
+ * Every pointer is DEVICE; nothing synchronises. */
+int ac_tokenize(const ac_tokenizer *tok, const uint8_t *text, const int64_t *offsets, int B, int max_length, int32_t *tokens,
+                int32_t *lengths, int32_t *max_len, void *workspace, size_t workspace_bytes, ac_stream_t stream);
+/* ids / mask / type_ids (nullable) [B, S], S <= max_length (the batch's longest, read back by the caller): the first lengths[i]
+ * tokens of row i, then the pad id with mask 0; type ids 0.  DEVICE pointers. */
+int ac_tokenize_pack(const ac_tokenizer *tok, const int32_t *tokens, const int32_t *lengths, int B, int max_length, int S,
+                     int32_t *ids, int32_t *mask, int32_t *type_ids, ac_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * predict_batch() glue on the device (classifier.py:1329-1384) and the end-to-end pipeline.
  * ------------------------------------------------------------------------------------------ */
 
