@@ -48,6 +48,7 @@ EXPORTS = [
     "ac_pipeline_encode", "ac_pipeline_embeddings", "ac_pipeline_search_shard", "ac_pipeline_finish_sharded",
     "ac_pipeline_debug_copy", "ac_pipeline_knn_stats", "ac_launch_count", "ac_profile_enable", "ac_profile_read",
     "ac_tokenizer_create", "ac_tokenizer_destroy", "ac_tokenize_workspace_bytes", "ac_tokenize", "ac_tokenize_pack",
+    "ac_tokenizer_create_bpe", "ac_tokenize_workspace_bytes_text",
 ]
 
 
@@ -95,6 +96,14 @@ class TokenizerSpec(Structure):
                 ("added_bytes", c_void_p), ("added_offsets", c_void_p), ("added_ids", c_void_p), ("n_added", c_int),
                 ("prefix", c_char_p), ("prefix_len", c_int),
                 ("cls_id", c_int), ("sep_id", c_int), ("pad_id", c_int), ("unk_id", c_int), ("max_input_chars", c_int)]
+
+
+class BPETokenizerSpec(Structure):
+    _fields_ = [("cls", c_void_p), ("split", c_int), ("add_prefix_space", c_int), ("ignore_merges", c_int),
+                ("vocab_bytes", c_void_p), ("vocab_offsets", c_void_p), ("vocab_ids", c_void_p), ("n_vocab", c_int),
+                ("byte_ids", c_void_p), ("merges", c_void_p), ("n_merges", c_int),
+                ("added_bytes", c_void_p), ("added_offsets", c_void_p), ("added_ids", c_void_p), ("added_flags", c_void_p),
+                ("n_added", c_int), ("cls_id", c_int), ("sep_id", c_int), ("pad_id", c_int)]
 
 
 class EncoderWeights(Structure):
@@ -182,6 +191,8 @@ def load_library() -> ctypes.CDLL:
     L.ac_tokenize.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                               c_void_p]
     L.ac_tokenize_pack.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.ac_tokenizer_create_bpe.argtypes = [POINTER(BPETokenizerSpec), POINTER(c_void_p)]
+    L.ac_tokenize_workspace_bytes_text.argtypes = [c_void_p, c_int, c_int64, c_int, POINTER(c_size_t)]
     L.ac_pipeline_knn_stats.argtypes = [c_void_p, c_void_p, c_int, c_void_p]
     L.ac_profile_read.argtypes = [c_int, POINTER(ctypes.c_double), POINTER(ctypes.c_double), POINTER(ctypes.c_double),
                                   POINTER(ctypes.c_longlong)]
@@ -1263,33 +1274,53 @@ def tokenizer_spec_struct(spec: dict):
     return st, keep
 
 
-class WordPieceTokenizer:
-    """Owner of an ac_tokenizer handle: `tokenizer(texts, max_length=..., truncation=True, padding=True)` of a WordPiece
-    tokenizer of the BERT shape (tokenizer.wordpiece_spec), computed on the device with identical ids."""
+def bpe_spec_struct(spec: dict):
+    """(BPETokenizerSpec, arrays it points into) from tokenizer.bpe_spec's dict and the codepoint classes"""
+    import numpy as np
+    from .tokenizer import bpe_classes, bpe_vocab_bytes, pack_strings
+    cls = bpe_classes()
+    words, wids = bpe_vocab_bytes(spec["vocab"])
+    vo = np.zeros(len(words) + 1, dtype=np.int64)
+    np.cumsum([len(w) for w in words], out=vo[1:])
+    vb = np.frombuffer(b"".join(words) or b"\0", dtype=np.uint8)
+    vi = np.asarray(wids, dtype=np.int32)
+    bi = np.asarray(spec["byte_ids"], dtype=np.int32)
+    mg = np.asarray(spec["merges"] or [(0, 0, 0)], dtype=np.int32).reshape(-1, 3)
+    added = spec["added"]
+    ab, ao = pack_strings([a[0] for a in added])
+    ai = np.asarray([a[1] for a in added] or [0], dtype=np.int32)
+    af = np.asarray([a[2] | a[3] << 1 | a[4] << 2 for a in added] or [0], dtype=np.uint8)
+    keep = [cls, vb, vo, vi, bi, mg, ab, ao, ai, af]
+    p = [a.ctypes.data for a in keep]
+    st = BPETokenizerSpec(p[0], spec["split"], int(spec["prefix_space"]), int(spec["ignore_merges"]), p[1], p[2], p[3],
+                          len(words), p[4], p[5], len(spec["merges"]), p[6], p[7], p[8], p[9], len(added),
+                          spec["cls_id"], spec["sep_id"], spec["pad_id"])
+    return st, keep
 
-    def __init__(self, spec: dict, device="cuda"):
-        L = load_library()
-        self._L = L
+
+class _DeviceTokenizer:
+    """What both device tokenizers share: the handle, one pinned H2D copy of the texts' offsets and bytes, the one readback of
+    the batch's longest row, and the pack into [B, S] tensors."""
+    _readback = 1                                   # int32 the call reads back: the longest row (BPE: and the texts left)
+
+    def _create(self, create, st, type_ids: bool, device):
+        self._L = load_library()
         self.device = torch.device(device)
-        self.type_ids = spec["type_ids"]
-        st, keep = tokenizer_spec_struct(spec)
+        self.type_ids = type_ids
         h = c_void_p()
         with torch.cuda.device(self.device):
-            check(L.ac_tokenizer_create(ctypes.byref(st), ctypes.byref(h)), "ac_tokenizer_create")
+            check(create(ctypes.byref(st), ctypes.byref(h)), create.__name__)
         self.handle = h
-        del keep
         self._host = torch.empty(0, dtype=torch.uint8).pin_memory()
         self._dev = torch.empty(0, dtype=torch.uint8, device=self.device)
-        self._max_len_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self._max_len_host = torch.zeros(self._readback, dtype=torch.int32).pin_memory()
 
-    @classmethod
-    def from_hf(cls, tokenizer, device="cuda"):
-        """(WordPieceTokenizer, "") for a supported tokenizer, else (None, the reason)"""
-        from .tokenizer import wordpiece_spec
-        spec, why = wordpiece_spec(tokenizer)
-        if spec is None:
-            return None, why
-        return cls(spec, device), ""
+    def _workspace_bytes(self, B: int, n_text: int, max_length: int) -> int:
+        raise NotImplementedError
+
+    def _left_rows(self, texts, max_length, tokens, lengths) -> int:
+        """rows of the texts the kernels left to the host (BPE); returns their longest length"""
+        return 0
 
     def __call__(self, texts, max_length: int):
         """ids, mask, type_ids (None when the tokenizer emits none) [B, S] int32 on the device, S = the batch's longest; None
@@ -1314,15 +1345,15 @@ class WordPieceTokenizer:
         with torch.cuda.device(self.device):
             self._dev[:total].copy_(self._host[:total], non_blocking=True)
             tokens = torch.empty((B, max_length), dtype=torch.int32, device=self.device)
-            lengths = torch.empty(B + 1, dtype=torch.int32, device=self.device)
-            nb = c_size_t()
-            check(self._L.ac_tokenize_workspace_bytes(self.handle, B, ctypes.byref(nb)), "ac_tokenize_workspace_bytes")
-            ws = _workspace(nb.value, self.device)
+            lengths = torch.empty(B + self._readback, dtype=torch.int32, device=self.device)
+            ws = _workspace(self._workspace_bytes(B, n_text, max_length), self.device)
             check(self._L.ac_tokenize(self.handle, self._dev.data_ptr() + head, self._dev.data_ptr(), B, max_length,
                                       tokens.data_ptr(), lengths.data_ptr(), lengths.data_ptr() + 4 * B, ws.data_ptr(),
                                       ws.numel(), stream_ptr()), "ac_tokenize")
             self._max_len_host.copy_(lengths[B:], non_blocking=False)     # the one readback: the encoder needs S at launch
             S = int(self._max_len_host[0])
+            if self._readback > 1 and int(self._max_len_host[1]):
+                S = max(S, self._left_rows(texts, max_length, tokens, lengths))
             ids = torch.empty((B, S), dtype=torch.int32, device=self.device)
             mask = torch.empty_like(ids)
             tt = torch.empty_like(ids) if self.type_ids else None
@@ -1340,6 +1371,69 @@ class WordPieceTokenizer:
             self.close()
         except Exception:
             pass
+
+
+class WordPieceTokenizer(_DeviceTokenizer):
+    """Owner of an ac_tokenizer handle: `tokenizer(texts, max_length=..., truncation=True, padding=True)` of a WordPiece
+    tokenizer of the BERT shape (tokenizer.wordpiece_spec), computed on the device with identical ids."""
+
+    def __init__(self, spec: dict, device="cuda"):
+        st, keep = tokenizer_spec_struct(spec)
+        self._create(load_library().ac_tokenizer_create, st, spec["type_ids"], device)
+        del keep
+
+    @classmethod
+    def from_hf(cls, tokenizer, device="cuda"):
+        """(WordPieceTokenizer, "") for a supported tokenizer, else (None, the reason)"""
+        from .tokenizer import wordpiece_spec
+        spec, why = wordpiece_spec(tokenizer)
+        if spec is None:
+            return None, why
+        return cls(spec, device), ""
+
+    def _workspace_bytes(self, B: int, n_text: int, max_length: int) -> int:
+        nb = c_size_t()
+        check(self._L.ac_tokenize_workspace_bytes(self.handle, B, ctypes.byref(nb)), "ac_tokenize_workspace_bytes")
+        return nb.value
+
+
+class BPETokenizer(_DeviceTokenizer):
+    """Owner of an ac_tokenizer handle of a byte-level BPE tokenizer (RoBERTa, ModernBERT, EuroBERT; tokenizer.bpe_spec):
+    `tokenizer(texts, max_length=..., truncation=True, padding=True)` computed on the device with identical ids.  A text with
+    a kept word longer than AC_BPE_MAX_WORD bytes is tokenized by `tokenizer` itself, on the host."""
+    _readback = 2
+
+    def __init__(self, spec: dict, tokenizer, device="cuda"):
+        st, keep = bpe_spec_struct(spec)
+        self._create(load_library().ac_tokenizer_create_bpe, st, spec["type_ids"], device)
+        del keep
+        self._hf = tokenizer
+
+    @classmethod
+    def from_hf(cls, tokenizer, device="cuda"):
+        """(BPETokenizer, "") for a supported tokenizer, else (None, the reason)"""
+        from .tokenizer import bpe_spec
+        spec, why = bpe_spec(tokenizer)
+        if spec is None:
+            return None, why
+        return cls(spec, tokenizer, device), ""
+
+    def _workspace_bytes(self, B: int, n_text: int, max_length: int) -> int:
+        nb = c_size_t()
+        check(self._L.ac_tokenize_workspace_bytes_text(self.handle, B, n_text, max_length, ctypes.byref(nb)),
+              "ac_tokenize_workspace_bytes_text")
+        return nb.value
+
+    def _left_rows(self, texts, max_length, tokens, lengths) -> int:
+        left = torch.nonzero(lengths[: len(texts)].cpu() < 0).flatten().tolist()
+        rows = self._hf([texts[i] for i in left], max_length=max_length, truncation=True)["input_ids"]
+        host = torch.zeros((len(left), max_length), dtype=torch.int32)
+        for r, ids in enumerate(rows):
+            host[r, : len(ids)] = torch.tensor(ids, dtype=torch.int32)
+        idx = torch.tensor(left, dtype=torch.int64, device=self.device)
+        tokens[idx] = host.to(self.device)
+        lengths[idx] = torch.tensor([len(r) for r in rows], dtype=torch.int32).to(self.device)
+        return max(len(r) for r in rows)
 
 
 def proto_class_scores(d, idx, row_class=None, n_classes: Optional[int] = None):

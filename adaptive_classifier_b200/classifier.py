@@ -73,14 +73,20 @@ class AdaptiveClassifier:
         self._max_tokens = int(self.config.config.get("b200_max_tokens", 65536))
         with torch.cuda.device(torch.device(self.device)):
             self.encoder = _cabi.Encoder.from_hf(hf, max_tokens=self._max_tokens, device=self.device)
-            # WordPiece tokenizers of the BERT shape run on the device with identical ids; every other one stays on the host,
-            # and so does one whose tables or handle cannot be built
-            try:
-                self.device_tokenizer, why = _cabi.WordPieceTokenizer.from_hf(self.tokenizer, device=self.device)
-            except (_cabi.AdaptiveB200Error, ValueError) as e:
-                self.device_tokenizer, why = None, f"building the device tokenizer failed: {e}"
+            # WordPiece tokenizers of the BERT shape and byte-level BPE tokenizers (RoBERTa, ModernBERT, EuroBERT) run on the
+            # device with identical ids; every other one stays on the host, and so does one whose tables or handle cannot be built
+            whys = []
+            self.device_tokenizer = None
+            for kind in (_cabi.WordPieceTokenizer, _cabi.BPETokenizer):
+                try:
+                    self.device_tokenizer, why = kind.from_hf(self.tokenizer, device=self.device)
+                except (_cabi.AdaptiveB200Error, ValueError) as e:
+                    self.device_tokenizer, why = None, f"building the device tokenizer failed: {e}"
+                if self.device_tokenizer is not None:
+                    break
+                whys.append(f"{kind.__name__}: {why}")
         if self.device_tokenizer is None:
-            logger.debug(f"tokenization stays on the host: {why}")
+            logger.debug(f"tokenization stays on the host: {'; '.join(whys)}")
 
         self.embedding_dim = getattr(self.model.config, "hidden_size", None) or self.model.config.dim
         self.memory = PrototypeMemory(self.embedding_dim, config=self.config)

@@ -7,6 +7,9 @@
 // pre-tokenizer class (table), and each finished word is cut by greedy longest-match WordPiece against an open-addressing hash
 // table of the vocab.  The walk stops once max_length - 2 tokens exist: later words cannot change the kept ids.
 //
+// Byte-level BPE tokenizers (RoBERTa, ModernBERT, EuroBERT) run on three kernels further down, sharing the UTF-8 decoding,
+// the handle, the uploads and tokenize_pack_kernel with WordPiece.
+//
 // The file is plain SIMT C++: with AC_CPU_SHIM defined (tests/cpu_shim) only the kernels and the host-side table builder are
 // compiled, so the control flow runs on the CPU as well.
 #ifndef AC_CPU_SHIM
@@ -254,6 +257,31 @@ struct HostTables {
     Tables t{};                     // scalars, prefix and first_byte filled; pointers left to the owner
 };
 
+// the open-addressing table (id, FNV-1a hash, byte offset, byte length) of n byte strings, load factor <= 1/2 so that every
+// probe chain ends; returns nullptr, or what is wrong with the strings
+inline const char *hash_byte_strings(const uint8_t *bytes, const int64_t *offsets, const int32_t *ids, int n,
+                                     std::vector<int4> &slots, int &max_key) {
+    size_t n_slots = 2;
+    while (n_slots < 2 * static_cast<size_t>(n)) n_slots <<= 1;
+    slots.assign(n_slots, int4{-1, 0, 0, 0});
+    max_key = 0;
+    for (int v = 0; v < n; ++v) {
+        const int64_t o0 = offsets[v], len = offsets[v + 1] - o0;
+        if (len <= 0 || o0 + len > INT32_MAX) return "empty vocab entry or vocab bytes over 2 GB";
+        const uint32_t hash = fnv1a(kFnvBasis, bytes + o0, static_cast<int>(len));
+        size_t i = hash & (n_slots - 1);
+        while (slots[i].x >= 0) {
+            const int4 &e = slots[i];
+            if (e.w == len && !memcmp(bytes + e.z, bytes + o0, len)) return "duplicate vocab entry";
+            i = (i + 1) & (n_slots - 1);
+        }
+        if (ids[v] < 0) return "negative vocab id";
+        slots[i] = int4{ids[v], static_cast<int>(hash), static_cast<int>(o0), static_cast<int>(len)};
+        max_key = std::max<int>(max_key, static_cast<int>(len));
+    }
+    return nullptr;
+}
+
 // returns nullptr, or what is wrong with the spec
 inline const char *build_host_tables(const ac_tokenizer_spec &s, HostTables &h) {
     if (!s.norm || !s.cls || (s.pool_len && !s.pool) || !s.vocab_bytes || !s.vocab_offsets || !s.vocab_ids || s.n_vocab <= 0)
@@ -262,24 +290,9 @@ inline const char *build_host_tables(const ac_tokenizer_spec &s, HostTables &h) 
     if (s.max_input_chars < 1) return "max_input_chars_per_word < 1";
     if (s.n_added < 0 || (s.n_added && (!s.added_bytes || !s.added_offsets || !s.added_ids))) return "bad added tokens";
     if (s.pool_len > (kOffsetMask >> 5)) return "expansion pool too large";
-    size_t n_slots = 2;
-    while (n_slots < 2 * static_cast<size_t>(s.n_vocab)) n_slots <<= 1;      // load factor <= 1/2: every probe chain ends
-    h.slots.assign(n_slots, int4{-1, 0, 0, 0});
     int max_key = 0;
-    for (int v = 0; v < s.n_vocab; ++v) {
-        const int64_t o0 = s.vocab_offsets[v], n = s.vocab_offsets[v + 1] - o0;
-        if (n <= 0 || o0 + n > INT32_MAX) return "empty vocab entry or vocab bytes over 2 GB";
-        const uint32_t hash = fnv1a(kFnvBasis, s.vocab_bytes + o0, static_cast<int>(n));
-        size_t i = hash & (n_slots - 1);
-        while (h.slots[i].x >= 0) {
-            const int4 &e = h.slots[i];
-            if (e.w == n && !memcmp(s.vocab_bytes + e.z, s.vocab_bytes + o0, n)) return "duplicate vocab entry";
-            i = (i + 1) & (n_slots - 1);
-        }
-        if (s.vocab_ids[v] < 0) return "negative vocab id";
-        h.slots[i] = int4{s.vocab_ids[v], static_cast<int>(hash), static_cast<int>(o0), static_cast<int>(n)};
-        max_key = std::max<int>(max_key, static_cast<int>(n));
-    }
+    if (const char *why = hash_byte_strings(s.vocab_bytes, s.vocab_offsets, s.vocab_ids, s.n_vocab, h.slots, max_key)) return why;
+    const size_t n_slots = h.slots.size();
     std::vector<int> order(s.n_added);
     for (int a = 0; a < s.n_added; ++a) {
         order[a] = a;
@@ -314,14 +327,513 @@ inline const char *build_host_tables(const ac_tokenizer_spec &s, HostTables &h) 
 
 inline size_t workspace_bytes(int max_chars, int B) { return static_cast<size_t>(B) * (max_chars + 1) * 8 + 256; }
 
+// ================================================================ byte-level BPE (RoBERTa, ModernBERT, EuroBERT)
+// Three kernels.  split: one thread per text matches the added tokens (normalized = false on the raw text, then
+// normalized = true inside the gaps), runs the split pattern over each remaining gap and records up to max_length - 2 entries:
+// an added token, or a word (a byte span, with ByteLevel's prefix space in front).  merge: one thread per word of the whole
+// batch runs the library's BPE (lowest rank first, leftmost on ties) with a binary heap, O(n log n) in the word's bytes.
+// gather: one warp per text lays the entries' tokens out as [CLS] tokens [SEP], truncated to max_length.  Every word yields
+// at least one token (the vocab holds all 256 byte symbols), so max_length - 2 entries are all the kept words.
+//
+// A word longer than kMaxWord bytes is not merged on the device: its text is left to the caller (lengths = -1, and
+// max_len[1] = 1), which tokenizes it on the host.  One GPU thread would otherwise run for a long time on one word.
+constexpr int kMaxWord = AC_BPE_MAX_WORD;
+enum { kSplitGpt2 = 0, kSplitLlama3 = 1 };
+// bpe class bits of a codepoint (tokenizer.bpe_classes): \p{L}, \p{N}, \s of the library's regex engine, Rust whitespace
+// (lstrip / rstrip); bits 4-7 the contraction letter it matches case-insensitively (1..8 = s t r e v m l d)
+enum { kL = 1, kN = 2, kS = 4, kRust = 8 };
+enum { kFoldS = 1, kFoldT, kFoldR, kFoldE, kFoldV, kFoldM, kFoldL, kFoldD };
+// added-token trie node terminal codes: (added index << 2) | lstrip << 1 | rstrip, or -1
+struct BpeTables {
+    const uint8_t *cls;
+    const int4 *merges;         // (left id, right id, rank, merged id); left < 0: empty
+    uint32_t merge_mask;
+    const int4 *words;          // ignore_merges: the model vocab over raw bytes, (id, hash, byte offset, byte length)
+    uint32_t word_mask;
+    const uint8_t *word_bytes;
+    const int2 *edges;          // added-token trie edges: (node << 8 | byte, child); key < 0: empty
+    uint32_t edge_mask;
+    const int2 *term;           // per trie node: terminal code of the raw pass, of the normalized pass
+    const int32_t *added_id;
+    uint32_t first_byte[2][8];  // bit set: a token of the raw / normalized pass starts with this byte
+    int n_pass[2];              // added tokens in each pass
+    int byte_id[256];
+    int split, prefix_space, ignore_merges;
+    int cls_id, sep_id, pad_id;
+};
+
+// one gap's view of the text: bytes [a, b) relative to the text, with ByteLevel's prefix space as byte a - 1 when vp
+struct Gap {
+    const uint8_t *p;
+    int64_t a, b;
+    bool vp;
+};
+
+__device__ inline int gap_decode(const Gap &g, int64_t i, uint32_t &c) {
+    if (i < g.a) { c = ' '; return 1; }
+    return utf8_decode(g.p + i, g.p + g.b, c);
+}
+
+// a text's slots: slot 1 + j belongs to byte j, slot 0 to the prefix space of a word at byte 0; a word's tokens are written
+// over its slots from its first one
+struct Entries {
+    int2 *e;                    // a word: (first slot, (bytes << 1) | vp); after the merge (first slot, -tokens).  (id, 0): an added token
+    int n, limit;
+    int64_t slots;              // slots the workspace holds for this text
+    bool huge;                  // a kept word is longer than kMaxWord
+};
+
+__device__ inline void emit_word(Entries &o, const Gap &g, int64_t i, int64_t j) {
+    if (o.n >= o.limit) return;
+    if (j - i > kMaxWord) { o.huge = true; return; }
+    const bool vp = i < g.a;
+    const int64_t slot = i + 1;              // the prefix space is byte a - 1: its slot belongs to the token before the gap
+    o.e[o.n++] = int2{static_cast<int>(slot), static_cast<int>(((j - i) << 1) | (vp ? 1 : 0))};
+}
+
+__device__ inline void emit_added(Entries &o, const BpeTables &t, int code) {
+    if (o.n >= o.limit) return;
+    o.e[o.n++] = int2{t.added_id[code >> 2], 0};
+}
+
+// the end of the run of codepoints from i whose class has any bit of `mask` (set: `want` true) or none (`want` false)
+__device__ inline int64_t class_run(const BpeTables &t, const Gap &g, int64_t i, int mask, bool want, int64_t *last = nullptr) {
+    while (i < g.b) {
+        uint32_t c;
+        const int n = gap_decode(g, i, c);
+        if (((t.cls[c] & mask) != 0) != want) break;
+        if (last) *last = i;
+        i += n;
+    }
+    return i;
+}
+
+__device__ inline int64_t rn_run(const Gap &g, int64_t i) {
+    while (i < g.b && (g.p[i] == '\r' || g.p[i] == '\n')) ++i;
+    return i;
+}
+
+// the end of the match at i of the split pattern; every codepoint starts a match of either pattern
+// G (GPT-2, ByteLevel use_regex): 's|'t|'re|'ve|'m|'ll|'d| ?\p{L}+| ?\p{N}+| ?[^\s\p{L}\p{N}]+|\s+(?!\S)|\s+
+// L (Llama-3): (?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+|\s+(?!\S)|\s+
+__device__ inline int64_t split_match(const BpeTables &t, const Gap &g, int64_t i) {
+    const bool llama = t.split == kSplitLlama3;
+    uint32_t c0, c1 = 0, c2 = 0;
+    const int n0 = gap_decode(g, i, c0);
+    const int64_t i1 = i + n0;
+    const int n1 = i1 < g.b ? gap_decode(g, i1, c1) : 0;
+    const int k0 = t.cls[c0], k1 = n1 ? t.cls[c1] : kS;     // past the end: no letter, number or other char follows
+    if (c0 == '\'' && n1) {
+        const int64_t i2 = i1 + n1;
+        const int n2 = i2 < g.b ? gap_decode(g, i2, c2) : 0;
+        if (llama) {
+            const int f1 = k1 >> 4, f2 = n2 ? t.cls[c2] >> 4 : 0;
+            if (f1 == kFoldS || f1 == kFoldT || f1 == kFoldM || f1 == kFoldD) return i2;
+            if (((f1 == kFoldR || f1 == kFoldV) && f2 == kFoldE) || (f1 == kFoldL && f2 == kFoldL)) return i2 + n2;
+        } else {
+            if (c1 == 's' || c1 == 't' || c1 == 'm' || c1 == 'd') return i2;
+            if (((c1 == 'r' || c1 == 'v') && c2 == 'e') || (c1 == 'l' && c2 == 'l')) return i2 + n2;
+        }
+    }
+    const bool o0 = !(k0 & (kL | kN | kS)), o1 = n1 && !(k1 & (kL | kN | kS));
+    if (llama) {
+        if (!(k0 & (kL | kN)) && c0 != '\r' && c0 != '\n' && n1 && (k1 & kL)) return class_run(t, g, i1, kL, true);
+        if (k0 & kL) return class_run(t, g, i, kL, true);
+        if (k0 & kN) {
+            int64_t j = i;
+            for (int k = 0; k < 3 && j < g.b; ++k) {
+                uint32_t c;
+                const int n = gap_decode(g, j, c);
+                if (!(t.cls[c] & kN)) break;
+                j += n;
+            }
+            return j;
+        }
+        if (c0 == ' ' && o1) return rn_run(g, class_run(t, g, i1, kL | kN | kS, false));
+        if (o0) return rn_run(g, class_run(t, g, i, kL | kN | kS, false));
+    } else {
+        if (c0 == ' ' && n1 && (k1 & kL)) return class_run(t, g, i1, kL, true);
+        if (c0 == ' ' && n1 && (k1 & kN)) return class_run(t, g, i1, kN, true);
+        if (c0 == ' ' && o1) return class_run(t, g, i1, kL | kN | kS, false);
+        if (k0 & kL) return class_run(t, g, i, kL, true);
+        if (k0 & kN) return class_run(t, g, i, kN, true);
+        if (o0) return class_run(t, g, i, kL | kN | kS, false);
+    }
+    // c0 is whitespace: the run of it, which \s*[\r\n]+ (L) ends after its last \r or \n, and \s+(?!\S) before its last char
+    // when a non-space follows
+    int64_t last = i;
+    const int64_t j = class_run(t, g, i, kS, true, &last);
+    if (llama) {
+        for (int64_t k = j - 1; k >= i && k >= g.a; --k)
+            if (g.p[k] == '\r' || g.p[k] == '\n') return k + 1;
+    }
+    if (j == g.b || last == i) return j;
+    return last;
+}
+
+// ByteLevel / Split over one gap: the words it yields, in order
+__device__ inline void split_gap(const BpeTables &t, const uint8_t *p, int64_t a, int64_t b, Entries &o) {
+    if (a >= b) return;                       // the library drops empty pieces before the pre-tokenizer runs
+    Gap g{p, a, b, t.prefix_space && p[a] != ' '};
+    for (int64_t i = g.vp ? a - 1 : a; i < b && o.n < o.limit && !o.huge;) {
+        const int64_t j = split_match(t, g, i);
+        emit_word(o, g, i, j);
+        i = j;
+    }
+}
+
+__device__ inline bool rust_space_at(const BpeTables &t, const uint8_t *p, int64_t i, int64_t end, int &n) {
+    uint32_t c;
+    n = utf8_decode(p + i, p + end, c);
+    return (t.cls[c] & kRust) != 0;
+}
+
+// the next added token of `pass` in [from, end) (aho-corasick leftmost-longest), widened by lstrip down to `from` and by
+// rstrip up to `end` over Rust whitespace: returns its terminal code and [*s, *e), or -1 with *s = end
+__device__ inline int next_added(const BpeTables &t, int pass, const uint8_t *p, int64_t from, int64_t end, int64_t *s,
+                                 int64_t *e) {
+    *s = end;
+    if (!t.n_pass[pass]) return -1;
+    for (int64_t i = from; i < end; ++i) {
+        if (!((t.first_byte[pass][p[i] >> 5] >> (p[i] & 31)) & 1u)) continue;
+        int node = 0, code = -1;
+        int64_t stop = i;
+        for (int64_t j = i; j < end; ++j) {
+            const int key = (node << 8) | p[j];
+            uint32_t h = static_cast<uint32_t>(key) * 0x9E3779B1u;
+            int child = -1;
+            for (uint32_t k = (h ^ (h >> 16)) & t.edge_mask;; k = (k + 1) & t.edge_mask) {
+                const int2 x = t.edges[k];
+                if (x.x < 0) break;
+                if (x.x == key) { child = x.y; break; }
+            }
+            if (child < 0) break;
+            node = child;
+            const int2 tm = t.term[node];
+            const int c = pass ? tm.y : tm.x;
+            if (c >= 0) { code = c; stop = j + 1; }
+        }
+        if (code < 0) continue;
+        int64_t a = i;
+        int n;
+        if (code & 2) {
+            while (a > from) {
+                int64_t q = a - 1;
+                while (q > from && a - q < 4 && (p[q] & 0xC0) == 0x80) --q;
+                if (!rust_space_at(t, p, q, a, n) || q + n != a) break;
+                a = q;
+            }
+        }
+        if (code & 1)
+            while (stop < end && rust_space_at(t, p, stop, end, n)) stop += n;
+        *s = a;
+        *e = stop;
+        return code;
+    }
+    return -1;
+}
+
+// entries of text b: ws_ent[b, 0 .. n_ent[b]); n_ent[b] = -1 and lengths[b] = -1 for a text left to the caller
+__global__ void __launch_bounds__(128) tokenize_bpe_split_kernel(BpeTables t, const uint8_t *text, const int64_t *offsets,
+                                                                 int B, int max_length, int64_t n_slots, int32_t *lengths,
+                                                                 int32_t *max_len, int2 *ws_ent, int32_t *n_ent) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const uint8_t *p = text + offsets[b];
+    const int64_t len = offsets[b + 1] - offsets[b], base = offsets[b] - offsets[0] + b;
+    const int limit = max_length - 2;
+    Entries o{ws_ent + static_cast<int64_t>(b) * limit, 0, limit, n_slots - base, false};
+    if (o.slots < len + 1 || len >= INT32_MAX) o.huge = true;       // the workspace was sized for fewer bytes
+    for (int64_t g1 = 0; g1 <= len && o.n < o.limit && !o.huge;) {
+        int64_t s1, e1;
+        const int code1 = next_added(t, 0, p, g1, len, &s1, &e1);
+        for (int64_t g2 = g1; o.n < o.limit && !o.huge;) {
+            int64_t s2, e2;
+            const int code2 = next_added(t, 1, p, g2, s1, &s2, &e2);
+            split_gap(t, p, g2, s2, o);
+            if (code2 < 0) break;
+            emit_added(o, t, code2);
+            g2 = e2;
+        }
+        if (code1 < 0 || o.huge) break;
+        emit_added(o, t, code1);
+        g1 = e1;
+    }
+    n_ent[b] = o.huge ? -1 : o.n;
+    if (o.huge) {
+        lengths[b] = -1;
+        atomicMax(max_len + 1, 1);
+    }
+}
+
+__device__ inline const int4 *merge_find(const BpeTables &t, int l, int r) {
+    uint32_t h = static_cast<uint32_t>(l) * 0x9E3779B1u ^ static_cast<uint32_t>(r) * 0x85EBCA77u;
+    h ^= h >> 15;
+    for (uint32_t i = h & t.merge_mask;; i = (i + 1) & t.merge_mask) {
+        const int4 *e = t.merges + i;
+        if (e->x < 0) return nullptr;
+        if (e->x == l && e->y == r) return e;
+    }
+}
+
+__device__ inline int word_find(const BpeTables &t, const uint8_t *w, int n, bool vp) {
+    uint32_t h = kFnvBasis;
+    if (vp) h = (h ^ ' ') * 16777619u;
+    h = fnv1a(h, w, n - vp);
+    for (uint32_t i = h & t.word_mask;; i = (i + 1) & t.word_mask) {
+        const int4 e = t.words[i];
+        if (e.x < 0) return -1;
+        if (static_cast<uint32_t>(e.y) != h || e.w != n) continue;
+        const uint8_t *v = t.word_bytes + e.z;
+        bool eq = !vp || v[0] == ' ';
+        for (int j = 0; j < n - vp && eq; ++j) eq = v[vp + j] == w[j];
+        if (eq) return e.x;
+    }
+}
+
+__device__ inline void heap_push(uint64_t *h, int &n, uint64_t v) {
+    int i = n++;
+    while (i > 0) {
+        const int up = (i - 1) >> 1;
+        if (h[up] <= v) break;
+        h[i] = h[up];
+        i = up;
+    }
+    h[i] = v;
+}
+
+__device__ inline uint64_t heap_pop(uint64_t *h, int &n) {
+    const uint64_t top = h[0], v = h[--n];
+    int i = 0;
+    for (;;) {
+        int c = 2 * i + 1;
+        if (c >= n) break;
+        if (c + 1 < n && h[c + 1] < h[c]) ++c;
+        if (v <= h[c]) break;
+        h[i] = h[c];
+        i = c;
+    }
+    if (n) h[i] = v;
+    return top;
+}
+
+__device__ inline void push_pair(const BpeTables &t, uint64_t *h, int &hn, const int32_t *id, int pos, int right) {
+    if (const int4 *m = merge_find(t, id[pos], id[right]))
+        heap_push(h, hn, (static_cast<uint64_t>(static_cast<uint32_t>(m->z)) << 32) | static_cast<uint32_t>(pos));
+}
+
+// the BPE tokens of entry k of text b, written over the word's slots from its first one; its info becomes -(token count)
+__global__ void __launch_bounds__(128) tokenize_bpe_merge_kernel(BpeTables t, const uint8_t *text, const int64_t *offsets,
+                                                                 int B, int max_length, int2 *ws_ent, const int32_t *n_ent,
+                                                                 int32_t *ws_tok, int32_t *ws_link, uint64_t *ws_heap) {
+    const int limit = max_length - 2;
+    const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (gid >= static_cast<int64_t>(B) * limit) return;
+    const int b = static_cast<int>(gid / limit), k = static_cast<int>(gid - static_cast<int64_t>(b) * limit);
+    if (k >= n_ent[b]) return;
+    int2 &ent = ws_ent[gid];
+    if (ent.y <= 0) return;
+    const int n = ent.y >> 1;
+    const bool vp = ent.y & 1;
+    const int64_t base = offsets[b] - offsets[0] + b + ent.x;       // the word's first slot
+    const uint8_t *w = text + offsets[b] + ent.x - 1 + vp;          // its first real byte
+    int32_t *id = ws_tok + base;
+    if (t.ignore_merges) {
+        const int v = word_find(t, w, n, vp);
+        if (v >= 0) {
+            id[0] = v;
+            ent.y = -1;
+            return;
+        }
+    }
+    for (int i = 0; i < n; ++i) id[i] = t.byte_id[(vp && i == 0) ? ' ' : w[i - vp]];
+    if (n == 1) {
+        ent.y = -1;
+        return;
+    }
+    int32_t *next = ws_link + 2 * base, *prev = next + n;
+    uint64_t *h = ws_heap + 3 * base;
+    int hn = 0;
+    for (int i = 0; i < n; ++i) {
+        next[i] = i + 1 < n ? i + 1 : -1;
+        prev[i] = i - 1;
+    }
+    for (int i = 0; i + 1 < n; ++i) push_pair(t, h, hn, id, i, i + 1);
+    while (hn) {
+        const uint64_t top = heap_pop(h, hn);
+        const int pos = static_cast<int>(top & 0xffffffffu), rank = static_cast<int>(top >> 32);
+        if (id[pos] < 0) continue;
+        const int nx = next[pos];
+        if (nx < 0) continue;
+        const int4 *m = merge_find(t, id[pos], id[nx]);
+        if (!m || m->z != rank) continue;                      // an entry for a pair that has changed since
+        id[pos] = m->w;
+        id[nx] = -1;
+        const int nn = next[nx];
+        next[pos] = nn;
+        if (nn >= 0) prev[nn] = pos;
+        if (prev[pos] >= 0) push_pair(t, h, hn, id, prev[pos], pos);
+        if (nn >= 0) push_pair(t, h, hn, id, pos, nn);
+    }
+    int c = 0;
+    for (int i = 0; i >= 0; i = next[i]) id[c++] = id[i];
+    ent.y = -c;
+}
+
+// tokens[b] = [CLS] the entries' tokens [SEP], truncated to max_length; one warp per text
+__global__ void __launch_bounds__(128) tokenize_bpe_gather_kernel(BpeTables t, const int64_t *offsets, int B, int max_length,
+                                                                  const int2 *ws_ent, const int32_t *n_ent,
+                                                                  const int32_t *ws_tok, int32_t *tokens, int32_t *lengths,
+                                                                  int32_t *max_len) {
+    const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (b >= B) return;
+    const int ne = n_ent[b];
+    if (ne < 0) return;
+    const int limit = max_length - 2;
+    const int2 *ent = ws_ent + static_cast<int64_t>(b) * limit;
+    const int32_t *slots = ws_tok + offsets[b] - offsets[0] + b;
+    int32_t *row = tokens + static_cast<int64_t>(b) * max_length;
+    int done = 0;
+    for (int k0 = 0; k0 < ne && done < limit; k0 += 32) {
+        const int k = k0 + lane;
+        const int2 e = k < ne ? ent[k] : int2{0, 0};
+        const int c = k < ne ? (e.y ? -e.y : 1) : 0;
+        int incl = c;
+        for (int d = 1; d < 32; d <<= 1) {
+            const int v = __shfl_sync(0xffffffffu, incl, lane >= d ? lane - d : lane);
+            if (lane >= d) incl += v;
+        }
+        for (int j = 0, at = done + incl - c; j < c && at + j < limit; ++j) row[1 + at + j] = e.y ? slots[e.x + j] : e.x;
+        done += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    if (lane == 0) {
+        const int n = done < limit ? done : limit;
+        row[0] = t.cls_id;
+        row[1 + n] = t.sep_id;
+        lengths[b] = n + 2;
+        atomicMax(max_len, n + 2);
+    }
+}
+
+// ---------------------------------------------------------------- host side of the BPE tables
+struct BpeHost {
+    std::vector<int4> merges, words;
+    std::vector<int2> edges, term;
+    std::vector<int32_t> added_id;
+    BpeTables t{};              // scalars, byte ids and first_byte filled; pointers left to the owner
+};
+
+inline uint32_t pow2_at_least(size_t n) {
+    size_t s = 2;
+    while (s < n) s <<= 1;
+    return static_cast<uint32_t>(s);
+}
+
+inline const char *build_bpe_host_tables(const ac_bpe_tokenizer_spec &s, BpeHost &h) {
+    if (!s.cls || !s.byte_ids || (s.n_merges && !s.merges) || s.n_merges < 0) return "null table";
+    if (s.split != kSplitGpt2 && s.split != kSplitLlama3) return "unknown split pattern";
+    if (s.ignore_merges && (!s.vocab_bytes || !s.vocab_offsets || !s.vocab_ids || s.n_vocab <= 0))
+        return "ignore_merges without a vocab";
+    if (s.n_added < 0 || (s.n_added && (!s.added_bytes || !s.added_offsets || !s.added_ids || !s.added_flags)))
+        return "bad added tokens";
+    for (int i = 0; i < 256; ++i) {
+        if (s.byte_ids[i] < 0) return "a byte has no symbol in the vocab";
+        h.t.byte_id[i] = s.byte_ids[i];
+    }
+    const uint32_t mm = pow2_at_least(2 * static_cast<size_t>(s.n_merges));
+    h.merges.assign(mm, int4{-1, 0, 0, 0});
+    for (int r = 0; r < s.n_merges; ++r) {
+        const int l = s.merges[3 * r], rt = s.merges[3 * r + 1], nw = s.merges[3 * r + 2];
+        if (l < 0 || rt < 0 || nw < 0) return "negative id in a merge";
+        uint32_t x = static_cast<uint32_t>(l) * 0x9E3779B1u ^ static_cast<uint32_t>(rt) * 0x85EBCA77u;
+        x ^= x >> 15;
+        uint32_t i = x & (mm - 1);
+        while (h.merges[i].x >= 0 && !(h.merges[i].x == l && h.merges[i].y == rt)) i = (i + 1) & (mm - 1);
+        h.merges[i] = int4{l, rt, r, nw};            // a repeated pair keeps its last rank, as the library's map does
+    }
+    h.words.assign(2, int4{-1, 0, 0, 0});
+    if (s.ignore_merges) {
+        int max_key = 0;
+        if (const char *why = hash_byte_strings(s.vocab_bytes, s.vocab_offsets, s.vocab_ids, s.n_vocab, h.words, max_key))
+            return why;
+    }
+    // trie of the added tokens' bytes, nodes numbered from the root 0; edges in an open-addressing table
+    std::vector<std::vector<std::pair<int, int>>> kids(1);
+    h.term.assign(1, int2{-1, -1});
+    memset(h.t.first_byte, 0, sizeof(h.t.first_byte));
+    for (int a = 0; a < s.n_added; ++a) {
+        const int64_t o0 = s.added_offsets[a], n = s.added_offsets[a + 1] - o0;
+        if (n <= 0) return "empty added token";
+        const int f = s.added_flags[a], pass = f & 1;
+        int node = 0;
+        for (int64_t j = 0; j < n; ++j) {
+            const int byte = s.added_bytes[o0 + j];
+            int child = -1;
+            for (auto &e : kids[node])
+                if (e.first == byte) child = e.second;
+            if (child < 0) {
+                child = static_cast<int>(kids.size());
+                if (child >= (1 << 23)) return "added tokens too long";
+                kids[node].push_back({byte, child});
+                kids.emplace_back();
+                h.term.push_back(int2{-1, -1});
+            }
+            node = child;
+        }
+        const int code = (a << 2) | (f & 2) | (f >> 2 & 1);     // lstrip << 1 | rstrip
+        int &slot = pass ? h.term[node].y : h.term[node].x;
+        if (slot < 0) slot = code;                    // the same content twice: the first one's id and flags
+        h.t.first_byte[pass][s.added_bytes[o0] >> 5] |= 1u << (s.added_bytes[o0] & 31);
+        ++h.t.n_pass[pass];
+        h.added_id.push_back(s.added_ids[a]);
+    }
+    if (h.added_id.empty()) h.added_id.push_back(0);
+    size_t n_edges = 0;
+    for (auto &k : kids) n_edges += k.size();
+    const uint32_t em = pow2_at_least(2 * n_edges);
+    h.edges.assign(em, int2{-1, 0});
+    for (size_t node = 0; node < kids.size(); ++node)
+        for (auto &e : kids[node]) {
+            const int key = static_cast<int>(node << 8) | e.first;
+            const uint32_t x = static_cast<uint32_t>(key) * 0x9E3779B1u;
+            uint32_t i = (x ^ (x >> 16)) & (em - 1);
+            while (h.edges[i].x >= 0) i = (i + 1) & (em - 1);
+            h.edges[i] = int2{key, e.second};
+        }
+    h.t.merge_mask = mm - 1;
+    h.t.word_mask = static_cast<uint32_t>(h.words.size() - 1);
+    h.t.edge_mask = em - 1;
+    h.t.split = s.split;
+    h.t.prefix_space = s.add_prefix_space ? 1 : 0;
+    h.t.ignore_merges = s.ignore_merges ? 1 : 0;
+    h.t.cls_id = s.cls_id;
+    h.t.sep_id = s.sep_id;
+    h.t.pad_id = s.pad_id;
+    return nullptr;
+}
+
+// workspace of a BPE call, in this order: entries int2 [B, max_length - 2], n_ent int32 [B], then per slot (text bytes + B
+// of them) the token / symbol id, the next and prev links and three heap entries
+constexpr size_t kBpeSlotBytes = 4 + 8 + 24;
+inline size_t bpe_fixed_bytes(int B, int max_length) {
+    return (static_cast<size_t>(B) * (max_length - 2) * 8 + static_cast<size_t>(B) * 4 + 255) / 256 * 256;
+}
+inline size_t bpe_workspace_bytes(int B, int64_t text_bytes, int max_length) {
+    return bpe_fixed_bytes(B, max_length) + (static_cast<size_t>(text_bytes) + B) * kBpeSlotBytes + 256;
+}
+
 }  // namespace tok
 }  // namespace ac
 
 #ifndef AC_CPU_SHIM
 using namespace ac;
 
+// one handle type for both kinds: `bpe` tells which of the two table sets the calls read
 struct ac_tokenizer {
+    bool bpe;
     tok::Tables t;
+    tok::BpeTables b;
+    int pad_id;
     std::vector<void *> owned;
 };
 
@@ -350,7 +862,9 @@ extern "C" int ac_tokenizer_create(const ac_tokenizer_spec *spec, ac_tokenizer *
         return AC_E_INVALID;
     }
     ac_tokenizer *k = new ac_tokenizer();
+    k->bpe = false;
     k->t = h.t;
+    k->pad_id = h.t.pad_id;
     const void *p[8];
     int rc = AC_OK;
     const int64_t vbytes = spec->vocab_offsets[spec->n_vocab];
@@ -377,9 +891,82 @@ extern "C" int ac_tokenizer_create(const ac_tokenizer_spec *spec, ac_tokenizer *
     return AC_OK;
 }
 
+extern "C" int ac_tokenizer_create_bpe(const ac_bpe_tokenizer_spec *spec, ac_tokenizer **out) {
+    AC_REQUIRE(spec && out, "ac_tokenizer_create_bpe: null argument");
+    *out = nullptr;
+    tok::BpeHost h;
+    if (const char *why = tok::build_bpe_host_tables(*spec, h)) {
+        set_error("ac_tokenizer_create_bpe: %s", why);
+        return AC_E_INVALID;
+    }
+    ac_tokenizer *k = new ac_tokenizer();
+    k->bpe = true;
+    k->b = h.t;
+    k->pad_id = h.t.pad_id;
+    const void *p[7];
+    int rc = AC_OK;
+    const int64_t vbytes = spec->ignore_merges ? spec->vocab_offsets[spec->n_vocab] : 0;
+    if ((rc = tok_upload(k, spec->cls, tok::kCodepoints, &p[0])) ||
+        (rc = tok_upload(k, h.merges.data(), sizeof(int4) * h.merges.size(), &p[1])) ||
+        (rc = tok_upload(k, h.words.data(), sizeof(int4) * h.words.size(), &p[2])) ||
+        (rc = tok_upload(k, spec->vocab_bytes, vbytes, &p[3])) ||
+        (rc = tok_upload(k, h.edges.data(), sizeof(int2) * h.edges.size(), &p[4])) ||
+        (rc = tok_upload(k, h.term.data(), sizeof(int2) * h.term.size(), &p[5])) ||
+        (rc = tok_upload(k, h.added_id.data(), sizeof(int32_t) * h.added_id.size(), &p[6]))) {
+        ac_tokenizer_destroy(k);
+        return rc;
+    }
+    k->b.cls = static_cast<const uint8_t *>(p[0]);
+    k->b.merges = static_cast<const int4 *>(p[1]);
+    k->b.words = static_cast<const int4 *>(p[2]);
+    k->b.word_bytes = static_cast<const uint8_t *>(p[3]);
+    k->b.edges = static_cast<const int2 *>(p[4]);
+    k->b.term = static_cast<const int2 *>(p[5]);
+    k->b.added_id = static_cast<const int32_t *>(p[6]);
+    *out = k;
+    return AC_OK;
+}
+
 extern "C" int ac_tokenize_workspace_bytes(const ac_tokenizer *tok, int B, size_t *bytes) {
     AC_REQUIRE(tok && bytes && B >= 0, "ac_tokenize_workspace_bytes: bad arguments");
+    AC_REQUIRE(!tok->bpe, "ac_tokenize_workspace_bytes: a BPE handle's workspace depends on the text bytes; use "
+                          "ac_tokenize_workspace_bytes_text");
     *bytes = tok::workspace_bytes(tok->t.max_chars, B);
+    return AC_OK;
+}
+
+extern "C" int ac_tokenize_workspace_bytes_text(const ac_tokenizer *tok, int B, int64_t text_bytes, int max_length,
+                                                size_t *bytes) {
+    AC_REQUIRE(tok && bytes && B >= 0 && text_bytes >= 0 && max_length >= 2, "ac_tokenize_workspace_bytes_text: bad arguments");
+    *bytes = tok->bpe ? tok::bpe_workspace_bytes(B, text_bytes, max_length) : tok::workspace_bytes(tok->t.max_chars, B);
+    return AC_OK;
+}
+
+static int tokenize_bpe(const ac_tokenizer *tok, const uint8_t *text, const int64_t *offsets, int B, int max_length,
+                        int32_t *tokens, int32_t *lengths, int32_t *max_len, void *workspace, size_t workspace_bytes,
+                        cudaStream_t s) {
+    const size_t fixed = tok::bpe_fixed_bytes(B, max_length);
+    AC_REQUIRE(workspace && workspace_bytes >= tok::bpe_workspace_bytes(B, 0, max_length), "ac_tokenize: workspace too small");
+    // the slots the workspace holds; a text past them is left to the caller like a text with a huge word
+    const int64_t n_slots = static_cast<int64_t>((workspace_bytes - fixed - 256) / tok::kBpeSlotBytes);
+    int2 *ent = static_cast<int2 *>(workspace);
+    int32_t *n_ent = reinterpret_cast<int32_t *>(ent + static_cast<size_t>(B) * (max_length - 2));
+    int32_t *ws_tok = reinterpret_cast<int32_t *>(static_cast<uint8_t *>(workspace) + fixed);
+    int32_t *ws_link = ws_tok + n_slots;
+    uint64_t *ws_heap = reinterpret_cast<uint64_t *>(reinterpret_cast<uintptr_t>(ws_link + 2 * n_slots + 1) & ~uintptr_t(7));
+    AC_CUDA(cudaMemsetAsync(max_len, 0, 2 * sizeof(int32_t), s));
+    tok::tokenize_bpe_split_kernel<<<(B + 127) / 128, 128, 0, s>>>(tok->b, text, offsets, B, max_length, n_slots, lengths,
+                                                                   max_len, ent, n_ent);
+    AC_LAUNCH_CHECK();
+    const int64_t words = static_cast<int64_t>(B) * (max_length - 2);
+    if (words) {
+        tok::tokenize_bpe_merge_kernel<<<static_cast<unsigned>((words + 127) / 128), 128, 0, s>>>(
+            tok->b, text, offsets, B, max_length, ent, n_ent, ws_tok, ws_link, ws_heap);
+        AC_LAUNCH_CHECK();
+    }
+    tok::tokenize_bpe_gather_kernel<<<(B + 3) / 4, 128, 0, s>>>(tok->b, offsets, B, max_length, ent, n_ent, ws_tok, tokens,
+                                                                lengths, max_len);
+    AC_LAUNCH_CHECK();
     return AC_OK;
 }
 
@@ -388,8 +975,9 @@ extern "C" int ac_tokenize(const ac_tokenizer *tok, const uint8_t *text, const i
                            ac_stream_t stream) {
     AC_REQUIRE(tok && text && offsets && tokens && lengths && max_len && B >= 1, "ac_tokenize: bad arguments");
     AC_REQUIRE(max_length >= 2, "ac_tokenize: max_length=%d < 2 leaves no room for the two special tokens", max_length);
-    AC_REQUIRE(workspace && workspace_bytes >= tok::workspace_bytes(tok->t.max_chars, B), "ac_tokenize: workspace too small");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (tok->bpe) return tokenize_bpe(tok, text, offsets, B, max_length, tokens, lengths, max_len, workspace, workspace_bytes, s);
+    AC_REQUIRE(workspace && workspace_bytes >= tok::workspace_bytes(tok->t.max_chars, B), "ac_tokenize: workspace too small");
     uint32_t *ws_cp = static_cast<uint32_t *>(workspace);
     uint8_t *ws_bytes = reinterpret_cast<uint8_t *>(ws_cp + static_cast<size_t>(B) * (tok->t.max_chars + 1));
     AC_CUDA(cudaMemsetAsync(max_len, 0, sizeof(int32_t), s));
@@ -405,7 +993,7 @@ extern "C" int ac_tokenize_pack(const ac_tokenizer *tok, const int32_t *tokens, 
     const int64_t total = static_cast<int64_t>(B) * S;
     const int grid = static_cast<int>(std::min<int64_t>((total + 255) / 256, 4 * sm_count()));
     tok::tokenize_pack_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(tokens, lengths, B, max_length, S,
-                                                                                   tok->t.pad_id, ids, mask, type_ids);
+                                                                                   tok->pad_id, ids, mask, type_ids);
     AC_LAUNCH_CHECK();
     return AC_OK;
 }

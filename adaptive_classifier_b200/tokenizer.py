@@ -1,4 +1,5 @@
-"""Which Hugging Face tokenizers the device WordPiece tokenizer (csrc/tokenizer.cu) reproduces, and the Unicode tables it runs on.
+"""Which Hugging Face tokenizers the device tokenizers (csrc/tokenizer.cu: WordPiece, byte-level BPE) reproduce, and the Unicode
+tables they run on.
 
 The tables are derived by probing the installed `tokenizers` library (`normalize_str`, `pre_tokenize_str`), not from Python's
 `unicodedata`: the Rust crates behind `tokenizers` carry their own Unicode version, and what must match is the library the host
@@ -84,13 +85,13 @@ def _reorder_ranks(nz, marks) -> dict:
     return {a: dense[int(below[i])] for i, a in enumerate(marks) if moved[i]}
 
 
-def _disk_cache_path(key) -> str:
+def _disk_cache_path(key, kind: str = "wordpiece") -> str:
     """file of the tables for `key` under the user's cache directory; the name carries the tokenizers version, the flags and a
     hash of this module, so a changed library or a changed probe never reads an old file"""
     with open(__file__, "rb") as f:
         src = hashlib.sha256(f.read()).hexdigest()[:16]
     root = os.environ.get("XDG_CACHE_HOME") or os.path.join(os.path.expanduser("~"), ".cache")
-    name = "wordpiece-tables-" + "-".join(str(k) for k in key) + f"-{src}.npz"
+    name = f"{kind}-tables-" + "-".join(str(k) for k in key) + f"-{src}.npz"
     return os.path.join(root, "adaptive_classifier_b200", name)
 
 
@@ -247,6 +248,201 @@ def wordpiece_spec(tokenizer) -> Tuple[Optional[dict], str]:
                        lower if strip is None else bool(strip), lower),
                 type_ids="token_type_ids" in getattr(tokenizer, "model_input_names", ()))
     return spec, ""
+
+
+# ================================================================ byte-level BPE (csrc/tokenizer.cu, tokenize_bpe_*)
+BPE_L, BPE_N, BPE_S, BPE_RUST = 1, 2, 4, 8
+FOLD_LETTERS = "strevmld"                   # class bits 4-7: 1 + the index of the letter a codepoint matches under (?i)
+SPLIT_GPT2, SPLIT_LLAMA3 = 0, 1
+LLAMA3_PATTERN = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+"
+                  r"|\s+(?!\S)|\s+")
+MAX_WORD = 1024                             # AC_BPE_MAX_WORD
+
+
+def _uncovered(pre_tokenizer, chars) -> np.ndarray:
+    """bool per char of `chars`: no piece of pre_tokenize_str covers it (what a 'removed' split or a whitespace split drops)"""
+    covered = np.zeros(len(chars), dtype=bool)
+    for _, (a, b) in pre_tokenizer.pre_tokenize_str("".join(chars)):
+        covered[a:b] = True
+    return ~covered
+
+
+def bpe_classes() -> np.ndarray:
+    """uint8 [N_CODEPOINTS] in the layout of ac_bpe_tokenizer_spec.cls: \\p{L}, \\p{N} and \\s as the library's regex engine
+    (Oniguruma) matches them, Rust's char::is_whitespace (which lstrip / rstrip strip), and the letter of s t r e v m l d a
+    codepoint matches case-insensitively.  Each class is one library call over every codepoint: a 'removed' split of a
+    one-char pattern drops exactly the codepoints it matches, WhitespaceSplit the whitespace.  Kept in the process and on disk."""
+    import tokenizers
+    key = ("bpe", tokenizers.__version__)
+    if key in _CACHE:
+        return _CACHE[key]
+    path = _disk_cache_path(key[1:], "bpe")
+    try:
+        with np.load(path) as z:
+            cls = z["cls"]
+    except (OSError, KeyError, ValueError):
+        from tokenizers import Regex, pre_tokenizers
+        cps = probe_codepoints()
+        chars = list(map(chr, cps.tolist()))
+        sub = np.zeros(len(chars), dtype=np.uint8)
+        for bit, pat in ((BPE_L, r"\p{L}"), (BPE_N, r"\p{N}"), (BPE_S, r"\s")):
+            sub |= np.where(_uncovered(pre_tokenizers.Split(Regex(pat), "removed"), chars), bit, 0).astype(np.uint8)
+        sub |= np.where(_uncovered(pre_tokenizers.WhitespaceSplit(), chars), BPE_RUST, 0).astype(np.uint8)
+        for i, letter in enumerate(FOLD_LETTERS):
+            hit = _uncovered(pre_tokenizers.Split(Regex(f"(?i:{letter})"), "removed"), chars)
+            if (sub[hit] >> 4).any():
+                raise ValueError(f"a codepoint matches two contraction letters under (?i) ({letter!r})")
+            sub |= np.where(hit, (i + 1) << 4, 0).astype(np.uint8)
+        cls = np.zeros(N_CODEPOINTS, dtype=np.uint8)
+        cls[cps] = sub
+        try:
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+            fd, tmp = tempfile.mkstemp(dir=os.path.dirname(path), suffix=".npz")
+            with os.fdopen(fd, "wb") as f:
+                np.savez(f, cls=cls)
+            os.replace(tmp, path)
+        except OSError as e:
+            logger.debug(f"tokenizer tables not cached on disk: {e}")
+    _CACHE[key] = cls
+    return cls
+
+
+def byte_level_map() -> dict:
+    """{byte-level symbol: byte}: GPT-2's bytes_to_unicode, which ByteLevel applies to every byte of a piece"""
+    keep = list(range(ord("!"), ord("~") + 1)) + list(range(ord("¡"), ord("¬") + 1)) + list(range(ord("®"), ord("ÿ") + 1))
+    out, n = {}, 0
+    for b in range(256):
+        if b in keep:
+            out[chr(b)] = b
+        else:
+            out[chr(256 + n)] = b
+            n += 1
+    return out
+
+
+def _special_pair(post) -> Tuple[Optional[Tuple[int, int]], str]:
+    """(cls id, sep id) of a single-sequence post-processor '[special] A [special]' with type id 0"""
+    pt = post.get("type")
+    if pt == "Sequence":
+        procs = post.get("processors") or []
+        rest = [p for p in procs if p.get("type") != "ByteLevel"]       # ByteLevel only moves offsets
+        if len(rest) != 1 or rest[0].get("type") == "Sequence":
+            return None, "post-processor Sequence is not ByteLevel and one '[special] A [special]' processor"
+        return _special_pair(rest[0])
+    if pt == "TemplateProcessing":
+        single = post.get("single") or []
+        kinds = [next(iter(x)) for x in single]
+        if kinds != ["SpecialToken", "Sequence", "SpecialToken"] or any(next(iter(x.values())).get("type_id", 0) for x in single):
+            return None, "post-processor template is not '[special] A [special]' with type id 0"
+        ids = []
+        for x in (single[0], single[2]):
+            st = post["special_tokens"].get(x["SpecialToken"]["id"], {})
+            if len(st.get("ids", [])) != 1:
+                return None, "post-processor special token with more than one id"
+            ids.append(st["ids"][0])
+        return (int(ids[0]), int(ids[1])), ""
+    if pt in ("BertProcessing", "RobertaProcessing"):
+        return (int(post["cls"][1]), int(post["sep"][1])), ""
+    return None, f"post_processor {pt!r} is not TemplateProcessing / BertProcessing / RobertaProcessing"
+
+
+def _rust_space(ch: str) -> bool:
+    return bool(bpe_classes()[ord(ch)] & BPE_RUST)
+
+
+def bpe_spec(tokenizer) -> Tuple[Optional[dict], str]:
+    """(spec, "") when the tokenizer is a byte-level BPE tokenizer the device kernels reproduce id for id, else (None, reason).
+    Read from `backend_tokenizer.to_str()`; accepts nothing looser than: a BPE model without dropout, affixes or byte fallback
+    whose vocab holds all 256 byte symbols, no normalizer, ByteLevel(use_regex) or Split(Llama-3 pattern) + ByteLevel, a
+    '[special] A [special]' post-processor with type id 0 (optionally in a Sequence with ByteLevel), right truncation and
+    padding, added tokens with single_word = false, and a Python wrapper that passes the text through unchanged."""
+    bt = getattr(tokenizer, "backend_tokenizer", None)
+    if bt is None:
+        return None, "no Rust `tokenizers` backend (slow tokenizer)"
+    j = json.loads(bt.to_str())
+    model, pre, post = j.get("model") or {}, j.get("pre_tokenizer") or {}, j.get("post_processor") or {}
+    if model.get("type") != "BPE":
+        return None, f"model {model.get('type')!r} is not BPE"
+    if model.get("dropout") is not None:
+        return None, "BPE dropout"
+    if model.get("continuing_subword_prefix") or model.get("end_of_word_suffix"):
+        return None, "BPE continuing_subword_prefix / end_of_word_suffix"
+    if model.get("byte_fallback"):
+        return None, "BPE byte_fallback"
+    if j.get("normalizer") is not None:
+        return None, f"normalizer {(j.get('normalizer') or {}).get('type')!r} (byte-level BPE takes none)"
+    if pre.get("type") == "ByteLevel":
+        if not pre.get("use_regex", True):
+            return None, "ByteLevel pre-tokenizer without use_regex"
+        split, prefix_space = SPLIT_GPT2, bool(pre.get("add_prefix_space", False))
+    elif pre.get("type") == "Sequence":
+        seq = pre.get("pretokenizers") or []
+        if len(seq) != 2 or seq[0].get("type") != "Split" or seq[1].get("type") != "ByteLevel":
+            return None, "pre_tokenizer Sequence is not [Split, ByteLevel]"
+        sp, bl = seq
+        if (sp.get("pattern") or {}).get("Regex") != LLAMA3_PATTERN:
+            return None, f"Split pattern {sp.get('pattern')!r} is not the Llama-3 pattern"
+        if sp.get("behavior") != "Isolated" or sp.get("invert"):
+            return None, "Split is not Isolated without invert"
+        if bl.get("use_regex", True) or bl.get("add_prefix_space", False):
+            return None, "ByteLevel after Split with use_regex or add_prefix_space"
+        split, prefix_space = SPLIT_LLAMA3, False
+    else:
+        return None, f"pre_tokenizer {pre.get('type')!r} is not ByteLevel or [Split, ByteLevel]"
+    vocab = model["vocab"]
+    sym = byte_level_map()
+    if any(s not in vocab for s in sym):
+        return None, "the vocab lacks some of the 256 byte-level symbols"
+    pair, why = _special_pair(post)
+    if pair is None:
+        return None, why
+    if getattr(tokenizer, "truncation_side", "right") != "right" or getattr(tokenizer, "padding_side", "right") != "right":
+        return None, "left truncation or left padding"
+    if getattr(bt, "encode_special_tokens", False):
+        return None, "encode_special_tokens splits the special tokens"
+    added = j.get("added_tokens") or []
+    for a in added:
+        if a.get("single_word", False):
+            return None, f"added token {a.get('content')!r} with single_word=True"
+        if not a.get("content"):
+            return None, "empty added token"
+    for norm in (False, True):
+        group = [a for a in added if bool(a.get("normalized", True)) == norm]
+        if any(a.get("rstrip") for a in group) and any(_rust_space(a["content"][0]) for a in group):
+            # the library resumes its scan inside the whitespace an rstrip token took, where such a token may match
+            return None, "an rstrip added token next to one that starts with whitespace"
+    if tokenizer.pad_token_id is None:
+        return None, "no pad token"
+    probe = _REPRESENTATIVE + [f"x{a['content']}y {a['content']} " for a in added]
+    try:
+        wrapped = tokenizer(probe)["input_ids"]
+        backend = [e.ids for e in bt.encode_batch(probe)]
+    except Exception as e:                       # noqa: BLE001 -- any failure means: not a shape we reproduce
+        return None, f"probe encoding failed: {e}"
+    if wrapped != backend:
+        return None, "the Python wrapper changes the text before the backend sees it"
+    merges = []
+    for m in model.get("merges") or []:
+        a, b = m.split(" ", 1) if isinstance(m, str) else m
+        merges.append((vocab[a], vocab[b], vocab[a + b]))
+    spec = dict(split=split, prefix_space=prefix_space, ignore_merges=bool(model.get("ignore_merges", False)),
+                vocab=vocab, byte_ids=[vocab[s] for s in sorted(sym, key=sym.get)], merges=merges,
+                added=[(a["content"], int(a["id"]), bool(a.get("normalized", True)), bool(a.get("lstrip", False)),
+                        bool(a.get("rstrip", False))) for a in added],
+                cls_id=pair[0], sep_id=pair[1], pad_id=int(tokenizer.pad_token_id),
+                type_ids="token_type_ids" in getattr(tokenizer, "model_input_names", ()))
+    return spec, ""
+
+
+def bpe_vocab_bytes(vocab: dict) -> Tuple[list, list]:
+    """(raw byte strings, ids) of the vocab entries made of byte-level symbols only, mapped back to the bytes they stand for"""
+    sym = byte_level_map()
+    words, ids = [], []
+    for w, i in vocab.items():
+        if all(c in sym for c in w):
+            words.append(bytes(sym[c] for c in w))
+            ids.append(int(i))
+    return words, ids
 
 
 def pack_strings(strings) -> Tuple[np.ndarray, np.ndarray]:

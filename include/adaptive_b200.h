@@ -461,6 +461,51 @@ int ac_tokenize(const ac_tokenizer *tok, const uint8_t *text, const int64_t *off
 int ac_tokenize_pack(const ac_tokenizer *tok, const int32_t *tokens, const int32_t *lengths, int B, int max_length, int S,
                      int32_t *ids, int32_t *mask, int32_t *type_ids, ac_stream_t stream);
 
+/* Byte-level BPE tokenizers (RoBERTa, ModernBERT, EuroBERT): no normalizer, the pre-tokenizer ByteLevel(use_regex) with the
+ * GPT-2 split or Split(Llama-3 pattern) + ByteLevel, a BPE model without dropout, affixes or byte fallback whose vocab holds
+ * all 256 byte symbols, "[special] A [special]", right truncation and padding, added tokens with single_word = false.  The
+ * same handle type and calls as above, with two differences:
+ *   - ac_tokenize_workspace_bytes refuses a BPE handle: its workspace depends on the batch's text bytes, so ask
+ *     ac_tokenize_workspace_bytes_text (which answers for either kind);
+ *   - ac_tokenize on a BPE handle takes max_len int32[2]: max_len[0] = max lengths[i] over the texts it tokenized, and
+ *     max_len[1] = 1 when it left texts to the caller (0 otherwise), each with lengths[i] = -1.  Those are the texts among whose
+ *     first max_length - 2 words is one longer than AC_BPE_MAX_WORD bytes (or that do not fit the workspace); the caller
+ *     tokenizes them on the host and writes their rows and lengths before ac_tokenize_pack. */
+#define AC_BPE_MAX_WORD 1024
+#define AC_BPE_SPLIT_GPT2 0     /* 's|'t|'re|'ve|'m|'ll|'d| ?\p{L}+| ?\p{N}+| ?[^\s\p{L}\p{N}]+|\s+(?!\S)|\s+ */
+#define AC_BPE_SPLIT_LLAMA3 1   /* (?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+|\s+(?!\S)|\s+ */
+
+typedef struct {
+    /* HOST class byte of every codepoint c < AC_TOKENIZER_CODEPOINTS, as the library's regex engine and Rust see it: bit 0
+       \p{L}, bit 1 \p{N}, bit 2 \s, bit 3 Rust char::is_whitespace (lstrip / rstrip); bits 4-7 the letter c matches
+       case-insensitively among s t r e v m l d (1 .. 8, 0 none; read by the Llama-3 contractions only) */
+    const uint8_t *cls;
+    int split;                   /* AC_BPE_SPLIT_GPT2 or AC_BPE_SPLIT_LLAMA3 */
+    int add_prefix_space;        /* ByteLevel: a space in front of every piece that does not start with one (GPT-2 split only) */
+    int ignore_merges;           /* a word that is a whole vocab entry is that entry */
+    /* the model vocab as raw bytes (byte symbols mapped back), entry v = vocab_bytes[vocab_offsets[v] .. vocab_offsets[v + 1])
+       with id vocab_ids[v]; read only with ignore_merges (may be NULL otherwise) */
+    const uint8_t *vocab_bytes;
+    const int64_t *vocab_offsets;
+    const int32_t *vocab_ids;
+    int n_vocab;
+    const int32_t *byte_ids;     /* [256] the id of each byte's symbol */
+    const int32_t *merges;       /* [n_merges, 3] left id, right id, merged id; the rank is the row */
+    int n_merges;
+    /* added tokens: bytes, offsets, ids as in ac_tokenizer_spec, and flags bit 0 normalized (matched after the others,
+       inside the gaps they leave), bit 1 lstrip, bit 2 rstrip */
+    const uint8_t *added_bytes;
+    const int64_t *added_offsets;
+    const int32_t *added_ids;
+    const uint8_t *added_flags;
+    int n_added;
+    int cls_id, sep_id, pad_id;
+} ac_bpe_tokenizer_spec;
+
+int ac_tokenizer_create_bpe(const ac_bpe_tokenizer_spec *spec, ac_tokenizer **out);
+/* bytes of workspace ac_tokenize needs for B texts of text_bytes bytes in all (offsets[B] - offsets[0]) at max_length */
+int ac_tokenize_workspace_bytes_text(const ac_tokenizer *tok, int B, int64_t text_bytes, int max_length, size_t *bytes);
+
 /* ------------------------------------------------------------------------------------------
  * predict_batch() glue on the device (classifier.py:1329-1384) and the end-to-end pipeline.
  * ------------------------------------------------------------------------------------------ */
