@@ -32,6 +32,9 @@ AC_ENCODER_MAX_S = 512
 AC_MODERNBERT_MAX_S = 8192
 AC_PREC_TF32, AC_PREC_F16 = 0, 1
 AC_FFN_GELU_ERF, AC_FFN_GELU_TANH, AC_FFN_SWIGLU = 0, 1, 2
+AC_PROJ_EMB, AC_PROJ_QKV, AC_PROJ_WO, AC_PROJ_FFN1, AC_PROJ_W2, AC_PROJ_FFN1_ROWS = 0, 1, 2, 3, 4, 5
+_PROJ_ROLES = {0: "AC_PROJ_EMB", 1: "AC_PROJ_QKV", 2: "AC_PROJ_WO", 3: "AC_PROJ_FFN1", 4: "AC_PROJ_W2",
+               5: "AC_PROJ_FFN1_ROWS"}
 # hidden_act of a post-LN (BERT-family) config -> ac_encoder_config.ffn_act (SwiGLU is NomicBERT's alone: nomic_bert_settings)
 FFN_ACTS = {"gelu": AC_FFN_GELU_ERF, "gelu_new": AC_FFN_GELU_TANH, "gelu_pytorch_tanh": AC_FFN_GELU_TANH}
 
@@ -42,6 +45,7 @@ EXPORTS = [
     "ac_head_forward", "ac_head_train_workspace_bytes", "ac_head_train_step", "ac_head_train_epoch", "ac_head_phase_timing", "ac_head_train_plan", "ac_head_grad", "ac_ewc_penalty",
     "ac_strategic_workspace_bytes", "ac_strategic_best_response", "ac_head_train_strategic_workspace_bytes", "ac_head_train_strategic",
     "ac_encoder_create", "ac_encoder_destroy", "ac_encoder_forward_cls", "ac_encoder_last_hidden", "ac_encoder_attention",
+    "ac_encoder_projection",
     "ac_linear_tc",
     "ac_proto_class_scores", "ac_proto_class_scores_n", "ac_blend_dense", "ac_topk_desc_workspace_bytes", "ac_topk_desc", "ac_blend_topk",
     "ac_pipeline_create", "ac_pipeline_destroy", "ac_pipeline_predict_device", "ac_pipeline_predict_host",
@@ -165,6 +169,8 @@ def load_library() -> ctypes.CDLL:
     L.ac_encoder_forward_cls.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
     L.ac_encoder_last_hidden.argtypes = [c_void_p, c_void_p, c_int64, c_void_p]
     L.ac_encoder_attention.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    L.ac_encoder_projection.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_void_p]
     L.ac_linear_tc.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                c_int, c_int, c_void_p]
     L.ac_proto_class_scores.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]
@@ -1044,6 +1050,8 @@ class Encoder:
         self._L = L
         self.hidden = hidden
         self.heads = heads
+        self.intermediate = intermediate
+        self.embedding_size = embedding_size or hidden
         self.max_tokens = max_tokens
         dev = torch.device(device)
         keep = {}
@@ -1242,6 +1250,49 @@ class Encoder:
         check(self._L.ac_encoder_attention(self.handle, qk.data_ptr(), vT.data_ptr(), ptr(mask), B, S, window,
                                            1 if cls_rows else 0, ctx.data_ptr(), stream_ptr()), "ac_encoder_attention")
         return ctx.view(B, S, heads, dh)
+
+    def projection(self, role: int, layer: int, B: int, S: int, a: torch.Tensor, y: Optional[torch.Tensor] = None,
+                   stats: Optional[torch.Tensor] = None) -> tuple:
+        """Parity entry: one projection role of layer `layer` alone (ac_encoder_projection, AC_PROJ_*), as the forward runs it.
+        a [B*S, K] fp16 (K = E, H or I by role), y [B*S, H] fp32 residual sums, stats [B*S, 2] fp32 (mu, r) rows; all CUDA.
+        Returns, by role: EMB (y, fp16 y); QKV (q | k [B*S, 2H], V^T [B*H, S_pad]); WO / W2 (y_new, fp16 y_new, stats of
+        y_new [B*S, 2]); FFN1 / FFN1_ROWS (activations [B*S, I],)."""
+        M, H, dev = B * S, self.hidden, a.device
+        # the C entry copies M rows of each input: a tensor of another shape would be read out of bounds
+        name = _PROJ_ROLES.get(role, f"role {role}")
+        width = {AC_PROJ_EMB: self.embedding_size, AC_PROJ_W2: self.intermediate}.get(role, H)
+        need = {"a": (a, (M, width))}
+        if role in (AC_PROJ_QKV, AC_PROJ_WO, AC_PROJ_FFN1, AC_PROJ_W2):
+            need["stats"] = (stats, (M, 2))
+        if role in (AC_PROJ_WO, AC_PROJ_W2):
+            need["y"] = (y, (M, H))
+        for arg, (t, shape) in need.items():
+            if t is None or tuple(t.shape) != shape:
+                got = "None" if t is None else f"shape {tuple(t.shape)}"
+                raise AdaptiveB200Error(f"Encoder.projection: {arg} is {got}; {name} needs {shape} (B={B} S={S})")
+        for arg, (t, _) in need.items():
+            if not t.is_cuda:
+                raise AdaptiveB200Error(f"Encoder.projection: {arg} is on {t.device}; {name} needs CUDA tensors")
+        a = a.to(torch.float16).contiguous()
+        if y is not None:
+            y = y.to(torch.float32).contiguous()
+        if stats is not None:
+            stats = stats.to(torch.float32).contiguous()
+        new = lambda *shape, dt=torch.float16: torch.empty(shape, dtype=dt, device=dev)
+        stats_out = None
+        if role == AC_PROJ_EMB:
+            outs = (new(M, H, dt=torch.float32), new(M, H))
+        elif role == AC_PROJ_QKV:
+            outs = (new(M, 2 * H), new(B * H, (S + 7) // 8 * 8))
+        elif role in (AC_PROJ_WO, AC_PROJ_W2):
+            stats_out = new(M, 2, dt=torch.float32)
+            outs = (new(M, H, dt=torch.float32), new(M, H), stats_out)
+        else:
+            outs = (new(M, self.intermediate),)
+        check(self._L.ac_encoder_projection(self.handle, layer, role, B, S, a.data_ptr(), ptr(y), ptr(stats),
+                                            outs[0].data_ptr(), ptr(outs[1] if len(outs) > 1 else None), ptr(stats_out),
+                                            stream_ptr()), "ac_encoder_projection")
+        return outs
 
     def close(self):
         if getattr(self, "handle", None):

@@ -1968,6 +1968,79 @@ static int launch_linear(const CUtensorMap &ta, const CUtensorMap &tb, int M, in
     return launch_gemm_tc<Epi, false, GEMM_KIND_F16>(ta, tb, M, N, K, epi, s);
 }
 
+// ---- one function per projection role: forward_layers and the parity entry ac_encoder_projection both run these, so the
+// epilogue, operand maps, biases, tables and pending LayerNorm of a role are stated once.  M = B * S rows.
+
+// ALBERT / ELECTRA embedding projection: e->ctx (LayerNorm-ed embedding rows, width E) -> e->x, e->xh
+static int run_emb_proj(ac_encoder *e, int M, cudaStream_t s) {
+    const int H = e->cfg.hidden;
+    EpiEmbProj ep{.bias = e->emb_proj_b, .y = e->x, .yh = e->xh, .M = M, .N = H, .ld = H};
+    return launch_linear(e->m_emb, e->m_emb_proj, M, H, e->cfg.embedding_size, ep, s);
+}
+
+// fused QKV of layer l on e->xh with the consumed norm's row statistics `stats` -> q | k in e->qk (RoPE with the layer's
+// table: the sliding one in a ModernBERT sliding layer), V^T in e->vT
+template <bool ROPE>
+static int run_qkv(ac_encoder *e, int l, int B, int S, const float2 *stats, cudaStream_t s) {
+    const int H = e->cfg.hidden, M = B * S;
+    const Layer &ly = e->layers[l];
+    EpiQKV<ROPE> eq{.qk = {.bias = ly.c0qkv, .c1 = ly.c1qkv, .row_stats = stats, .Y = e->qk, .M = M, .N = 3 * H, .ldy = 2 * H,
+                           .S = S, .rope = e->rope[ly.window ? 1 : 0]},
+                    .vT = e->vT, .vt_col0 = 2 * H, .S_pad = (S + 7) / 8 * 8, .H = H};
+    return launch_linear(e->m_xh, ly.m_wqkv, M, 3 * H, H, eq, s);
+}
+
+// The LayerNorm pending on the residual sums when layer l's Wo (ffn = false) or W2 (ffn = true) adds them back, with the
+// sums' statistics `stats`: post-LN blocks leave the previous layer's output LayerNorm (nothing before layer 0) and the
+// layer's attention-output LayerNorm pending; pre-LN blocks keep the identity pending throughout.
+struct PendingNorm { const float2 *stats; const float *gamma, *beta; };
+template <bool PRE_LN>
+static PendingNorm pending_norm(const ac_encoder *e, int l, bool ffn, const float2 *stats) {
+    if (PRE_LN || (!ffn && l == 0)) return {e->stats_id, e->ones, e->zeros};
+    if (ffn) return {stats, e->layers[l].ln_ffn_w, e->layers[l].ln_ffn_b};
+    return {stats, e->layers[l - 1].ln_out_w, e->layers[l - 1].ln_out_b};
+}
+
+// residual projection of layer l, Wo on e->ctx (ffn = false) or W2 on e->ffn (ffn = true), in place on e->x / e->xh:
+// y <- a W^T + b + LN_pending(y), then the row statistics of the new sums into stats_out
+template <bool PRE_LN, Norm NORM>
+static int run_resid(ac_encoder *e, int l, bool ffn, int M, const float2 *stats, float2 *stats_out, cudaStream_t s) {
+    const ac_encoder_config &c = e->cfg;
+    const int H = c.hidden;
+    const int64_t pstride = static_cast<int64_t>(e->T);
+    const Layer &ly = e->layers[l];
+    const PendingNorm p = pending_norm<PRE_LN>(e, l, ffn, stats);
+    EpiResidDefer ep{.bias = ffn ? ly.b2 : ly.bo, .y = e->x, .yh = e->xh, .stats_prev = p.stats, .gamma = p.gamma, .beta = p.beta,
+                     .parts = e->parts, .part_stride = pstride, .M = M, .N = H, .ld = H};
+    int rc = launch_linear(ffn ? e->m_ffn : e->m_ctx, ffn ? ly.m_w2 : ly.m_wo, M, H, ffn ? c.intermediate : H, ep, s);
+    if (rc) return rc;
+    ln_stats_kernel<NORM><<<(M + 255) / 256, 256, 0, s>>>(e->parts, H / GEMM_EPI_COLS, pstride, M, H, c.ln_eps, stats_out);
+    AC_LAUNCH_CHECK();
+    return AC_OK;
+}
+
+// accumulator columns of FFN1 (GLU: activated + multiplier rows)
+template <Act FFN_ACT>
+static int ffn1_cols(const ac_encoder *e) {
+    return FFN_ACT == Act::GeGLU || FFN_ACT == Act::SwiGLU ? 2 * e->cfg.intermediate : e->cfg.intermediate;
+}
+
+// FFN1 of layer l on e->xh, consuming its pending norm with row statistics `stats` -> e->ffn
+template <Act FFN_ACT>
+static int run_ffn1(ac_encoder *e, int l, int M, const float2 *stats, cudaStream_t s) {
+    const Layer &ly = e->layers[l];
+    EpiF16<FFN_ACT, true> e1{.bias = ly.c0f, .c1 = ly.c1f, .row_stats = stats, .Y = e->ffn, .M = M, .N = ffn1_cols<FFN_ACT>(e),
+                             .ldy = e->cfg.intermediate};
+    return launch_linear(e->m_xh, ly.m_w1, M, e1.N, e->cfg.hidden, e1, s);
+}
+
+// FFN1 of the last layer on materialised LayerNorm rows (the CLS-only tail): the plain weight w1_last on `ta` -> out
+template <Act FFN_ACT>
+static int run_ffn1_rows(ac_encoder *e, const CUtensorMap &ta, __half *out, int M, cudaStream_t s) {
+    EpiF16<FFN_ACT, false> e1{.bias = e->b1_last, .Y = out, .M = M, .N = ffn1_cols<FFN_ACT>(e), .ldy = e->cfg.intermediate};
+    return launch_linear(ta, e->p_w1_last, M, e1.N, e->cfg.hidden, e1, s);
+}
+
 // The layer stack, for post-LN (BERT / RoBERTa / DistilBERT, modeling_bert.py) or pre-LN (ModernBERT,
 // modeling_modernbert.py ModernBertModel.forward; EuroBERT, modeling_eurobert.py, with RMSNorm and SwiGLU) blocks:
 //     post-LN   y = LN1(y + attn(y))               y = LN2(y + GELU-FFN(y))               out = y
@@ -1988,24 +2061,17 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
                          : NORM == Norm::Layer && FFN_ACT != Act::GeGLU,
                   "pre-LN blocks are ModernBERT's (LayerNorm, RoPE, GeGLU) and EuroBERT's (RMSNorm, RoPE, SwiGLU); post-LN "
                   "blocks use LayerNorm");
-    constexpr bool GLU = FFN_ACT == Act::GeGLU || FFN_ACT == Act::SwiGLU;
-    using EpiFfn1 = EpiF16<FFN_ACT, true>;
-    using EpiFfn1Rows = EpiF16<FFN_ACT, false>;                     // on materialised LayerNorm rows (CLS-only tail)
     const ac_encoder_config &c = e->cfg;
     const int H = c.hidden, I = c.intermediate, M = B * S;
-    const int N1 = GLU ? 2 * I : I;                                 // FFN1 accumulator columns (GLU: activated + multiplier)
     // a post-LN RoPE encoder's e->pos is one zero row: the embedding kernel's clamp to max_pos - 1 = 0 reads it
     const int emb_pos = (ROPE && !PRE_LN) ? 1 : c.max_pos;
-    const int S_pad = (S + 7) / 8 * 8;
     const int wpb = 8;
     const int row_blocks = (M + wpb - 1) / wpb;
-    const int nparts = H / GEMM_EPI_COLS;
-    const int64_t pstride = static_cast<int64_t>(e->T);
     const bool cls_tail = c.cls_only && static_cast<size_t>(B) <= e->Bc;
     int rc;
-    // the embeddings arrive normalised (or projected): identity LayerNorm pending, and identity statistics for layer 0's QKV;
-    // EuroBERT's arrive raw, with the RMS statistics of layer 0's input_layernorm in stats_a
-    const float2 *pst = e->stats_id, *st_qkv = e->stats_id;
+    // the embeddings arrive normalised (or projected): identity statistics for layer 0's QKV (and the identity LayerNorm
+    // pending, pending_norm); EuroBERT's arrive raw, with the RMS statistics of layer 0's input_layernorm in stats_a
+    const float2 *st_qkv = e->stats_id;
     if constexpr (NORM == Norm::Rms) {
         embed_ln_kernel<true, true><<<row_blocks, wpb * 32, 0, s>>>(ids, nullptr, e->word, nullptr, nullptr, nullptr, nullptr,
                                                                     c.ln_eps, B, S, H, c.arch, c.pad_idx, c.vocab, c.max_pos,
@@ -2024,35 +2090,19 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
                                                                e->emb_ln_b, c.ln_eps, B, S, E, c.arch, c.pad_idx, c.vocab,
                                                                c.max_pos, c.type_vocab, nullptr, e->ctx);
         AC_LAUNCH_CHECK();
-        EpiEmbProj ep{.bias = e->emb_proj_b, .y = e->x, .yh = e->xh, .M = M, .N = H, .ld = H};
-        if ((rc = launch_linear(e->m_emb, e->m_emb_proj, M, H, E, ep, s))) return rc;
+        if ((rc = run_emb_proj(e, M, s))) return rc;
     }
-    const float *pg = e->ones, *pb = e->zeros;
     for (int l = 0; l < c.layers; ++l) {
         const Layer &ly = e->layers[l];
-        EpiQKV<ROPE> eq{.qk = {.bias = ly.c0qkv, .c1 = ly.c1qkv, .row_stats = st_qkv, .Y = e->qk, .M = M, .N = 3 * H,
-                                 .ldy = 2 * H, .S = S, .rope = e->rope[ly.window ? 1 : 0]},
-                          .vT = e->vT, .vt_col0 = 2 * H, .S_pad = S_pad, .H = H};
-        if ((rc = launch_linear(e->m_xh, ly.m_wqkv, M, 3 * H, H, eq, s))) return rc;
+        if ((rc = run_qkv<ROPE>(e, l, B, S, st_qkv, s))) return rc;
         if ((rc = launch_attention(e, mask, B, S, ly.window, l == c.layers - 1 && cls_tail, l, s))) return rc;
         if (l == c.layers - 1 && cls_tail) break;
         // attention output projection + residual: y <- ctx Wo^T + bo + LN_pending(y); statistics of the new sums
-        EpiResidDefer eo{.bias = ly.bo, .y = e->x, .yh = e->xh, .stats_prev = pst, .gamma = pg, .beta = pb, .parts = e->parts,
-                         .part_stride = pstride, .M = M, .N = H, .ld = H};
-        if ((rc = launch_linear(e->m_ctx, ly.m_wo, M, H, H, eo, s))) return rc;
-        ln_stats_kernel<NORM><<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_b);
-        AC_LAUNCH_CHECK();
-        EpiFfn1 e1{.bias = ly.c0f, .c1 = ly.c1f, .row_stats = e->stats_b, .Y = e->ffn, .M = M, .N = N1, .ldy = I};
-        if ((rc = launch_linear(e->m_xh, ly.m_w1, M, N1, H, e1, s))) return rc;
-        if constexpr (!PRE_LN) { pst = e->stats_b; pg = ly.ln_ffn_w; pb = ly.ln_ffn_b; }
+        if ((rc = run_resid<PRE_LN, NORM>(e, l, false, M, e->stats_a, e->stats_b, s))) return rc;
+        if ((rc = run_ffn1<FFN_ACT>(e, l, M, e->stats_b, s))) return rc;
         // FFN output projection + residual: y <- ffn W2^T + b2 + LN_pending(y)
-        EpiResidDefer e2{.bias = ly.b2, .y = e->x, .yh = e->xh, .stats_prev = pst, .gamma = pg, .beta = pb, .parts = e->parts,
-                         .part_stride = pstride, .M = M, .N = H, .ld = H};
-        if ((rc = launch_linear(e->m_ffn, ly.m_w2, M, H, I, e2, s))) return rc;
-        ln_stats_kernel<NORM><<<(M + 255) / 256, 256, 0, s>>>(e->parts, nparts, pstride, M, H, c.ln_eps, e->stats_a);
-        AC_LAUNCH_CHECK();
+        if ((rc = run_resid<PRE_LN, NORM>(e, l, true, M, e->stats_b, e->stats_a, s))) return rc;
         st_qkv = e->stats_a;
-        if constexpr (!PRE_LN) { pst = e->stats_a; pg = ly.ln_out_w; pb = ly.ln_out_b; }
     }
     const Layer &last = e->layers.back();
     if (cls_tail) {
@@ -2061,18 +2111,18 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
         // LN1-normalised rows, pre-LN the raw sums; the output LayerNorm reads the new sums from `sum` and writes `res`.
         float *res = PRE_LN ? e->tmp_cls : e->x_cls, *sum = PRE_LN ? e->x_cls : e->tmp_cls;
         const int cb = (B + wpb - 1) / wpb;
-        if (pst == e->stats_id)   // identity pending: pre-LN, or the embeddings of a single-layer encoder
+        const PendingNorm p = pending_norm<PRE_LN>(e, c.layers - 1, false, e->stats_a);
+        if (p.stats == e->stats_id)   // identity pending: pre-LN, or the embeddings of a single-layer encoder
             gather_cls_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, e->ctx_cls, e->x_cls);
         else
-            gather_cls_ln_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, pg, pb, c.ln_eps, e->ctx_cls, e->x_cls);
+            gather_cls_ln_kernel<<<cb, wpb * 32, 0, s>>>(e->ctx, e->x, B, S, H, p.gamma, p.beta, c.ln_eps, e->ctx_cls, e->x_cls);
         AC_LAUNCH_CHECK();
         EpiF32<false, true> eo{.bias = last.bo, .residual = e->x_cls, .Y = e->tmp_cls, .M = B, .N = H, .ldy = H};
         if ((rc = launch_linear(e->m_ctx_cls, last.m_wo, B, H, H, eo, s))) return rc;
         layernorm_kernel<NORM><<<cb, wpb * 32, 0, s>>>(e->tmp_cls, last.ln_ffn_w, last.ln_ffn_b, c.ln_eps, B, H, PRE_LN ? nullptr : res,
                                                  e->xh_cls);
         AC_LAUNCH_CHECK();
-        EpiFfn1Rows e1{.bias = e->b1_last, .Y = e->ffn_cls, .M = B, .N = N1, .ldy = I};
-        if ((rc = launch_linear(e->m_xh_cls, e->p_w1_last, B, N1, H, e1, s))) return rc;
+        if ((rc = run_ffn1_rows<FFN_ACT>(e, e->m_xh_cls, e->ffn_cls, B, s))) return rc;
         EpiF32<false, true> e2{.bias = last.b2, .residual = res, .Y = sum, .M = B, .N = H, .ldy = H};
         if ((rc = launch_linear(e->m_ffn_cls, last.m_w2, B, H, I, e2, s))) return rc;
         layernorm_kernel<NORM><<<cb, wpb * 32, 0, s>>>(sum, last.ln_out_w, last.ln_out_b, c.ln_eps, B, H, res, nullptr);
@@ -2088,6 +2138,28 @@ static int forward_layers(ac_encoder *e, const int32_t *ids, const int32_t *mask
     e->last_S = S;
     e->last_cls_only = cls_tail;
     return AC_OK;
+}
+
+// The block kind of a handle's architecture as forward_layers' template arguments: f(BlockKind<..>{}) with the handle's.
+template <bool PRE_LN_, bool ROPE_, Act FFN_ACT_, Norm NORM_>
+struct BlockKind {
+    static constexpr bool PRE_LN = PRE_LN_, ROPE = ROPE_;
+    static constexpr Act FFN_ACT = FFN_ACT_;
+    static constexpr Norm NORM = NORM_;
+};
+template <class F>
+static int with_block_kind(const ac_encoder *e, F &&f) {
+    constexpr Norm LN = Norm::Layer;
+    const ac_encoder_config &c = e->cfg;
+    if (c.arch == AC_ARCH_MODERNBERT) return f(BlockKind<true, true, Act::GeGLU, LN>{});
+    if (c.arch == AC_ARCH_EUROBERT) return f(BlockKind<true, true, Act::SwiGLU, Norm::Rms>{});
+    if (c.arch == AC_ARCH_ROTARY) {
+        if (c.ffn_act == AC_FFN_SWIGLU) return f(BlockKind<false, true, Act::SwiGLU, LN>{});
+        if (c.ffn_act == AC_FFN_GELU_TANH) return f(BlockKind<false, true, Act::GeluTanh, LN>{});
+        return f(BlockKind<false, true, Act::Gelu, LN>{});
+    }
+    if (c.ffn_act == AC_FFN_GELU_TANH) return f(BlockKind<false, false, Act::GeluTanh, LN>{});
+    return f(BlockKind<false, false, Act::Gelu, LN>{});
 }
 
 // Shape checks every entry that runs attention shares, then the V^T view of a (B, S) call: rows (b, h, d), S_pad keys per
@@ -2149,21 +2221,73 @@ extern "C" int ac_encoder_forward_cls(ac_encoder *e, const int32_t *ids, const i
     int rc = check_shape_map_vt(e, "ac_encoder_forward_cls", B, S);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    constexpr Norm LN = Norm::Layer;
-    if (e->cfg.arch == AC_ARCH_MODERNBERT)
-        return forward_layers<true, true, Act::GeGLU, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-    if (e->cfg.arch == AC_ARCH_EUROBERT)
-        return forward_layers<true, true, Act::SwiGLU, Norm::Rms>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-    if (e->cfg.arch == AC_ARCH_ROTARY) {
-        if (e->cfg.ffn_act == AC_FFN_SWIGLU)
-            return forward_layers<false, true, Act::SwiGLU, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-        if (e->cfg.ffn_act == AC_FFN_GELU_TANH)
-            return forward_layers<false, true, Act::GeluTanh, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-        return forward_layers<false, true, Act::Gelu, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-    }
-    if (e->cfg.ffn_act == AC_FFN_GELU_TANH)
-        return forward_layers<false, false, Act::GeluTanh, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
-    return forward_layers<false, false, Act::Gelu, LN>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    return with_block_kind(e, [&](auto k) {
+        using K = decltype(k);
+        return forward_layers<K::PRE_LN, K::ROPE, K::FFN_ACT, K::NORM>(e, ids, mask, type_ids, B, S, out_unit_cls, s);
+    });
+}
+
+// parity entry: one projection role of layer `layer` on caller-supplied inputs, through the handle's own packed operands,
+// buffers and the role functions forward_layers runs (include/adaptive_b200.h)
+extern "C" int ac_encoder_projection(ac_encoder *e, int layer, int role, int B, int S, const void *a, const float *y,
+                                     const float *stats, void *out0, void *out1, float *stats_out, ac_stream_t stream) {
+    AC_REQUIRE(e && a && out0, "ac_encoder_projection: null argument");
+    const ac_encoder_config &c = e->cfg;
+    AC_REQUIRE(role >= AC_PROJ_EMB && role <= AC_PROJ_FFN1_ROWS, "ac_encoder_projection: unknown role=%d", role);
+    AC_REQUIRE(layer >= 0 && layer < c.layers, "ac_encoder_projection: layer=%d outside 0..%d", layer, c.layers - 1);
+    AC_REQUIRE(role != AC_PROJ_EMB || e->emb_proj_w, "ac_encoder_projection: AC_PROJ_EMB needs an encoder with an embedding "
+                                                     "projection (emb_proj_w)");
+    AC_REQUIRE(role != AC_PROJ_FFN1_ROWS || c.cls_only, "ac_encoder_projection: AC_PROJ_FFN1_ROWS needs a cls_only encoder");
+    AC_REQUIRE(B > 0 && S > 0 && static_cast<int64_t>(B) * S <= c.max_tokens,
+               "ac_encoder_projection: B=%d S=%d: B*S must be in 1..max_tokens=%d", B, S, c.max_tokens);
+    const bool resid = role == AC_PROJ_WO || role == AC_PROJ_W2;
+    AC_REQUIRE((role == AC_PROJ_EMB || role == AC_PROJ_FFN1_ROWS || stats) && (!resid || (y && stats_out)) &&
+                   (role == AC_PROJ_FFN1 || role == AC_PROJ_FFN1_ROWS || out1),
+               "ac_encoder_projection: role=%d lacks one of stats, y, out1, stats_out", role);
+    int rc;
+    if (role == AC_PROJ_QKV && (rc = check_shape_map_vt(e, "ac_encoder_projection", B, S))) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const size_t M = static_cast<size_t>(B) * S, H = c.hidden, I = c.intermediate, h2 = sizeof(__half);
+    const auto copy = [&](void *dst, const void *src, size_t bytes) {
+        return check_cuda(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s), "ac_encoder_projection copy");
+    };
+    const float2 *st_in = reinterpret_cast<const float2 *>(stats);
+    return with_block_kind(e, [&](auto k) -> int {
+        using K = decltype(k);
+        int rc;
+        switch (role) {
+        case AC_PROJ_EMB:
+            if ((rc = copy(e->ctx, a, M * c.embedding_size * h2)) || (rc = run_emb_proj(e, static_cast<int>(M), s)) ||
+                (rc = copy(out0, e->x, M * H * sizeof(float))))
+                return rc;
+            return copy(out1, e->xh, M * H * h2);
+        case AC_PROJ_QKV:
+            if ((rc = copy(e->xh, a, M * H * h2)) || (rc = copy(e->stats_a, stats, M * sizeof(float2))) ||
+                (rc = run_qkv<K::ROPE>(e, layer, B, S, e->stats_a, s)) || (rc = copy(out0, e->qk, M * 2 * H * h2)))
+                return rc;
+            return copy(out1, e->vT, B * H * ((S + 7) / 8 * 8) * h2);
+        case AC_PROJ_FFN1:
+            if ((rc = copy(e->xh, a, M * H * h2)) || (rc = copy(e->stats_b, stats, M * sizeof(float2))) ||
+                (rc = run_ffn1<K::FFN_ACT>(e, layer, static_cast<int>(M), e->stats_b, s)))
+                return rc;
+            return copy(out0, e->ffn, M * I * h2);
+        case AC_PROJ_FFN1_ROWS:
+            AC_REQUIRE(layer == c.layers - 1, "ac_encoder_projection: AC_PROJ_FFN1_ROWS is the last layer's (layer=%d)", layer);
+            if ((rc = copy(e->xh, a, M * H * h2)) || (rc = run_ffn1_rows<K::FFN_ACT>(e, e->m_xh, e->ffn, static_cast<int>(M), s)))
+                return rc;
+            return copy(out0, e->ffn, M * I * h2);
+        default: {   // AC_PROJ_WO, AC_PROJ_W2: the residual sums y and their statistics in, the new sums and theirs out
+            const bool ffn = role == AC_PROJ_W2;
+            float2 *st = ffn ? e->stats_b : e->stats_a;
+            if ((rc = copy(ffn ? e->ffn : e->ctx, a, M * (ffn ? I : H) * h2)) || (rc = copy(e->x, y, M * H * sizeof(float))) ||
+                (rc = copy(st, st_in, M * sizeof(float2))) ||
+                (rc = run_resid<K::PRE_LN, K::NORM>(e, layer, ffn, static_cast<int>(M), st, ffn ? e->stats_a : e->stats_b, s)) ||
+                (rc = copy(out0, e->x, M * H * sizeof(float))) || (rc = copy(out1, e->xh, M * H * h2)))
+                return rc;
+            return copy(stats_out, ffn ? e->stats_a : e->stats_b, M * sizeof(float2));
+        }
+        }
+    });
 }
 
 // parity entry: the attention stage alone, through the handle's own buffers, V^T view and launch_attention

@@ -399,6 +399,27 @@ int ac_encoder_last_hidden(ac_encoder *enc, float *out, int64_t n_floats, ac_str
 int ac_encoder_attention(ac_encoder *enc, const void *qk, const void *vT, const int32_t *mask, int B, int S, int window,
                          int cls_rows, void *ctx_out, ac_stream_t stream);
 
+/* debugging / parity: run one projection of layer `layer` alone on caller-supplied inputs, with this encoder's packed
+ * operands, buffers and fused epilogue, exactly as ac_encoder_forward_cls runs it.  M = B*S <= max_tokens rows; fp16
+ * arrays are row-major, stats / stats_out are [M] (mu, r) float pairs (RMSNorm: (0, r)).
+ *   AC_PROJ_EMB        a = LayerNorm-ed embedding rows [M, E] fp16 -> out0 y = a Wp^T + bp [M, H] fp32, out1 fp16(y)
+ *                      (encoders with an embedding projection only)
+ *   AC_PROJ_QKV        a = fp16 residual sums [M, H], stats of the norm the layer's QKV consumes ((0, 1) where that is
+ *                      the identity) -> out0 q | k [M, 2H] fp16 (RoPE with the layer's table on rotary encoders), out1 V^T
+ *                      [B*H, S_pad] fp16 at (b*H + feature) * S_pad + key, S_pad = roundup(S, 8); pad keys unspecified
+ *   AC_PROJ_WO, _W2    a = attention context [M, H] / FFN activations [M, I] fp16, y = residual sums [M, H] fp32 and
+ *                      their stats -> out0 y_new = a W^T + b + LN_pending(y) [M, H] fp32, out1 fp16(y_new), stats_out the
+ *                      statistics of y_new.  LN_pending is what the forward leaves pending there: post-LN, the previous
+ *                      layer's output LayerNorm before Wo (the identity in layer 0) and the attention-output LayerNorm
+ *                      before W2; pre-LN, the identity (stats are then not read)
+ *   AC_PROJ_FFN1       a = fp16 residual sums [M, H], stats of the norm FFN1 consumes -> out0 activations [M, I] fp16
+ *   AC_PROJ_FFN1_ROWS  the CLS-only tail's FFN1 (cls_only encoders, last layer): a = normalised rows [M, H] fp16 -> out0
+ *                      activations [M, I] fp16
+ * Unused pointers may be NULL.  Overwrites the handle's activation buffers.  All pointers DEVICE. */
+enum { AC_PROJ_EMB = 0, AC_PROJ_QKV = 1, AC_PROJ_WO = 2, AC_PROJ_FFN1 = 3, AC_PROJ_W2 = 4, AC_PROJ_FFN1_ROWS = 5 };
+int ac_encoder_projection(ac_encoder *enc, int layer, int role, int B, int S, const void *a, const float *y,
+                          const float *stats, void *out0, void *out1, float *stats_out, ac_stream_t stream);
+
 /* generic tensor-core linear (the encoder's GEMM with its fused epilogues), exposed for parity tests and roofline
  * measurement: Y[M,N] = epi(X[M,K] W[N,K]^T + bias) (+ residual).  epi: 0 bias, 1 bias+GELU(erf), 2 bias+fp32 residual,
  * 3 bias+GELU(tanh) (AC_PREC_F16 with out_half != 0 only), 4 SwiGLU (AC_PREC_F16 with out_half != 0, N % 64 == 0): W's

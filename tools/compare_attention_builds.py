@@ -9,7 +9,11 @@ a process of its own, and compares the outputs with torch.equal.  One encoder pe
 (ModernBERT three: one full, two sliding), three sequences of lengths S, S - 37 and min(S, 90) under a padding mask:
 
     BERT-base shape (head_dim 64)   S 128, 384      MPNet       S 128, 384      ModernBERT (half-window 64)   S 1024
-    MiniLM shape (head_dim 32)      S 128, 384      DeBERTa-v3  S 77, 384
+    MiniLM shape (head_dim 32)      S 128, 384      DeBERTa-v3  S 77, 384       EuroBERT (RMSNorm, SwiGLU)    S 128, 384
+    ALBERT (E = 128, tanh GELU)     S 128, 384      NomicBERT (post-LN RoPE, SwiGLU)  S 128, 384
+
+so that every layer-loop instantiation (post-LN with erf / tanh GELU, with RoPE and SwiGLU, the embedding projection;
+pre-LN with LayerNorm / GeGLU and RMSNorm / SwiGLU) runs.
 
 Per case: `Encoder.forward_cls` (unit CLS rows, fp32) and `Encoder.attention` on seeded q, k, v (the stage alone, fp16; with
 the sliding half-window on ModernBERT).  Prints one line per case and exits 1 if any bit differs.  Writes only to a
@@ -31,7 +35,8 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 VOCAB = 2000
-CASES = (("bert", (128, 384)), ("minilm", (128, 384)), ("mpnet", (128, 384)), ("deberta", (77, 384)), ("modernbert", (1024,)))
+CASES = (("bert", (128, 384)), ("minilm", (128, 384)), ("mpnet", (128, 384)), ("deberta", (77, 384)), ("modernbert", (1024,)),
+         ("eurobert", (128, 384)), ("albert", (128, 384)), ("nomic", (128, 384)))
 
 
 def model(name):
@@ -55,6 +60,19 @@ def model(name):
         with torch.no_grad():          # N(0, 1) relative embeddings, so that the position terms move the scores
             m.encoder.rel_embeddings.weight.normal_(0.0, 1.0)
         return m
+    if name == "eurobert":
+        cfg = tf.EuroBertConfig(vocab_size=VOCAB, hidden_size=768, num_hidden_layers=2, num_attention_heads=12,
+                                num_key_value_heads=4, intermediate_size=2048, max_position_embeddings=8192, bos_token_id=0,
+                                eos_token_id=2, pad_token_id=1, mask_token_id=3)
+        return tf.EuroBertModel(cfg).eval()
+    if name == "albert":
+        cfg = tf.AlbertConfig(vocab_size=VOCAB, embedding_size=128, hidden_size=768, num_hidden_layers=2,
+                              num_attention_heads=12, intermediate_size=3072, hidden_act="gelu_new")
+        return tf.AlbertModel(cfg, add_pooling_layer=False).eval()
+    if name == "nomic":
+        cfg = tf.NomicBertConfig(vocab_size=VOCAB, hidden_size=768, num_hidden_layers=2, num_attention_heads=12,
+                                 intermediate_size=3072, max_position_embeddings=2048, type_vocab_size=2)
+        return tf.NomicBertModel(cfg).eval()
     cfg = tf.ModernBertConfig(vocab_size=VOCAB, num_hidden_layers=3, pad_token_id=VOCAB - 1, bos_token_id=VOCAB - 3,
                               eos_token_id=VOCAB - 2, cls_token_id=VOCAB - 3, sep_token_id=VOCAB - 2)
     return tf.ModernBertModel(cfg).eval()
