@@ -12,7 +12,7 @@ only (EuroBertModel.forward takes no token_type_ids).
     eurobert_long   make_golden_xlmr_long.main's recipe with max_length 1024 (texts past 512 tokens)
 Every value is rounded through bfloat16 and the norm weights are moved off 1.  Both runs use the same seeded checkpoint; its
 tensors are stored once, spread over golden_classifier_eurobert_bert0 .. _bert3.npz so that every file stays under 1 MB
-(tests/test_eurobert_cpu.py::load_golden reads them back for either run).
+(tests/golden_npz.py::load reads them back for either run, with weights_from for the long one).
 """
 import os
 import sys

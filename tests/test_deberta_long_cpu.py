@@ -137,18 +137,11 @@ def test_box_memory_of_the_base_and_large_shapes():
 
 
 # ------------------------------------------------------------------------------------------------ golden
-def _golden_long():
-    g = golden_npz.load("golden_classifier_deberta_long")
-    w = golden_npz.load("golden_classifier_deberta")
-    assert json.loads(str(g["bert_config"])) == json.loads(str(w["bert_config"]))
-    g.update({k: w[k] for k in w.files if k.startswith("bert_") and k != "bert_config"})
-    return g
-
-
 def test_deberta_oracle_reproduces_reference_embeddings_at_max_length_1024():
     from transformers import DebertaV2Config
-    g = _golden_long()
+    g = golden_npz.load("golden_classifier_deberta_long", weights_from="golden_classifier_deberta")
     cfgd = json.loads(str(g["bert_config"]))
+    assert cfgd == json.loads(str(golden_npz.load("golden_classifier_deberta")["bert_config"]))
     c = DebertaV2Config(**{k: v for k, v in cfgd.items() if k not in ("model_type", "transformers_version", "architectures")})
     sd = {k[5:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("bert_") and k != "bert_config"}
     ids = torch.from_numpy(g["input_ids"])

@@ -9,7 +9,6 @@
   * eurobert_settings, remote-code and ac_encoder_create refusals, which run before any device call"""
 import ctypes
 import json
-import os
 import re
 
 import numpy as np
@@ -55,15 +54,6 @@ def sd_of(m):
 def hf_forward(m, ids, mask):
     with torch.no_grad():
         return m(input_ids=ids, attention_mask=mask).last_hidden_state
-
-
-def load_golden(name):
-    """a golden run with the tiny checkpoint both runs share (stored once with golden_classifier_eurobert)"""
-    g = golden_npz.load(name)
-    for i in range(4):
-        with np.load(os.path.join(golden_npz.GOLD, f"golden_classifier_eurobert_bert{i}.npz")) as z:
-            g.update({k: z[k] for k in z.files})
-    return g
 
 
 @pytest.mark.parametrize("kv", [4, 2, 1])
@@ -136,7 +126,7 @@ def test_sequence_limit_follows_max_position_embeddings(cabi, mpe, expect):
 # ------------------------------------------------------------------------------------------------ goldens
 @pytest.mark.parametrize("name", ["golden_classifier_eurobert", "golden_classifier_eurobert_long"])
 def test_golden_embeddings_match_the_oracle(name):
-    golden = load_golden(name)
+    golden = golden_npz.load(name, weights_from="golden_classifier_eurobert")
     cfg = json.loads(str(golden["bert_config"]))
     sd = {k[5:]: torch.from_numpy(golden[k]).float() for k in golden.files if k.startswith("bert_") and k != "bert_config"}
     ids = torch.from_numpy(golden["input_ids"]).long()

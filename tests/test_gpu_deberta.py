@@ -1,7 +1,7 @@
 """GPU tests of the DeBERTa-v3 encoders (deberta-v3-xsmall / small / base / large, mdeberta-v3-base: the post-LN BERT block
 with disentangled c2p + p2c attention) against the fp32 oracle of oracle/deberta_oracle.py (pinned to HF DebertaV2Model by
-tests/test_deberta_cpu.py), HF itself on the CPU, an fp64 reference of the attention stage alone, and the reference's own
-classifier outputs on the golden DeBERTa checkpoint; then the CUDA-graph pipeline step and the drop-in classifier.
+tests/test_deberta_cpu.py), HF itself on the CPU and an fp64 reference of the attention stage alone.  The golden classifier
+run, the CUDA-graph pipeline step and the drop-in classifier on a local checkpoint are tests/test_gpu_encoder_families.py's.
 
 Attention-stage bound, per output element (test_gpu_attention.py's, plus one term for the score arithmetic):
 
@@ -14,16 +14,13 @@ Attention-stage bound, per output element (test_gpu_attention.py's, plus one ter
 import json
 import math
 
-import numpy as np
 import pytest
 import torch
 
-import golden_npz
 from oracle import deberta_oracle as do
-from test_deberta_cpu import deberta_ids, deberta_model, deberta_tokenizer_words
+from test_deberta_cpu import deberta_ids, deberta_model
 from test_gpu_attention import attended_ref
 from test_gpu_minilm import _check_cls
-from test_gpu_parity import _head, _synthetic_index
 
 pytestmark = pytest.mark.gpu
 
@@ -202,141 +199,3 @@ def test_deberta_attention_at_every_block_seam(cabi, S):
 def test_deberta_attention_report_fractions():
     """prints the largest error seen per family as a fraction of the bound (recorded in DESIGN.md)"""
     print("deberta attention error / bound:", json.dumps({k: round(v, 3) for k, v in sorted(FRACTIONS.items())}))
-
-
-# ------------------------------------------------------------------------------------------------ golden classifier
-@pytest.fixture(scope="module")
-def golden():
-    return golden_npz.load("golden_classifier_deberta")
-
-
-@pytest.fixture(scope="module")
-def trained(cabi, golden, tmp_path_factory):
-    """the tiny seeded 2-head x 64 DeBERTa-v3 checkpoint + tokenizer the reference ran on, through the drop-in classifier"""
-    from transformers import DebertaV2Config, DebertaV2Model
-    import adaptive_classifier_b200 as acb
-    d = str(tmp_path_factory.mktemp("golden_deberta"))
-    cfgd = json.loads(str(golden["bert_config"]))
-    cfg = DebertaV2Config(**{k: v for k, v in cfgd.items() if k not in ("model_type", "transformers_version",
-                                                                         "architectures")})
-    m = DebertaV2Model(cfg)
-    m.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("bert_") and k != "bert_config"})
-    m.save_pretrained(d)
-    deberta_tokenizer_words(golden["vocab"].tolist()[5:]).save_pretrained(d)
-    texts, labels = golden["texts"].tolist(), golden["labels"].tolist()
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda")
-    clf.add_examples(texts[:24], labels[:24])
-    clf.add_examples(texts[24:], labels[24:])
-    return clf
-
-
-def test_deberta_classifier_embeddings_and_prototypes_match_reference(trained, golden):
-    emb = torch.stack(trained._get_embeddings(golden["texts"].tolist())).numpy()
-    ref = golden["emb_train"]
-    assert emb.shape == ref.shape
-    assert np.abs(emb - ref).max() < 3e-4 and np.linalg.norm(emb - ref, axis=1).max() < 1e-3
-    names = golden["label_names"].tolist()
-    assert [trained.id_to_label[i] for i in range(len(names))] == names
-    assert trained.training_history == json.loads(str(golden["training_history"]))
-    protos = np.stack([trained.memory.prototypes[l].numpy() for l in sorted(trained.memory.prototypes)])
-    assert golden["proto_labels"].tolist() == sorted(trained.memory.prototypes)
-    assert np.abs(protos - golden["prototypes"]).max() < 3e-4
-
-
-def test_deberta_classifier_predictions_match_reference_with_the_reference_trained_head(trained, golden, tmp_path):
-    """predict / predict_batch with the reference-trained head, then the same answers after a save / load round trip"""
-    import adaptive_classifier_b200 as acb
-    names = golden["label_names"].tolist()
-    own_head = {k: v.detach().clone() for k, v in trained.adaptive_head.state_dict().items()}
-    trained.adaptive_head.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("head_")})
-    tests_ = golden["test_texts"].tolist()
-
-    def cmp(preds, L, S):
-        for p, l_row, s_row in zip(preds, L, S):
-            exp = [(names[i], s) for i, s in zip(l_row.tolist(), s_row.tolist()) if i >= 0]
-            assert [l for l, _ in p] == [l for l, _ in exp], (p, exp)
-            assert np.allclose([s for _, s in p], [s for _, s in exp], atol=1e-3), (p, exp)
-
-    try:
-        cmp([trained.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"])
-        cmp([trained.predict(t, k=1) for t in tests_], golden["pred_k1_labels"], golden["pred_k1_scores"])
-        cmp(trained.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"])
-        out = str(tmp_path / "saved")
-        trained.save(out)
-        clf2 = acb.AdaptiveClassifier.load(out, device="cuda")
-        assert clf2.label_to_id == trained.label_to_id
-        cmp([clf2.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"])
-        cmp(clf2.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"])
-    finally:
-        trained.adaptive_head.load_state_dict(own_head)
-
-
-# ------------------------------------------------------------------------------------------------ downstream
-def test_pipeline_host_step_replayed_as_a_cuda_graph_equals_the_eager_step_deberta(cabi):
-    """a 3-layer DeBERTa encoder, 768-wide prototypes and head: the captured host step replays like the device step"""
-    m = deberta_model(num_hidden_layers=3, **WIDE)
-    Bmax, S, N, D, C, k = 8, 64, 3000, 768, 20, 5
-    P, _ = _synthetic_index(N, D, C)
-    enc = _deberta_encoder(cabi, m, Bmax * S)
-    _, pg = _head(D, C)
-    row_class = (torch.arange(N) % C).to(torch.int32).cuda()
-    pl = cabi.Pipeline(enc, P.cuda(), Bmax, S, k, head=pg, row_class=row_class)
-    for rep, B in enumerate([3, 3, 3, 3, 8, 8, 8, 1, 1]):
-        ids, _ = deberta_ids(B, S, False, vocab=WIDE["vocab_size"], seed=100 + rep)
-        ids = ids.to(torch.int32)
-        oc_h, osc_h = pl.predict_host(ids.pin_memory())
-        oc_h, osc_h = oc_h.clone(), osc_h.clone()
-        oc, osc = pl.predict_device(ids.cuda())
-        torch.cuda.synchronize()
-        assert torch.equal(oc.cpu(), oc_h) and torch.equal(osc.cpu(), osc_h), (rep, B)
-    emb, _, _ = pl.debug_views(1)
-    ids, _ = deberta_ids(1, S, False, vocab=WIDE["vocab_size"], seed=108)
-    ref = do.deberta_forward_cls(_hf_sd(m), ids, None, m.config)
-    assert (emb.cpu() - ref).norm(dim=1).max() < 1e-3
-    pl.close(); enc.close()
-
-
-def test_adaptive_classifier_on_a_local_deberta_checkpoint(cabi, tmp_path):
-    """AdaptiveClassifier on a fabricated local DeBERTa-v3 checkpoint directory (DebertaV2Model + DebertaV2Tokenizer, loaded
-    through AutoModel / AutoTokenizer): add_examples, predict, predict_batch and a save / load round trip; the embeddings
-    equal the fp32 oracle's"""
-    import adaptive_classifier_b200 as acb
-    words = [f"w{i}" for i in range(195)]
-    tok = deberta_tokenizer_words(words)
-    m = deberta_model(seed=77, num_hidden_layers=4, proj_scale=2.0, hidden_size=768, num_attention_heads=12,
-                      intermediate_size=3072, vocab_size=5 + len(words))
-    with torch.no_grad():
-        m.embeddings.word_embeddings.weight.mul_(4.0)
-        m.embeddings.word_embeddings.weight[1].zero_()
-    d = str(tmp_path / "deberta")
-    m.save_pretrained(d)
-    tok.save_pretrained(d)
-    rng = np.random.default_rng(3)
-    classes = {"a": words[0:60], "b": words[60:120], "c": words[120:180]}
-    texts, labels = [], []
-    for lab, ws in classes.items():
-        for _ in range(8):
-            texts.append(" ".join(rng.choice(ws, size=int(rng.integers(5, 12)))))
-            labels.append(lab)
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda")
-    assert clf.embedding_dim == 768
-    clf.add_examples(texts[:16], labels[:16])
-    clf.add_examples(texts[16:], labels[16:])
-    emb = torch.stack(clf._get_embeddings(texts[:6]))
-    enc = clf.tokenizer(texts[:6], max_length=512, truncation=True, padding=True, return_tensors="pt")
-    ref = do.deberta_forward_cls(_hf_sd(m), enc["input_ids"], enc["attention_mask"], m.config)
-    assert (emb - ref).norm(dim=1).max() < 1e-3
-    queries = [" ".join(rng.choice(ws, size=9)) for ws in classes.values()]
-    single = [clf.predict(q, k=3) for q in queries]
-    batch = clf.predict_batch(queries, k=3)
-    assert len(batch) == len(queries)
-    for p in single + batch:
-        assert 1 <= len(p) <= 3 and {l for l, _ in p} <= {"a", "b", "c"} and abs(sum(s for _, s in p) - 1.0) < 1e-5
-    out = str(tmp_path / "saved")
-    clf.save(out)
-    clf2 = acb.AdaptiveClassifier.load(out, device="cuda")
-    assert clf2.embedding_dim == 768 and clf2.label_to_id == clf.label_to_id
-    for p, p2 in zip(single + batch, [clf2.predict(q, k=3) for q in queries] + clf2.predict_batch(queries, k=3)):
-        assert [l for l, _ in p2] == [l for l, _ in p] and np.allclose([s for _, s in p2], [s for _, s in p], atol=1e-5)

@@ -1,20 +1,16 @@
 """GPU tests of DeBERTa-v3 encoders past 512 tokens (handles built with rel_radius AC_MODERNBERT_MAX_S: relative operand
 boxes of block offsets -D .. D, larger offsets clamped to +-D): the attention stage alone against the fp64 reference and
 per-element bound of test_gpu_deberta.py, bit equality with radius-512 handles at S <= 512, whole encoders against the
-fp32 oracle up to 8192 tokens, the refusals, the reference's golden classifier at max_length 1024 and the CUDA-graph
-pipeline step."""
-import json
+fp32 oracle up to 8192 tokens and the refusals.  The reference's golden classifier at max_length 1024 and the CUDA-graph
+pipeline step at S = 1024 are tests/test_gpu_encoder_families.py's."""
 import math
 
-import numpy as np
 import pytest
 import torch
 
-import golden_npz
 from oracle import deberta_oracle as do
-from test_deberta_cpu import deberta_ids, deberta_model, deberta_tokenizer_words
+from test_deberta_cpu import deberta_ids, deberta_model
 from test_gpu_deberta import WIDE, _mask, _qkv
-from test_gpu_parity import _head, _synthetic_index
 
 pytestmark = pytest.mark.gpu
 
@@ -239,107 +235,3 @@ def test_refusals(cabi):
     dims["rel_index_long"] = cabi.deberta_rel_index(256, 512, LONG)[0]
     with pytest.raises(cabi.AdaptiveB200Error, match="all-zero pos_emb"):
         cabi.Encoder(sd, arch="deberta", max_tokens=1024, **dims)
-
-
-# ------------------------------------------------------------------------------------------------ golden classifier
-@pytest.fixture(scope="module")
-def golden():
-    g = golden_npz.load("golden_classifier_deberta_long")
-    w = golden_npz.load("golden_classifier_deberta")
-    assert json.loads(str(g["bert_config"])) == json.loads(str(w["bert_config"]))
-    g.update({k: w[k] for k in w.files if k.startswith("bert_") and k != "bert_config"})
-    return g
-
-
-@pytest.fixture(scope="module")
-def trained(cabi, golden, tmp_path_factory):
-    """the golden DeBERTa-v3 checkpoint + tokenizer through the drop-in classifier at max_length 1024"""
-    from transformers import DebertaV2Config, DebertaV2Model
-    import adaptive_classifier_b200 as acb
-    d = str(tmp_path_factory.mktemp("golden_deberta_long"))
-    cfgd = json.loads(str(golden["bert_config"]))
-    cfg = DebertaV2Config(**{k: v for k, v in cfgd.items() if k not in ("model_type", "transformers_version",
-                                                                         "architectures")})
-    m = DebertaV2Model(cfg)
-    m.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("bert_") and k != "bert_config"})
-    m.save_pretrained(d)
-    deberta_tokenizer_words(golden["vocab"].tolist()[5:]).save_pretrained(d)
-    texts, labels = golden["texts"].tolist(), golden["labels"].tolist()
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda", config={"max_length": int(golden["max_length"])})
-    clf.add_examples(texts[:12], labels[:12])
-    clf.add_examples(texts[12:], labels[12:])
-    return clf
-
-
-def test_long_classifier_embeddings_and_prototypes_match_reference(trained, golden):
-    enc = trained.tokenizer(golden["texts"].tolist() + golden["test_texts"].tolist(), max_length=1024, truncation=True,
-                            padding=True, return_tensors="pt")
-    assert torch.equal(enc["input_ids"].to(torch.int32), torch.from_numpy(golden["input_ids"]))
-    emb = torch.stack(trained._get_embeddings(golden["texts"].tolist())).numpy()
-    ref = golden["emb_train"]
-    assert emb.shape == ref.shape
-    assert np.abs(emb - ref).max() < 3e-4 and np.linalg.norm(emb - ref, axis=1).max() < 1e-3
-    emb_t = torch.stack(trained._get_embeddings(golden["test_texts"].tolist())).numpy()
-    assert np.linalg.norm(emb_t - golden["emb_test"], axis=1).max() < 1e-3
-    names = golden["label_names"].tolist()
-    assert [trained.id_to_label[i] for i in range(len(names))] == names
-    assert trained.training_history == json.loads(str(golden["training_history"]))
-    protos = np.stack([trained.memory.prototypes[l].numpy() for l in sorted(trained.memory.prototypes)])
-    assert golden["proto_labels"].tolist() == sorted(trained.memory.prototypes)
-    assert np.abs(protos - golden["prototypes"]).max() < 3e-4
-
-
-def test_long_classifier_predictions_match_reference_with_the_reference_trained_head(trained, golden, tmp_path):
-    """predict / predict_batch with the reference-trained head, then the same answers after a save / load round trip"""
-    import adaptive_classifier_b200 as acb
-    names = golden["label_names"].tolist()
-    own_head = {k: v.detach().clone() for k, v in trained.adaptive_head.state_dict().items()}
-    trained.adaptive_head.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("head_")})
-    tests_ = golden["test_texts"].tolist()
-
-    def cmp(preds, L, S):
-        for p, l_row, s_row in zip(preds, L, S):
-            exp = [(names[i], s) for i, s in zip(l_row.tolist(), s_row.tolist()) if i >= 0]
-            assert [l for l, _ in p] == [l for l, _ in exp], (p, exp)
-            assert np.allclose([s for _, s in p], [s for _, s in exp], atol=1e-3), (p, exp)
-
-    try:
-        cmp([trained.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"])
-        cmp([trained.predict(t, k=1) for t in tests_], golden["pred_k1_labels"], golden["pred_k1_scores"])
-        cmp(trained.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"])
-        out = str(tmp_path / "saved")
-        trained.save(out)
-        clf2 = acb.AdaptiveClassifier.load(out, device="cuda")
-        assert clf2.label_to_id == trained.label_to_id and clf2.config.max_length == 1024
-        cmp([clf2.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"])
-        cmp(clf2.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"])
-    finally:
-        trained.adaptive_head.load_state_dict(own_head)
-
-
-# ------------------------------------------------------------------------------------------------ downstream
-def test_pipeline_host_step_replayed_as_a_cuda_graph_equals_the_eager_step_deberta_1024(cabi):
-    """a 3-layer DeBERTa encoder at S = 1024, 768-wide prototypes and head: the captured host step replays like the device
-    step"""
-    m = deberta_model(num_hidden_layers=3, **WIDE)
-    Bmax, S, N, D, C, k = 4, 1024, 3000, 768, 20, 5
-    P, _ = _synthetic_index(N, D, C)
-    sd, dims = _dims(cabi, m)
-    enc = cabi.Encoder(sd, arch="deberta", max_tokens=Bmax * S, **dims)
-    _, pg = _head(D, C)
-    row_class = (torch.arange(N) % C).to(torch.int32).cuda()
-    pl = cabi.Pipeline(enc, P.cuda(), Bmax, S, k, head=pg, row_class=row_class)
-    for rep, B in enumerate([3, 3, 3, 4, 4, 1, 1]):
-        ids, _ = deberta_ids(B, S, False, vocab=WIDE["vocab_size"], seed=100 + rep)
-        ids = ids.to(torch.int32)
-        oc_h, osc_h = pl.predict_host(ids.pin_memory())
-        oc_h, osc_h = oc_h.clone(), osc_h.clone()
-        oc, osc = pl.predict_device(ids.cuda())
-        torch.cuda.synchronize()
-        assert torch.equal(oc.cpu(), oc_h) and torch.equal(osc.cpu(), osc_h), (rep, B)
-    emb, _, _ = pl.debug_views(1)
-    ids, _ = deberta_ids(1, S, False, vocab=WIDE["vocab_size"], seed=106)
-    ref = _oracle(m, ids, None)
-    assert (emb.cpu() - ref).norm(dim=1).max() < 1e-3
-    pl.close(); enc.close()

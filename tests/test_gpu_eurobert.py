@@ -8,19 +8,16 @@ TINY_BOUND (tiny models) and SHAPE_BOUND (eurobert_210m, the goldens) instead of
     TF32 off: S <= 512 with cls_only on and off and the full hidden state, S up to 8192 with both paddings and a mask hole,
     with and without grouped-query attention, a single layer, and a residual stream with rows up to ~1e4
   * the eurobert_210m shape at B = 512 x 128 (sampled rows), 1 x 8192 and 2 x 2048
-  * from_hf against HF, the S > max_pos refusal, the reference's classifier outputs (goldens of
-    oracle/make_golden_eurobert.py) with save / load through AdaptiveClassifier on a local checkpoint directory, and the
-    CUDA-graph replay of the pipeline step"""
-import json
-
+  * from_hf against HF, the S > max_pos refusal, and AdaptiveClassifier with max_length 8192 on the golden runs' local
+    checkpoint directory
+The reference's classifier outputs (goldens of oracle/make_golden_eurobert.py) and the CUDA-graph replay of the pipeline
+step are tests/test_gpu_encoder_families.py's."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import eurobert_oracle as eo
-from test_eurobert_cpu import GPU_UNIT_BOUND as TINY_BOUND, load_golden, padded_batch, tiny_model
-from test_gpu_parity import _head, _synthetic_index
-from test_gpu_rotary import _cmp
+from test_eurobert_cpu import GPU_UNIT_BOUND as TINY_BOUND, padded_batch, tiny_model
 
 pytestmark = pytest.mark.gpu
 SHAPE_BOUND = 2.5e-3
@@ -189,105 +186,19 @@ def test_eurobert_210m_long_matches_oracle(cabi, B, S, pad):
     _check(out, ref, SHAPE_BOUND)
 
 
-# ------------------------------------------------------------------------------------------------ pipeline
-@pytest.mark.parametrize("S", [128, 1024])
-def test_pipeline_host_step_replayed_as_a_cuda_graph_equals_the_eager_step(cabi, S):
-    m = tiny_model(seed=3, layers=3, kv=2)
-    Bmax, N, D, C, k = 8, 3000, 256, 20, 5
-    P, _ = _synthetic_index(N, D, C)
-    enc = cabi.Encoder.from_hf(m, max_tokens=Bmax * S)
-    _, pg = _head(D, C)
-    row_class = (torch.arange(N) % C).to(torch.int32).cuda()
-    pl = cabi.Pipeline(enc, P.cuda(), Bmax, S, k, head=pg, row_class=row_class)
-    for rep, B in enumerate([3, 3, 3, 3, 8, 8, 8]):
-        ids = torch.randint(5, 300, (B, S), generator=torch.Generator().manual_seed(100 + rep)).to(torch.int32)
-        oc_h, osc_h = pl.predict_host(ids.pin_memory())
-        oc_h, osc_h = oc_h.clone(), osc_h.clone()
-        oc, osc = pl.predict_device(ids.cuda())
-        torch.cuda.synchronize()
-        assert torch.equal(oc.cpu(), oc_h) and torch.equal(osc.cpu(), osc_h), (rep, B)
-    pl.close(); enc.close()
-
-
-# ------------------------------------------------------------------------------------------------ the reference's classifier
-def _golden_checkpoint(golden, d):
-    """the tiny seeded checkpoint and the tokenizer the golden run used, saved to directory d"""
-    from transformers import EuroBertConfig, EuroBertModel
-    cfgd = json.loads(str(golden["bert_config"]))
-    cfgd = {k: v for k, v in cfgd.items() if k not in ("model_type", "transformers_version", "architectures")}
-    sd = {k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("bert_") and k != "bert_config"}
-    m = EuroBertModel(EuroBertConfig(**cfgd))
-    m.load_state_dict(sd)
-    m.save_pretrained(d)
-    vocab = golden["vocab"].tolist() if "vocab" in golden else golden["vocab_pieces"].tolist()
-    assert vocab[:len(eo.SPECIALS)] == eo.SPECIALS
-    eo.eurobert_tokenizer(vocab[len(eo.SPECIALS):]).save_pretrained(d)
-
-
+# ------------------------------------------------------------------------------------------------ max_length 8192
 @pytest.fixture(scope="module", params=["golden_classifier_eurobert", "golden_classifier_eurobert_long"])
 def golden_run(cabi, request, tmp_path_factory):
-    """AdaptiveClassifier on the local checkpoint directory the reference ran on (AutoModel / AutoTokenizer); the long run
-    with max_length 8192 would tokenize the same texts the same way (the longest is under 1024 tokens only after
-    truncation), so it uses the reference's 1024"""
-    import adaptive_classifier_b200 as acb
-    golden = load_golden(request.param)
+    """the local checkpoint directory a golden run of the reference used (AutoModel / AutoTokenizer), and the run"""
+    from test_gpu_encoder_families import golden_checkpoint
     d = str(tmp_path_factory.mktemp(request.param))
-    _golden_checkpoint(golden, d)
-    texts, labels = golden["texts"].tolist(), golden["labels"].tolist()
-    half = 24 if "max_length" not in golden else 12
-    config = {} if "max_length" not in golden else {"max_length": int(golden["max_length"]), "b200_max_tokens": 4096}
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda", config=config)
-    clf.add_examples(texts[:half], labels[:half])
-    clf.add_examples(texts[half:], labels[half:])
-    return clf, golden, d
-
-
-def test_classifier_embeddings_and_prototypes_match_reference(golden_run):
-    trained, golden, _ = golden_run
-    ids, mask, tt = trained._tokenize(golden["texts"].tolist() + golden["test_texts"].tolist())
-    assert tt is None and torch.equal(ids.long(), torch.from_numpy(golden["input_ids"]).long())
-    emb = torch.stack(trained._get_embeddings(golden["texts"].tolist())).numpy()
-    ref = golden["emb_train"]
-    assert emb.shape == ref.shape
-    assert np.linalg.norm(emb - ref, axis=1).max() < SHAPE_BOUND
-    emb_t = torch.stack(trained._get_embeddings(golden["test_texts"].tolist())).numpy()
-    assert np.linalg.norm(emb_t - golden["emb_test"], axis=1).max() < SHAPE_BOUND
-    names = golden["label_names"].tolist()
-    assert [trained.id_to_label[i] for i in range(len(names))] == names
-    protos = np.stack([trained.memory.prototypes[l].numpy() for l in sorted(trained.memory.prototypes)])
-    assert golden["proto_labels"].tolist() == sorted(trained.memory.prototypes)
-    assert np.linalg.norm(protos - golden["prototypes"], axis=1).max() < SHAPE_BOUND
-
-
-def test_classifier_predictions_match_reference_and_survive_save_load(golden_run, tmp_path):
-    import adaptive_classifier_b200 as acb
-    trained, golden, _ = golden_run
-    names = golden["label_names"].tolist()
-    own_head = {k: v.detach().clone() for k, v in trained.adaptive_head.state_dict().items()}
-    trained.adaptive_head.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("head_")})
-    tests_ = golden["test_texts"].tolist()
-    try:
-        _cmp([trained.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"], names)
-        _cmp([trained.predict(t, k=1) for t in tests_], golden["pred_k1_labels"], golden["pred_k1_scores"], names)
-        _cmp(trained.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"], names)
-        before = [trained.predict(t, k=3) for t in tests_]
-        out = str(tmp_path / "saved")
-        trained.save(out)
-        clf2 = acb.AdaptiveClassifier.load(out, device="cuda")
-        assert clf2.label_to_id == trained.label_to_id
-        after = [clf2.predict(t, k=3) for t in tests_]
-        for p, p2 in zip(before, after):
-            assert [l for l, _ in p2] == [l for l, _ in p]
-            assert np.allclose([s for _, s in p2], [s for _, s in p], atol=1e-5)
-    finally:
-        trained.adaptive_head.load_state_dict(own_head)
+    return golden_checkpoint(request.param, d), d
 
 
 def test_classifier_with_max_length_8192_embeds_trains_predicts_saves_and_loads(golden_run, tmp_path):
     """AdaptiveClassifier(<local EuroBERT checkpoint>, config={"max_length": 8192}) on texts of up to ~6000 tokens"""
     import adaptive_classifier_b200 as acb
-    _, golden, d = golden_run
+    golden, d = golden_run
     words = golden["vocab"].tolist()[4:] if "vocab" in golden else golden["vocab_pieces"].tolist()[4:]
     rng = np.random.default_rng(3)
     classes = {"a": words[0:60], "b": words[60:120]}

@@ -1,19 +1,16 @@
 """GPU tests of the head_dim-32 encoders (all-MiniLM-L6/L12-v2, BGE-small, E5-small, GTE-small: BertModel with 384 hidden =
 12 heads of 32) against the fp32 oracle of oracle/encoder_oracle.py (pinned to HF BertModel at that shape by
-tests/test_minilm_cpu.py), HF itself on the CPU, and the reference's own classifier outputs on the golden head_dim-32
-checkpoint; then the D = 384 stages downstream of the encoder (kNN, CUDA-graph pipeline step, head training, the drop-in
-classifier)."""
-import json
-
+tests/test_minilm_cpu.py) and HF itself on the CPU; then the D = 384 stages downstream of the encoder (kNN, head
+training).  The golden classifier run, the CUDA-graph pipeline step and the drop-in classifier on a local checkpoint are
+tests/test_gpu_encoder_families.py's."""
 import numpy as np
 import pytest
 import torch
 
-import golden_npz
 from oracle import encoder_oracle as eo
 from oracle import head_oracle as ho
 from oracle import knn_oracle as ko
-from test_gpu_parity import _encoder, _head, _perturb_layernorms, _synthetic_index
+from test_gpu_parity import _encoder, _head, _perturb_layernorms
 
 pytestmark = pytest.mark.gpu
 
@@ -161,67 +158,6 @@ def test_minilm_bert_through_from_hf_matches_hf(cabi):
     enc.close()
 
 
-# ------------------------------------------------------------------------------------------------ golden classifier
-@pytest.fixture(scope="module")
-def golden():
-    return golden_npz.load("golden_classifier_minilm")
-
-
-@pytest.fixture(scope="module")
-def trained(cabi, golden, tmp_path_factory):
-    """the tiny seeded 4-head x 32 checkpoint + vocab the reference ran on, driven through the drop-in classifier"""
-    from transformers import BertConfig, BertModel, BertTokenizerFast
-    import adaptive_classifier_b200 as acb
-    d = str(tmp_path_factory.mktemp("golden_minilm"))
-    cfg = BertConfig(**{k: v for k, v in json.loads(str(golden["bert_config"])).items()
-                        if k in ("vocab_size", "hidden_size", "num_hidden_layers", "num_attention_heads",
-                                 "intermediate_size", "max_position_embeddings", "type_vocab_size", "pad_token_id")})
-    assert cfg.hidden_size // cfg.num_attention_heads == 32
-    m = BertModel(cfg)
-    m.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("bert_") and k != "bert_config"})
-    m.save_pretrained(d)
-    BertTokenizerFast(vocab={w: i for i, w in enumerate(golden["vocab"].tolist())}, do_lower_case=True).save_pretrained(d)
-    texts, labels = golden["texts"].tolist(), golden["labels"].tolist()
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda")
-    clf.add_examples(texts[:24], labels[:24])
-    clf.add_examples(texts[24:], labels[24:])
-    return clf
-
-
-def test_minilm_classifier_embeddings_and_prototypes_match_reference(trained, golden):
-    emb = torch.stack(trained._get_embeddings(golden["texts"].tolist())).numpy()
-    ref = golden["emb_train"]
-    assert emb.shape == ref.shape
-    assert np.abs(emb - ref).max() < 3e-4 and np.linalg.norm(emb - ref, axis=1).max() < 1e-3
-    names = golden["label_names"].tolist()
-    assert [trained.id_to_label[i] for i in range(len(names))] == names
-    assert trained.training_history == json.loads(str(golden["training_history"]))
-    protos = np.stack([trained.memory.prototypes[l].numpy() for l in sorted(trained.memory.prototypes)])
-    assert golden["proto_labels"].tolist() == sorted(trained.memory.prototypes)
-    assert np.abs(protos - golden["prototypes"]).max() < 3e-4
-
-
-def test_minilm_classifier_predictions_match_reference_with_the_reference_trained_head(trained, golden):
-    names = golden["label_names"].tolist()
-    own_head = {k: v.detach().clone() for k, v in trained.adaptive_head.state_dict().items()}
-    trained.adaptive_head.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("head_")})
-    tests_ = golden["test_texts"].tolist()
-
-    def cmp(preds, L, S):
-        for p, l_row, s_row in zip(preds, L, S):
-            exp = [(names[i], s) for i, s in zip(l_row.tolist(), s_row.tolist()) if i >= 0]
-            assert [l for l, _ in p] == [l for l, _ in exp], (p, exp)
-            assert np.allclose([s for _, s in p], [s for _, s in exp], atol=1e-3), (p, exp)
-
-    try:
-        cmp([trained.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"])
-        cmp([trained.predict(t, k=1) for t in tests_], golden["pred_k1_labels"], golden["pred_k1_scores"])
-        cmp(trained.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"])
-    finally:
-        trained.adaptive_head.load_state_dict(own_head)
-
-
 # ------------------------------------------------------------------------------------------------ D = 384 downstream
 @pytest.mark.parametrize("k", [5, 1000])
 def test_knn_tensor_path_at_d384_equals_oracle(cabi, k):
@@ -242,28 +178,6 @@ def test_knn_tensor_path_at_d384_equals_oracle(cabi, k):
     assert bool((d1[:, 1:] >= d1[:, :-1]).all())
     d_ref, i_ref = ko.knn_l2(Q[sel[:16]].cpu().numpy(), P.cpu().numpy(), k)
     assert np.array_equal(i1[sel[:16]].cpu().numpy(), i_ref) and np.array_equal(d1[sel[:16]].cpu().numpy(), d_ref)
-
-
-def test_pipeline_host_step_replayed_as_a_cuda_graph_equals_the_eager_step_minilm(cabi):
-    """a 3-layer MiniLM-shaped encoder, 384-wide prototypes and head: the captured step replays like the 768-wide one"""
-    sd, cfg = _minilm(3)
-    Bmax, S, N, D, C, k = 8, 64, 3000, 384, 20, 5
-    P, _ = _synthetic_index(N, D, C)
-    enc = _encoder(cabi, sd, cfg, max_tokens=Bmax * S)
-    _, pg = _head(D, C)
-    row_class = (torch.arange(N) % C).to(torch.int32).cuda()
-    pl = cabi.Pipeline(enc, P.cuda(), Bmax, S, k, head=pg, row_class=row_class)
-    for rep, B in enumerate([3, 3, 3, 3, 8, 8, 8, 1, 1]):
-        ids = eo.synthetic_ids(B, S, seed=100 + rep).to(torch.int32)
-        oc_h, osc_h = pl.predict_host(ids.pin_memory())
-        oc_h, osc_h = oc_h.clone(), osc_h.clone()
-        oc, osc = pl.predict_device(ids.cuda())
-        torch.cuda.synchronize()
-        assert torch.equal(oc.cpu(), oc_h) and torch.equal(osc.cpu(), osc_h), (rep, B)
-    emb, _, _ = pl.debug_views(1)
-    ref = eo.encoder_forward_cls(sd, eo.synthetic_ids(1, S, seed=108), None, num_heads=12)
-    assert (emb.cpu() - ref).norm(dim=1).max() < 1e-3
-    pl.close(); enc.close()
 
 
 def test_head_train_steps_match_oracle_at_d384(cabi):
@@ -296,52 +210,3 @@ def test_head_train_steps_match_oracle_at_d384(cabi):
             solid = grads[k].abs() > 1e-6 * grads[k].abs().max()
             assert diff[solid].max() < 2e-5, (step, k, float(diff[solid].max()))
             assert diff.max() <= 2.1e-3 * step, (step, k)
-
-
-def test_adaptive_classifier_on_a_minilm_shaped_checkpoint(cabi, tmp_path):
-    """AdaptiveClassifier on a local seeded 6 x 384 / 12-head checkpoint directory: add_examples, predict, predict_batch and a
-    save / load round trip; the embeddings equal the fp32 oracle's"""
-    from transformers import BertConfig, BertModel, BertTokenizerFast
-    import adaptive_classifier_b200 as acb
-    words = [f"w{i}" for i in range(195)]
-    vocab = ["[PAD]", "[UNK]", "[CLS]", "[SEP]", "[MASK]"] + words
-    torch.manual_seed(77)
-    cfg = BertConfig(vocab_size=len(vocab), num_hidden_layers=6, max_position_embeddings=64, **MINILM)
-    m = BertModel(cfg).eval()
-    with torch.no_grad():
-        m.embeddings.word_embeddings.weight.mul_(4.0)
-        m.embeddings.word_embeddings.weight[2].zero_()
-        m.embeddings.position_embeddings.weight[0].zero_()
-        m.embeddings.token_type_embeddings.weight.zero_()
-    d = str(tmp_path / "minilm")
-    m.save_pretrained(d)
-    BertTokenizerFast(vocab={w: i for i, w in enumerate(vocab)}, do_lower_case=True).save_pretrained(d)
-    rng = np.random.default_rng(3)
-    classes = {"a": words[0:60], "b": words[60:120], "c": words[120:180]}
-    texts, labels = [], []
-    for lab, ws in classes.items():
-        for _ in range(8):
-            texts.append(" ".join(rng.choice(ws, size=int(rng.integers(5, 12)))))
-            labels.append(lab)
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda")
-    assert clf.embedding_dim == 384
-    clf.add_examples(texts[:16], labels[:16])
-    clf.add_examples(texts[16:], labels[16:])
-    emb = torch.stack(clf._get_embeddings(texts[:6]))
-    enc = clf.tokenizer(texts[:6], max_length=512, truncation=True, padding=True, return_tensors="pt")
-    sd = {k: v.detach().float() for k, v in m.state_dict().items()}
-    ref = eo.encoder_forward_cls(sd, enc["input_ids"], enc["attention_mask"], num_heads=12, ln_eps=cfg.layer_norm_eps)
-    assert (emb - ref).norm(dim=1).max() < 1e-3
-    queries = [" ".join(rng.choice(ws, size=9)) for ws in classes.values()]
-    single = [clf.predict(q, k=3) for q in queries]
-    batch = clf.predict_batch(queries, k=3)
-    assert len(batch) == len(queries)
-    for p in single + batch:
-        assert 1 <= len(p) <= 3 and {l for l, _ in p} <= {"a", "b", "c"} and abs(sum(s for _, s in p) - 1.0) < 1e-5
-    out = str(tmp_path / "saved")
-    clf.save(out)
-    clf2 = acb.AdaptiveClassifier.load(out, device="cuda")
-    assert clf2.embedding_dim == 384 and clf2.label_to_id == clf.label_to_id
-    for p, p2 in zip(single + batch, [clf2.predict(q, k=3) for q in queries] + clf2.predict_batch(queries, k=3)):
-        assert [l for l, _ in p2] == [l for l, _ in p] and np.allclose([s for _, s in p2], [s for _, s in p], atol=1e-5)

@@ -1,15 +1,11 @@
 """GPU tests of the ModernBERT encoder (pre-LN blocks, RoPE and GeGLU epilogues, sliding-window attention) against the fp32
-oracle of oracle/modernbert_oracle.py (pinned to HF ModernBertModel by tests/test_modernbert_cpu.py), the reference's own
-classifier outputs on the golden ModernBERT checkpoint, and the CUDA-graph replay of the pipeline step."""
-import json
-
-import numpy as np
+oracle of oracle/modernbert_oracle.py (pinned to HF ModernBertModel by tests/test_modernbert_cpu.py).  The reference's
+classifier outputs on the golden ModernBERT checkpoint and the CUDA-graph replay of the pipeline step are
+tests/test_gpu_encoder_families.py's."""
 import pytest
 import torch
 
-import golden_npz
 from oracle import modernbert_oracle as eo
-from test_gpu_parity import _head, _synthetic_index
 
 pytestmark = pytest.mark.gpu
 
@@ -130,77 +126,3 @@ def test_modernbert_published_shapes(cabi, name, B, S, pad):
     out = enc.forward_cls(ids.to(torch.int32).cuda(), mask.to(torch.int32).cuda()).cpu()
     _check(out, ref)
     enc.close()
-
-
-@pytest.fixture(scope="module")
-def golden():
-    return golden_npz.load("golden_classifier_modernbert")
-
-
-@pytest.fixture(scope="module")
-def trained(cabi, golden, tmp_path_factory):
-    """the tiny seeded ModernBERT checkpoint + vocab the reference ran on, driven through the drop-in classifier"""
-    from transformers import BertTokenizerFast, ModernBertConfig, ModernBertModel
-    import adaptive_classifier_b200 as acb
-    d = str(tmp_path_factory.mktemp("golden_modernbert"))
-    m = ModernBertModel(ModernBertConfig(**json.loads(str(golden["bert_config"]))))
-    m.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("bert_") and k != "bert_config"})
-    m.save_pretrained(d)
-    tok = BertTokenizerFast(vocab={w: i for i, w in enumerate(golden["vocab"].tolist())}, do_lower_case=True)
-    tok.model_input_names = ["input_ids", "attention_mask"]
-    tok.save_pretrained(d)
-    texts, labels = golden["texts"].tolist(), golden["labels"].tolist()
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda")
-    clf.add_examples(texts[:24], labels[:24])
-    clf.add_examples(texts[24:], labels[24:])
-    return clf
-
-
-def test_classifier_embeddings_and_prototypes_match_reference(trained, golden):
-    emb = torch.stack(trained._get_embeddings(golden["texts"].tolist())).numpy()
-    ref = golden["emb_train"]
-    assert emb.shape == ref.shape
-    assert np.abs(emb - ref).max() < 3e-4 and np.linalg.norm(emb - ref, axis=1).max() < 1e-3
-    names = golden["label_names"].tolist()
-    assert [trained.id_to_label[i] for i in range(len(names))] == names
-    protos = np.stack([trained.memory.prototypes[l].numpy() for l in sorted(trained.memory.prototypes)])
-    assert golden["proto_labels"].tolist() == sorted(trained.memory.prototypes)
-    assert np.abs(protos - golden["prototypes"]).max() < 3e-4
-
-
-def test_classifier_predictions_match_reference_with_the_reference_trained_head(trained, golden):
-    names = golden["label_names"].tolist()
-    own_head = {k: v.detach().clone() for k, v in trained.adaptive_head.state_dict().items()}
-    trained.adaptive_head.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("head_")})
-    tests_ = golden["test_texts"].tolist()
-
-    def cmp(preds, L, S):
-        for p, l_row, s_row in zip(preds, L, S):
-            exp = [(names[i], s) for i, s in zip(l_row.tolist(), s_row.tolist()) if i >= 0]
-            assert [l for l, _ in p] == [l for l, _ in exp], (p, exp)
-            assert np.allclose([s for _, s in p], [s for _, s in exp], atol=1e-3), (p, exp)
-
-    cmp([trained.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"])
-    cmp([trained.predict(t, k=1) for t in tests_], golden["pred_k1_labels"], golden["pred_k1_scores"])
-    cmp(trained.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"])
-    trained.adaptive_head.load_state_dict(own_head)
-
-
-def test_pipeline_host_step_replayed_as_a_cuda_graph_equals_the_eager_step_modernbert(cabi):
-    """the RoPE tables are built at create time, so the ModernBERT step captures and replays like the BERT one"""
-    m = _model(3, hidden_size=768, num_attention_heads=12, intermediate_size=1152, num_hidden_layers=3, vocab_size=1000)
-    Bmax, S, N, D, C, k = 8, 160, 3000, 768, 20, 5
-    P, _ = _synthetic_index(N, D, C)
-    enc = cabi.Encoder.from_hf(m, max_tokens=Bmax * S)
-    _, pg = _head(D, C)
-    row_class = (torch.arange(N) % C).to(torch.int32).cuda()
-    pl = cabi.Pipeline(enc, P.cuda(), Bmax, S, k, head=pg, row_class=row_class)
-    for rep, B in enumerate([3, 3, 3, 3, 8, 8, 8]):
-        ids = _ids(B, S, 1000, 100 + rep, False)[0].to(torch.int32)
-        oc_h, osc_h = pl.predict_host(ids.pin_memory())
-        oc_h, osc_h = oc_h.clone(), osc_h.clone()
-        oc, osc = pl.predict_device(ids.cuda())
-        torch.cuda.synchronize()
-        assert torch.equal(oc.cpu(), oc_h) and torch.equal(osc.cpu(), osc_h), (rep, B)
-    pl.close(); enc.close()

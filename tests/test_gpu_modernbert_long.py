@@ -1,17 +1,13 @@
 """GPU tests of ModernBERT at 512 < S <= 8192 (the streamed one-pass attention kernel and max_pos-row RoPE tables) against
 the query-block fp32 oracle of oracle/modernbert_long_oracle.py (pinned to HF ModernBertModel by
-tests/test_modernbert_long_cpu.py), run on the GPU in fp32 with TF32 off; the reference's classifier outputs with
-max_length 1024; the unchanged S <= 512 results; and the CUDA-graph replay of the pipeline step at S = 1024."""
-import json
-
-import numpy as np
+tests/test_modernbert_long_cpu.py), run on the GPU in fp32 with TF32 off; the unchanged S <= 512 results; the refusals.
+The reference's classifier outputs with max_length 1024 and the CUDA-graph replay of the pipeline step at S = 1024 are
+tests/test_gpu_encoder_families.py's."""
 import pytest
 import torch
 
-import golden_npz
 from oracle.modernbert_long_oracle import modernbert_forward_cls_blocked
 from test_gpu_modernbert import _check, _ids, _model
-from test_gpu_parity import _head, _synthetic_index
 
 pytestmark = pytest.mark.gpu
 
@@ -130,101 +126,3 @@ def test_bert_past_512_and_modernbert_past_max_pos_are_refused(cabi):
     with pytest.raises(cabi.AdaptiveB200Error, match="max_pos=1024"):
         enc.forward_cls(torch.full((1, 1025), 7, dtype=torch.int32, device="cuda"))
     enc.close()
-
-
-@pytest.fixture(scope="module")
-def golden():
-    return golden_npz.load("golden_classifier_modernbert_long")
-
-
-@pytest.fixture(scope="module")
-def ckpt(golden, tmp_path_factory):
-    """the tiny seeded ModernBERT checkpoint (weights of golden_classifier_modernbert, max_position_embeddings 8192)"""
-    from transformers import BertTokenizerFast, ModernBertConfig, ModernBertModel
-    d = str(tmp_path_factory.mktemp("golden_modernbert_long"))
-    w = golden_npz.load("golden_classifier_modernbert")
-    m = ModernBertModel(ModernBertConfig(**json.loads(str(golden["bert_config"]))))
-    m.load_state_dict({k[5:]: torch.from_numpy(w[k]) for k in w.files if k.startswith("bert_") and k != "bert_config"})
-    m.save_pretrained(d)
-    tok = BertTokenizerFast(vocab={w: i for i, w in enumerate(golden["vocab"].tolist())}, do_lower_case=True)
-    tok.model_input_names = ["input_ids", "attention_mask"]
-    tok.save_pretrained(d)
-    return d
-
-
-@pytest.fixture(scope="module")
-def trained(cabi, golden, ckpt):
-    """driven through the drop-in classifier with max_length 1024; a 4096-token workspace makes _embed_ids_device split the
-    1024-token batches into chunks of 4 sequences"""
-    import adaptive_classifier_b200 as acb
-    texts, labels = golden["texts"].tolist(), golden["labels"].tolist()
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(ckpt, device="cuda", config={"max_length": int(golden["max_length"]), "b200_max_tokens": 4096})
-    clf.add_examples(texts[:12], labels[:12])
-    clf.add_examples(texts[12:], labels[12:])
-    return clf
-
-
-def test_long_classifier_embeddings_and_prototypes_match_reference(trained, golden):
-    ids, _, _ = trained._tokenize(golden["texts"].tolist() + golden["test_texts"].tolist())
-    assert torch.equal(ids, torch.from_numpy(golden["input_ids"]))        # truncation at 1024 and padding as the reference
-    emb = torch.stack(trained._get_embeddings(golden["texts"].tolist())).numpy()
-    ref = golden["emb_train"]
-    assert emb.shape == ref.shape
-    assert np.abs(emb - ref).max() < 3e-4 and np.linalg.norm(emb - ref, axis=1).max() < 1e-3
-    emb_t = torch.stack(trained._get_embeddings(golden["test_texts"].tolist())).numpy()
-    assert np.abs(emb_t - golden["emb_test"]).max() < 3e-4
-    names = golden["label_names"].tolist()
-    assert [trained.id_to_label[i] for i in range(len(names))] == names
-    protos = np.stack([trained.memory.prototypes[l].numpy() for l in sorted(trained.memory.prototypes)])
-    assert golden["proto_labels"].tolist() == sorted(trained.memory.prototypes)
-    assert np.abs(protos - golden["prototypes"]).max() < 3e-4
-
-
-def _cmp(preds, L, S, names):
-    for p, l_row, s_row in zip(preds, L, S):
-        exp = [(names[i], s) for i, s in zip(l_row.tolist(), s_row.tolist()) if i >= 0]
-        assert [l for l, _ in p] == [l for l, _ in exp], (p, exp)
-        assert np.allclose([s for _, s in p], [s for _, s in exp], atol=1e-3), (p, exp)
-
-
-def test_long_classifier_predictions_match_reference_and_survive_save_load(trained, golden, tmp_path):
-    import adaptive_classifier_b200 as acb
-    names = golden["label_names"].tolist()
-    own_head = {k: v.detach().clone() for k, v in trained.adaptive_head.state_dict().items()}
-    trained.adaptive_head.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("head_")})
-    tests_ = golden["test_texts"].tolist()
-    try:
-        _cmp([trained.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"], names)
-        _cmp([trained.predict(t, k=1) for t in tests_], golden["pred_k1_labels"], golden["pred_k1_scores"], names)
-        _cmp(trained.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"], names)
-        before = [trained.predict(t, k=3) for t in tests_]
-        out = str(tmp_path / "saved")
-        trained.save(out)
-        clf2 = acb.AdaptiveClassifier.load(out, device="cuda")
-        assert clf2.config.max_length == 1024
-        after = [clf2.predict(t, k=3) for t in tests_]
-        for p, p2 in zip(before, after):
-            assert [l for l, _ in p2] == [l for l, _ in p] and np.allclose([s for _, s in p2], [s for _, s in p], atol=1e-5)
-    finally:
-        trained.adaptive_head.load_state_dict(own_head)
-
-
-def test_pipeline_host_step_replayed_as_a_cuda_graph_equals_the_eager_step_at_1024(cabi):
-    """the streamed attention kernel captures and replays like the S <= 512 ones"""
-    m = _model(3, hidden_size=768, num_attention_heads=12, intermediate_size=1152, num_hidden_layers=3, vocab_size=1000,
-               local_attention=128, max_position_embeddings=8192)
-    Bmax, S, N, D, C, k = 8, 1024, 3000, 768, 20, 5
-    P, _ = _synthetic_index(N, D, C)
-    enc = cabi.Encoder.from_hf(m, max_tokens=Bmax * S)
-    _, pg = _head(D, C)
-    row_class = (torch.arange(N) % C).to(torch.int32).cuda()
-    pl = cabi.Pipeline(enc, P.cuda(), Bmax, S, k, head=pg, row_class=row_class)
-    for rep, B in enumerate([3, 3, 3, 3, 8, 8, 8]):
-        ids = _ids(B, S, 1000, 100 + rep, False)[0].to(torch.int32)
-        oc_h, osc_h = pl.predict_host(ids.pin_memory())
-        oc_h, osc_h = oc_h.clone(), osc_h.clone()
-        oc, osc = pl.predict_device(ids.cuda())
-        torch.cuda.synchronize()
-        assert torch.equal(oc.cpu(), oc_h) and torch.equal(osc.cpu(), osc_h), (rep, B)
-    pl.close(); enc.close()

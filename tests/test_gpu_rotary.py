@@ -4,19 +4,14 @@
     fp32 with TF32 off: S <= 512 with cls_only on and off and the full hidden state, S up to 2048 (Nomic) / 8192 (jina)
     with both paddings and a mask hole
   * the nomic_v15 shape at B = 512 x 128 and the jina_v3 shape at 1 x 8192 and 2 x 2048
-  * from_hf against HF, the S > max_pos refusal, the reference's classifier outputs (goldens of
-    oracle/make_golden_rotary.py) with save / load through AdaptiveClassifier on local checkpoint directories, and the
-    CUDA-graph replay of the pipeline step"""
-import json
-
-import numpy as np
+  * from_hf against HF and the S > max_pos refusal
+The reference's classifier outputs (goldens of oracle/make_golden_rotary.py) and the CUDA-graph replay of the pipeline
+step are tests/test_gpu_encoder_families.py's."""
 import pytest
 import torch
 
-import golden_npz
 from oracle import rotary_oracle as ro
 from test_albert_cpu import fp16_grid
-from test_gpu_parity import _head, _synthetic_index
 from test_rotary_cpu import padded_batch, silu64, silu_bound, tiny_model
 
 pytestmark = pytest.mark.gpu
@@ -199,107 +194,3 @@ def test_jina_v3_shape_matches_oracle(cabi, B, S, pad):
     enc.close()
     ref, _ = _oracle(m, ids, mask)
     _check(out, ref, unit_tol=1.5e-3)
-
-
-# ------------------------------------------------------------------------------------------------ pipeline
-@pytest.mark.parametrize("family,S", [("nomic", 128), ("jina", 1024)])
-def test_pipeline_host_step_replayed_as_a_cuda_graph_equals_the_eager_step(cabi, family, S):
-    m = tiny_model(family, seed=3, layers=3)
-    Bmax, N, D, C, k = 8, 3000, 128, 20, 5
-    P, _ = _synthetic_index(N, D, C)
-    enc = cabi.Encoder.from_hf(m, max_tokens=Bmax * S)
-    _, pg = _head(D, C)
-    row_class = (torch.arange(N) % C).to(torch.int32).cuda()
-    pl = cabi.Pipeline(enc, P.cuda(), Bmax, S, k, head=pg, row_class=row_class)
-    for rep, B in enumerate([3, 3, 3, 3, 8, 8, 8]):
-        ids = torch.randint(5, 300, (B, S), generator=torch.Generator().manual_seed(100 + rep)).to(torch.int32)
-        oc_h, osc_h = pl.predict_host(ids.pin_memory())
-        oc_h, osc_h = oc_h.clone(), osc_h.clone()
-        oc, osc = pl.predict_device(ids.cuda())
-        torch.cuda.synchronize()
-        assert torch.equal(oc.cpu(), oc_h) and torch.equal(osc.cpu(), osc_h), (rep, B)
-    pl.close(); enc.close()
-
-
-# ------------------------------------------------------------------------------------------------ the reference's classifier
-def _golden_checkpoint(golden, d):
-    """the tiny seeded checkpoint and the tokenizer the golden run used, saved to directory d"""
-    from transformers import (BertTokenizerFast, JinaEmbeddingsV3Config, JinaEmbeddingsV3Model, NomicBertConfig,
-                              NomicBertModel, XLMRobertaTokenizer)
-    cfgd = json.loads(str(golden["bert_config"]))
-    cfgd = {k: v for k, v in cfgd.items() if k not in ("model_type", "transformers_version", "architectures")}
-    sd = {k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("bert_") and k != "bert_config"}
-    if "vocab_pieces" in golden:
-        m = JinaEmbeddingsV3Model(JinaEmbeddingsV3Config(**cfgd))
-        vocab = [(p, float(s)) for p, s in zip(golden["vocab_pieces"].tolist(), golden["vocab_scores"].tolist())]
-        tok = XLMRobertaTokenizer(vocab=vocab)
-    else:
-        m = NomicBertModel(NomicBertConfig(**cfgd))
-        tok = BertTokenizerFast(vocab={w: i for i, w in enumerate(golden["vocab"].tolist())}, do_lower_case=True)
-    m.load_state_dict(sd)
-    m.save_pretrained(d)
-    tok.save_pretrained(d)
-
-
-@pytest.fixture(scope="module", params=["golden_classifier_nomic", "golden_classifier_jina3"])
-def golden_run(cabi, request, tmp_path_factory):
-    """AdaptiveClassifier on the local checkpoint directory the reference ran on (AutoModel / AutoTokenizer)"""
-    import adaptive_classifier_b200 as acb
-    golden = golden_npz.load(request.param)
-    d = str(tmp_path_factory.mktemp(request.param))
-    _golden_checkpoint(golden, d)
-    texts, labels = golden["texts"].tolist(), golden["labels"].tolist()
-    half = 24 if "max_length" not in golden else 12
-    config = {} if "max_length" not in golden else {"max_length": int(golden["max_length"]), "b200_max_tokens": 4096}
-    np.random.seed(0)
-    clf = acb.AdaptiveClassifier(d, device="cuda", config=config)
-    clf.add_examples(texts[:half], labels[:half])
-    clf.add_examples(texts[half:], labels[half:])
-    return clf, golden
-
-
-def test_classifier_embeddings_and_prototypes_match_reference(golden_run):
-    trained, golden = golden_run
-    ids, _, _ = trained._tokenize(golden["texts"].tolist() + golden["test_texts"].tolist())
-    assert torch.equal(ids.long(), torch.from_numpy(golden["input_ids"]).long())
-    emb = torch.stack(trained._get_embeddings(golden["texts"].tolist())).numpy()
-    ref = golden["emb_train"]
-    assert emb.shape == ref.shape
-    assert np.abs(emb - ref).max() < 3e-4 and np.linalg.norm(emb - ref, axis=1).max() < 1e-3
-    emb_t = torch.stack(trained._get_embeddings(golden["test_texts"].tolist())).numpy()
-    assert np.abs(emb_t - golden["emb_test"]).max() < 3e-4
-    names = golden["label_names"].tolist()
-    assert [trained.id_to_label[i] for i in range(len(names))] == names
-    protos = np.stack([trained.memory.prototypes[l].numpy() for l in sorted(trained.memory.prototypes)])
-    assert golden["proto_labels"].tolist() == sorted(trained.memory.prototypes)
-    assert np.abs(protos - golden["prototypes"]).max() < 3e-4
-
-
-def _cmp(preds, L, S, names):
-    for p, l_row, s_row in zip(preds, L, S):
-        exp = [(names[i], s) for i, s in zip(l_row.tolist(), s_row.tolist()) if i >= 0]
-        assert [l for l, _ in p] == [l for l, _ in exp], (p, exp)
-        assert np.allclose([s for _, s in p], [s for _, s in exp], atol=1e-3), (p, exp)
-
-
-def test_classifier_predictions_match_reference_and_survive_save_load(golden_run, tmp_path):
-    import adaptive_classifier_b200 as acb
-    trained, golden = golden_run
-    names = golden["label_names"].tolist()
-    own_head = {k: v.detach().clone() for k, v in trained.adaptive_head.state_dict().items()}
-    trained.adaptive_head.load_state_dict({k[5:]: torch.from_numpy(golden[k]) for k in golden.files if k.startswith("head_")})
-    tests_ = golden["test_texts"].tolist()
-    try:
-        _cmp([trained.predict(t, k=3) for t in tests_], golden["pred_labels"], golden["pred_scores"], names)
-        _cmp([trained.predict(t, k=1) for t in tests_], golden["pred_k1_labels"], golden["pred_k1_scores"], names)
-        _cmp(trained.predict_batch(tests_, k=2), golden["predb_labels"], golden["predb_scores"], names)
-        before = [trained.predict(t, k=3) for t in tests_]
-        out = str(tmp_path / "saved")
-        trained.save(out)
-        clf2 = acb.AdaptiveClassifier.load(out, device="cuda")
-        assert clf2.label_to_id == trained.label_to_id
-        after = [clf2.predict(t, k=3) for t in tests_]
-        for p, p2 in zip(before, after):
-            assert [l for l, _ in p2] == [l for l, _ in p] and np.allclose([s for _, s in p2], [s for _, s in p], atol=1e-5)
-    finally:
-        trained.adaptive_head.load_state_dict(own_head)

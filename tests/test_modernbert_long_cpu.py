@@ -109,11 +109,10 @@ def test_max_position_embeddings_over_8192_is_refused_by_name():
 def test_query_block_oracle_reproduces_reference_long_embeddings():
     """the oracle on the golden checkpoint gives the unmodified reference's _get_embeddings output with max_length 1024"""
     from transformers import ModernBertConfig
-    gold = golden_npz.load("golden_classifier_modernbert_long")
-    weights = golden_npz.load("golden_classifier_modernbert")
+    gold = golden_npz.load("golden_classifier_modernbert_long", weights_from="golden_classifier_modernbert")
     cfg = ModernBertConfig(**json.loads(str(gold["bert_config"])))
     assert cfg.max_position_embeddings == 8192 and int(gold["max_length"]) == 1024
-    sd = {k[5:]: torch.from_numpy(weights[k]) for k in weights.files if k.startswith("bert_") and k != "bert_config"}
+    sd = {k[5:]: torch.from_numpy(gold[k]) for k in gold.files if k.startswith("bert_") and k != "bert_config"}
     ids = torch.from_numpy(gold["input_ids"]).long()
     mask = torch.from_numpy(gold["attention_mask"]).long()
     lens = mask.sum(1)
