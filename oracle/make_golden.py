@@ -12,7 +12,8 @@ Fixtures
                          inter-prototype d = 0.001965: near-tie stress) + reference search results
   golden_head.npz        AdaptiveHead forward / EWC loss values of the reference on seeded inputs
   golden_classifier.npz  tiny seeded BERT checkpoint + vocab, reference _get_embeddings / add_examples /
-                         predict / predict_batch outputs and the reference-trained head
+                         predict / predict_batch outputs and the reference-trained head: the bert row of
+                         make_golden_encoders.py, which makes the other encoder families' runs too
   golden_training.npz    the reference's two training loops (_train_adaptive_head, _train_new_classes + EWC/Fisher)
                          run UNMODIFIED with recorders hooked onto torch/numpy entry points: the dataset of every
                          training call, every batch index list the DataLoader yielded, np.random.choice draws,
@@ -24,6 +25,7 @@ import json
 import os
 import sys
 import tempfile
+from typing import Any, NamedTuple
 
 import numpy as np
 import torch
@@ -36,15 +38,59 @@ sys.path.insert(0, ROOT)
 OUT = os.path.join(ROOT, "tests", "golden")
 
 
-def save_split(name, arrays):
-    """golden_<name>.npz + the checkpoint weights (bert_*) in _bert0 / _bert1 (layer 1): every file stays under 1 MB;
-    tests/golden_npz.py loads them back as one mapping"""
-    parts = {"": {}, "_bert0": {}, "_bert1": {}}
-    for k, v in arrays.items():
-        suffix = "" if not k.startswith("bert_") or k == "bert_config" else ("_bert1" if ".layer.1." in k else "_bert0")
-        parts[suffix][k] = v
-    for suffix, p in parts.items():
-        np.savez_compressed(os.path.join(OUT, f"{name}{suffix}.npz"), **p)
+def save(out, name, arrays, parts):
+    """<name>.npz holds the recorded outputs, <name>_bert0.npz, _bert1.npz, ... the checkpoint's tensors (bert_*, but not
+    bert_config) as parts(weights, outputs) -> [outputs file, part 0, part 1, ...] assigns them; every file stays under
+    1 MB and tests/golden_npz.py loads them back as one mapping"""
+    outputs = {k: v for k, v in arrays.items() if not k.startswith("bert_") or k == "bert_config"}
+    weights = {k: v for k, v in arrays.items() if k not in outputs}
+    files = parts(weights, outputs) if weights else [outputs]
+    for i, f in enumerate(files):
+        path = os.path.join(out, f"{name}_bert{i - 1}.npz" if i else f"{name}.npz")
+        np.savez_compressed(path, **f)
+        print(os.path.basename(path), os.path.getsize(path))
+        assert os.path.getsize(path) < 1_000_000, path
+
+
+def by_prefix(*prefixes):
+    """parts for save: part 1 holds the tensors whose names start with one of prefixes, part 0 the rest"""
+    def split(weights, outputs):
+        return [outputs, {k: v for k, v in weights.items() if not k.startswith(prefixes)},
+                {k: v for k, v in weights.items() if k.startswith(prefixes)}]
+    return split
+
+
+def greedy(n_parts, with_outputs=False):
+    """parts for save: largest tensor first, each into the part with the fewest bytes so far, over n_parts parts and,
+    with_outputs, the outputs file"""
+    def split(weights, outputs):
+        files = [dict(outputs)] + [{} for _ in range(n_parts)]
+        bins = files if with_outputs else files[1:]
+        size = [sum(np.asarray(v).nbytes for v in b.values()) for b in bins]
+        for k in sorted(weights, key=lambda k: -np.asarray(weights[k]).nbytes):
+            i = size.index(min(size))
+            bins[i][k] = weights[k]
+            size[i] += np.asarray(weights[k]).nbytes
+        return files
+    return split
+
+
+def perturb_param(n, p, g):
+    """norms and biases move by 0.1 randn, 2-D weights grow x3 and the word embeddings x4: at the init std 0.02 every CLS
+    row is nearly identical; now token identity survives to the CLS row, so the classes are learnable (on the bert
+    checkpoint, nearest-centroid accuracy 0.93 on the short recipe's sentences) and the training loops do not early-stop
+    at once"""
+    if "norm" in n.lower() or n.endswith(".bias"):
+        p.add_(0.1 * torch.randn(p.shape, generator=g))
+    elif "weight" in n and p.dim() == 2:
+        p.mul_(4.0 if n.endswith(("word_embeddings.weight", "embed_tokens.weight")) else 3.0)
+
+
+def perturb(model, seed):
+    g = torch.Generator().manual_seed(seed)
+    with torch.no_grad():
+        for n, p in model.named_parameters():
+            perturb_param(n, p, g)
 
 
 def unit(x):
@@ -127,70 +173,24 @@ def gen_head():
     print("golden_head ok", loss0, loss1, loss1_b32)
 
 
-def gen_classifier():
-    from adaptive_classifier import AdaptiveClassifier
-    tmp, words, vocab, model, cfg = _tiny_checkpoint()
+class Checkpoint(NamedTuple):
+    dir: str            # what the reference loads
+    words: list
+    vocab: list         # token strings, or the (piece, score) pairs of a unigram tokenizer
+    model: Any
+    config: Any
 
-    rng = np.random.default_rng(7)
-    class_words = {"sports": words[0:40], "finance": words[40:80], "cooking": words[80:120]}
 
-    def sentence(label, n):
-        own = rng.choice(class_words[label], size=n, replace=True)
-        noise = rng.choice(words[120:], size=max(1, n // 4), replace=True)
-        toks = list(own) + list(noise)
-        rng.shuffle(toks)
-        return " ".join(toks)
-
-    texts, labels = [], []
-    for label in ["sports", "finance", "cooking"]:
-        for _ in range(12):
-            texts.append(sentence(label, int(rng.integers(4, 14))))
-            labels.append(label)
-    test_texts = [sentence(l, 9) for l in ["sports", "finance", "cooking", "finance", "sports", "cooking"]]
-
-    torch.manual_seed(0)
-    np.random.seed(0)
-    clf = AdaptiveClassifier(tmp, device="cpu", use_onnx=False)
-    clf.add_examples(texts[:24], labels[:24])           # sports + finance -> _train_adaptive_head
-    clf.add_examples(texts[24:], labels[24:])           # new class cooking -> _train_new_classes (+EWC)
-    emb_train = torch.stack(clf._get_embeddings(texts)).numpy()
-    emb_test = torch.stack(clf._get_embeddings(test_texts)).numpy()
-    enc = clf.tokenizer(texts + test_texts, max_length=512, truncation=True, padding=True, return_tensors="pt")
-    label_names = [clf.id_to_label[i] for i in range(len(clf.id_to_label))]
-    pred = [clf.predict(t, k=3) for t in test_texts]
-    pred_k1 = [clf.predict(t, k=1) for t in test_texts]
-    pred_b = clf.predict_batch(test_texts, k=2)
-    train_top1 = [p[0][0] for p in clf.predict_batch(texts, k=1)]     # end metric of the reference's own training
-
-    def pack(preds, k):
-        L = np.full((len(preds), k), -1, dtype=np.int64)
-        S = np.zeros((len(preds), k), dtype=np.float64)
-        for i, p in enumerate(preds):
-            for j, (l, s) in enumerate(p):
-                L[i, j] = label_names.index(l)
-                S[i, j] = s
-        return L, S
-
-    pl, ps = pack(pred, 3)
-    p1l, p1s = pack(pred_k1, 1)
-    pbl, pbs = pack(pred_b, 2)
-    head_sd = {("head_" + k): v.detach().numpy() for k, v in clf.adaptive_head.state_dict().items()}
-    model_sd = {("bert_" + k): v.detach().numpy() for k, v in model.state_dict().items()}
-    protos = np.stack([clf.memory.prototypes[l].numpy() for l in sorted(clf.memory.prototypes)])
-    save_split(
-        "golden_classifier", dict(
-        vocab=np.array(vocab), texts=np.array(texts), labels=np.array(labels), test_texts=np.array(test_texts),
-        label_names=np.array(label_names), input_ids=enc["input_ids"].numpy(), attention_mask=enc["attention_mask"].numpy(),
-        emb_train=emb_train, emb_test=emb_test, prototypes=protos, proto_labels=np.array(sorted(clf.memory.prototypes)),
-        training_history=json.dumps(clf.training_history), train_steps=clf.train_steps,
-        pred_labels=pl, pred_scores=ps, pred_k1_labels=p1l, pred_k1_scores=p1s, predb_labels=pbl, predb_scores=pbs,
-        train_top1=np.array([label_names.index(l) for l in train_top1]),
-        bert_config=json.dumps(cfg.to_dict()), **head_sd, **model_sd))
-    print("golden_classifier ok; labels", label_names, "pred[0]", pred[0])
+def saved(model, tokenizer, words, vocab):
+    """model and tokenizer saved to a fresh directory"""
+    tmp = tempfile.mkdtemp(prefix="golden_ckpt_")
+    model.save_pretrained(tmp)
+    tokenizer.save_pretrained(tmp)
+    return Checkpoint(tmp, words, vocab, model, model.config)
 
 
 def _tiny_checkpoint(hidden=128):
-    """seeded 2-layer BERT + synthetic vocab on disk (same recipe as gen_classifier)"""
+    """seeded 2-layer BERT + synthetic vocab on disk (the bert row of make_golden_encoders.py)"""
     from transformers import BertConfig, BertModel, BertTokenizerFast
     words = [f"w{i}" for i in range(195)]
     vocab = ["[PAD]", "[UNK]", "[CLS]", "[SEP]", "[MASK]"] + words
@@ -198,26 +198,16 @@ def _tiny_checkpoint(hidden=128):
                      intermediate_size=2 * hidden, max_position_embeddings=64, type_vocab_size=2, pad_token_id=0)
     torch.manual_seed(1234)
     model = BertModel(cfg)
-    g = torch.Generator().manual_seed(99)
+    perturb(model, 99)
     with torch.no_grad():
-        for n, p in model.named_parameters():
-            if "LayerNorm" in n or n.endswith(".bias"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif "weight" in n and p.dim() == 2:
-                # word embeddings x4: token identity survives to the CLS row, so the classes are learnable (nearest-centroid
-                # accuracy 0.93 on the sentences below) and the loops do not early-stop at once
-                p.mul_(4.0 if "word_embeddings" in n else 3.0)
-        # ... and the constant part of the CLS row's input ([CLS] word row, position 0, token types) is zeroed, otherwise every
+        # the constant part of the CLS row's input ([CLS] word row, position 0, token types) is zeroed, otherwise every
         # sentence embeds within 0.2 of every other one and 10 epochs of lr 1e-3 learn nothing (mean pair distance 1.14 now)
         model.embeddings.word_embeddings.weight[2].zero_()
         model.embeddings.position_embeddings.weight[0].zero_()
         model.embeddings.token_type_embeddings.weight.zero_()
-    tmp = tempfile.mkdtemp(prefix="golden_ckpt_")
-    model.save_pretrained(tmp)
     # transformers 5.x: BertTokenizerFast(vocab_file=...) silently keeps only the special tokens (every word -> [UNK]);
     # the vocabulary has to be passed as a dict
-    BertTokenizerFast(vocab={w: i for i, w in enumerate(vocab)}, do_lower_case=True).save_pretrained(tmp)
-    return tmp, words, vocab, model, cfg
+    return saved(model, BertTokenizerFast(vocab={w: i for i, w in enumerate(vocab)}, do_lower_case=True), words, vocab)
 
 
 class _Recorder:
@@ -471,10 +461,15 @@ def gen_training():
     out["vocab"] = np.array(vocab)
     for k, v in clf.model.state_dict().items():
         out["bert_" + k] = v.detach().numpy()
-    save_split("golden_training", out)
+    save(OUT, "golden_training", out, by_prefix("bert_encoder.layer.1."))
     print("golden_training ok: h3 steps", len(out["h3_loss"]), "epochs", len(out["h3_steps_per_epoch"]),
           "| h4 steps", len(out["h4_loss"]), "epochs", len(out["h4_steps_per_epoch"]), "rows", out["h4_X"].shape,
           "| fisher batches", len(out["h4_fisher_batch_sizes"]), "| ml steps", len(out["ml_loss"]), "preds", preds[:2])
+
+
+def gen_classifier():
+    import make_golden_encoders
+    make_golden_encoders.generate(["bert"], OUT)
 
 
 if __name__ == "__main__":

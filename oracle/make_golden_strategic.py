@@ -3,9 +3,9 @@ oracle/make_golden.py).
 
     python oracle/make_golden_strategic.py     # writes tests/golden/golden_strategic_{linear,separable,readme}.npz
 
-Runs the UNMODIFIED reference classifier (make_golden's tiny seeded BERT checkpoint, the same texts and seeds as
-gen_classifier) with nn.Dropout patched to identity -- as gen_training does: CPU dropout masks cannot be reproduced on a GPU --
-for list coefficients of both cost types with strategic_training_frequency = 1, and records:
+Runs the UNMODIFIED reference classifier (make_golden's tiny seeded BERT checkpoint, the same texts and seeds as the
+bert row of make_golden_encoders.py) with nn.Dropout patched to identity -- as gen_training does: CPU dropout masks
+cannot be reproduced on a GPU -- for list coefficients of both cost types with strategic_training_frequency = 1, and records:
   * every strategic training call: its inputs, the head state before and after, the per-step strategic losses
     (StrategicOptimizer.strategic_loss wrapped) and pre-clip grad norms, and the train_steps at which it ran;
   * every compute_best_response call: x, the chosen candidate index and the margin between the best and second-best fp32
@@ -30,7 +30,7 @@ MIN_MARGIN = 1e-4          # fp32 utilities of a 128 -> 128 -> 64 -> C head carr
 
 
 def texts_and_labels(words):
-    """make_golden.gen_classifier's sentences (same generator, same draws)"""
+    """the sentences of make_golden_encoders.short at seed 7 (same generator, same draws)"""
     rng = np.random.default_rng(7)
     class_words = {"sports": words[0:40], "finance": words[40:80], "cooking": words[80:120]}
 

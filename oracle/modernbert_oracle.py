@@ -11,7 +11,7 @@ Restated from the published algorithm (ModernBertEmbeddings, pre-LN ModernBertEn
 attn_norm, ModernBertRotaryEmbedding, eager attention with the bidirectional sliding-window mask, GeGLU ModernBertMLP,
 final_norm) and PINNED against the installed HF module by tests/test_modernbert_cpu.py (1e-5 on CLS rows and hidden states,
 padded batches, sliding band edge, both RoPE theta) and against the reference's own _get_embeddings on
-tests/golden/golden_classifier_modernbert*.npz (oracle/make_golden_modernbert.py).
+tests/golden/golden_classifier_modernbert*.npz (oracle/make_golden_encoders.py modernbert).
 """
 from __future__ import annotations
 

@@ -3,7 +3,7 @@
     = heads, heads / 2 and 1, and a non-default RoPE theta
   * the RoPE table the encoder reads against EuroBertRotaryEmbedding, bit for bit, at 8192 rows
   * the mapping consumes every parameter, and its GQA expansion is HF repeat_kv bit for bit
-  * the golden classifier runs of oracle/make_golden_eurobert.py against the oracle
+  * the golden classifier runs of oracle/make_golden_encoders.py eurobert eurobert_long against the oracle
   * each wrong rule (LayerNorm for RMSNorm, centred RMSNorm, layer-0 norm as identity, final norm skipped, RoPE dropped,
     padding-aware positions, tiled kv heads, gate / up swapped) moves the embeddings far past the GPU bound
   * eurobert_settings, remote-code and ac_encoder_create refusals, which run before any device call"""

@@ -1,5 +1,6 @@
 """GPU tests every encoder family shares, driven by FAMILIES: one row per golden classifier run of the reference
-(tests/golden/golden_classifier_<name>.npz, made by oracle/make_golden_*.py from the unmodified reference).
+(tests/golden/golden_classifier_<name>.npz, made by the same row of oracle/make_golden_encoders.py from the unmodified
+reference).
 
   * the drop-in classifier on the tiny seeded checkpoint and tokenizer the reference ran on: tokenized ids, embeddings,
     label ids, training history, prototypes; then predict (k = 3, k = 1) and predict_batch (k = 2) with the

@@ -10,8 +10,8 @@ TINY_BOUND (tiny models) and SHAPE_BOUND (eurobert_210m, the goldens) instead of
   * the eurobert_210m shape at B = 512 x 128 (sampled rows), 1 x 8192 and 2 x 2048
   * from_hf against HF, the S > max_pos refusal, and AdaptiveClassifier with max_length 8192 on the golden runs' local
     checkpoint directory
-The reference's classifier outputs (goldens of oracle/make_golden_eurobert.py) and the CUDA-graph replay of the pipeline
-step are tests/test_gpu_encoder_families.py's."""
+The reference's classifier outputs (goldens of oracle/make_golden_encoders.py eurobert eurobert_long) and the CUDA-graph
+replay of the pipeline step are tests/test_gpu_encoder_families.py's."""
 import numpy as np
 import pytest
 import torch

@@ -5,8 +5,8 @@
     with both paddings and a mask hole
   * the nomic_v15 shape at B = 512 x 128 and the jina_v3 shape at 1 x 8192 and 2 x 2048
   * from_hf against HF and the S > max_pos refusal
-The reference's classifier outputs (goldens of oracle/make_golden_rotary.py) and the CUDA-graph replay of the pipeline
-step are tests/test_gpu_encoder_families.py's."""
+The reference's classifier outputs (goldens of oracle/make_golden_encoders.py nomic jina3) and the CUDA-graph replay of
+the pipeline step are tests/test_gpu_encoder_families.py's."""
 import pytest
 import torch
 

@@ -3,7 +3,7 @@
     and without token_type_ids, S from 16 to 2048
   * the RoPE table the encoder reads against HF's rotary_emb, bit for bit
   * the mappings consume every parameter but the pooler, and supply zero biases where the checkpoint has none
-  * the golden classifier runs of oracle/make_golden_rotary.py against the oracle
+  * the golden classifier runs of oracle/make_golden_encoders.py nomic jina3 against the oracle
   * each wrong rule (no RoPE, GPT-J pairs, padding-aware positions, RoPE on v, gate / up swapped) moves the embeddings far
     past the GPU bound
   * from_hf and ac_encoder_create refusals, which run before any device call"""

@@ -1,6 +1,6 @@
 """CPU tests of the long XLM-RoBERTa path's references: oracle/encoder_oracle.py (arch "roberta") against HF XLMRobertaModel
 (eager attention) with an 8194-row position table at S past 512, where RoBERTa positions run past 514; and the golden
-classifier run of oracle/make_golden_xlmr_long.py (the reference with max_length 1024) against that oracle."""
+classifier run of oracle/make_golden_encoders.py xlmr_long (the reference with max_length 1024) against that oracle."""
 import json
 
 import numpy as np
