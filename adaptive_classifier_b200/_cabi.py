@@ -52,7 +52,7 @@ EXPORTS = [
     "ac_pipeline_encode", "ac_pipeline_embeddings", "ac_pipeline_search_shard", "ac_pipeline_finish_sharded",
     "ac_pipeline_debug_copy", "ac_pipeline_knn_stats", "ac_launch_count", "ac_profile_enable", "ac_profile_read",
     "ac_tokenizer_create", "ac_tokenizer_destroy", "ac_tokenize_workspace_bytes", "ac_tokenize", "ac_tokenize_pack",
-    "ac_tokenizer_create_bpe", "ac_tokenize_workspace_bytes_text",
+    "ac_tokenizer_create_bpe", "ac_tokenize_workspace_bytes_text", "ac_tokenizer_create_unigram",
 ]
 
 
@@ -106,6 +106,15 @@ class BPETokenizerSpec(Structure):
     _fields_ = [("cls", c_void_p), ("split", c_int), ("add_prefix_space", c_int), ("ignore_merges", c_int),
                 ("vocab_bytes", c_void_p), ("vocab_offsets", c_void_p), ("vocab_ids", c_void_p), ("n_vocab", c_int),
                 ("byte_ids", c_void_p), ("merges", c_void_p), ("n_merges", c_int),
+                ("added_bytes", c_void_p), ("added_offsets", c_void_p), ("added_ids", c_void_p), ("added_flags", c_void_p),
+                ("n_added", c_int), ("cls_id", c_int), ("sep_id", c_int), ("pad_id", c_int)]
+
+
+class UnigramTokenizerSpec(Structure):
+    _fields_ = [("cls", c_void_p), ("map_keys", c_void_p), ("map_key_offsets", c_void_p), ("map_values", c_void_p),
+                ("map_value_offsets", c_void_p), ("n_map", c_int), ("grow", c_int),
+                ("piece_bytes", c_void_p), ("piece_offsets", c_void_p), ("piece_scores", c_void_p), ("n_pieces", c_int),
+                ("unk_id", c_int),
                 ("added_bytes", c_void_p), ("added_offsets", c_void_p), ("added_ids", c_void_p), ("added_flags", c_void_p),
                 ("n_added", c_int), ("cls_id", c_int), ("sep_id", c_int), ("pad_id", c_int)]
 
@@ -199,6 +208,7 @@ def load_library() -> ctypes.CDLL:
     L.ac_tokenize_pack.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     L.ac_tokenizer_create_bpe.argtypes = [POINTER(BPETokenizerSpec), POINTER(c_void_p)]
     L.ac_tokenize_workspace_bytes_text.argtypes = [c_void_p, c_int, c_int64, c_int, POINTER(c_size_t)]
+    L.ac_tokenizer_create_unigram.argtypes = [POINTER(UnigramTokenizerSpec), POINTER(c_void_p)]
     L.ac_pipeline_knn_stats.argtypes = [c_void_p, c_void_p, c_int, c_void_p]
     L.ac_profile_read.argtypes = [c_int, POINTER(ctypes.c_double), POINTER(ctypes.c_double), POINTER(ctypes.c_double),
                                   POINTER(ctypes.c_longlong)]
@@ -1349,10 +1359,35 @@ def bpe_spec_struct(spec: dict):
     return st, keep
 
 
+def unigram_spec_struct(spec: dict):
+    """(UnigramTokenizerSpec, arrays it points into) from tokenizer.unigram_spec's dict and the codepoint classes"""
+    import numpy as np
+    from .tokenizer import pack_strings, unigram_classes
+    cls = unigram_classes()
+    def packed(blobs):
+        off = np.zeros(len(blobs) + 1, dtype=np.int64)
+        np.cumsum([len(x) for x in blobs], out=off[1:])
+        return np.frombuffer(b"".join(blobs) or b"\0", dtype=np.uint8), off
+    mk, mko = packed([k for k, _ in spec["charsmap"]])
+    mv, mvo = packed([v for _, v in spec["charsmap"]])
+    pb, po = packed([p for p, _ in spec["pieces"]])
+    ps = np.asarray([sc for _, sc in spec["pieces"]], dtype=np.float64)
+    added = spec["added"]
+    ab, ao = pack_strings([a[0] for a in added])
+    ai = np.asarray([a[1] for a in added] or [0], dtype=np.int32)
+    af = np.asarray([a[2] | a[3] << 1 | a[4] << 2 for a in added] or [0], dtype=np.uint8)
+    keep = [cls, mk, mko, mv, mvo, pb, po, ps, ab, ao, ai, af]
+    p = [a.ctypes.data for a in keep]
+    st = UnigramTokenizerSpec(p[0], p[1], p[2], p[3], p[4], len(spec["charsmap"]), spec["grow"], p[5], p[6], p[7],
+                              len(spec["pieces"]), spec["unk_id"], p[8], p[9], p[10], p[11], len(added),
+                              spec["cls_id"], spec["sep_id"], spec["pad_id"])
+    return st, keep
+
+
 class _DeviceTokenizer:
-    """What both device tokenizers share: the handle, one pinned H2D copy of the texts' offsets and bytes, the one readback of
-    the batch's longest row, and the pack into [B, S] tensors."""
-    _readback = 1                                   # int32 the call reads back: the longest row (BPE: and the texts left)
+    """What every device tokenizer (WordPiece, BPE, Unigram) shares: the handle, one pinned H2D copy of the texts' offsets and
+    bytes, the one readback of the batch's longest row, and the pack into [B, S] tensors."""
+    _readback = 1                                   # int32 the call reads back: the longest row (BPE, Unigram: and the texts left)
 
     def _create(self, create, st, type_ids: bool, device):
         self._L = load_library()
@@ -1370,7 +1405,7 @@ class _DeviceTokenizer:
         raise NotImplementedError
 
     def _left_rows(self, texts, max_length, tokens, lengths) -> int:
-        """rows of the texts the kernels left to the host (BPE); returns their longest length"""
+        """rows of the texts the kernels left to the host (BPE, Unigram); returns their longest length"""
         return 0
 
     def __call__(self, texts, max_length: int):
@@ -1448,23 +1483,21 @@ class WordPieceTokenizer(_DeviceTokenizer):
         return nb.value
 
 
-class BPETokenizer(_DeviceTokenizer):
-    """Owner of an ac_tokenizer handle of a byte-level BPE tokenizer (RoBERTa, ModernBERT, EuroBERT; tokenizer.bpe_spec):
-    `tokenizer(texts, max_length=..., truncation=True, padding=True)` computed on the device with identical ids.  A text with
-    a kept word longer than AC_BPE_MAX_WORD bytes is tokenized by `tokenizer` itself, on the host."""
+class _HandBackTokenizer(_DeviceTokenizer):
+    """A device tokenizer whose kernels leave some texts (lengths = -1, max_len[1] = 1) to the host tokenizer: the handle's
+    workspace depends on the text bytes, and the rows of the texts left are written before the pack."""
     _readback = 2
 
     def __init__(self, spec: dict, tokenizer, device="cuda"):
-        st, keep = bpe_spec_struct(spec)
-        self._create(load_library().ac_tokenizer_create_bpe, st, spec["type_ids"], device)
+        st, keep = self._spec_struct(spec)
+        self._create(self._create_fn(load_library()), st, spec["type_ids"], device)
         del keep
         self._hf = tokenizer
 
     @classmethod
     def from_hf(cls, tokenizer, device="cuda"):
-        """(BPETokenizer, "") for a supported tokenizer, else (None, the reason)"""
-        from .tokenizer import bpe_spec
-        spec, why = bpe_spec(tokenizer)
+        """(tokenizer, "") for a supported tokenizer, else (None, the reason)"""
+        spec, why = cls._spec(tokenizer)
         if spec is None:
             return None, why
         return cls(spec, tokenizer, device), ""
@@ -1485,6 +1518,39 @@ class BPETokenizer(_DeviceTokenizer):
         tokens[idx] = host.to(self.device)
         lengths[idx] = torch.tensor([len(r) for r in rows], dtype=torch.int32).to(self.device)
         return max(len(r) for r in rows)
+
+
+class BPETokenizer(_HandBackTokenizer):
+    """Owner of an ac_tokenizer handle of a byte-level BPE tokenizer (RoBERTa, ModernBERT, EuroBERT; tokenizer.bpe_spec):
+    `tokenizer(texts, max_length=..., truncation=True, padding=True)` computed on the device with identical ids.  A text with
+    a kept word longer than AC_BPE_MAX_WORD bytes is tokenized by `tokenizer` itself, on the host."""
+    _spec_struct = staticmethod(bpe_spec_struct)
+
+    @staticmethod
+    def _create_fn(L):
+        return L.ac_tokenizer_create_bpe
+
+    @staticmethod
+    def _spec(tokenizer):
+        from .tokenizer import bpe_spec
+        return bpe_spec(tokenizer)
+
+
+class UnigramTokenizer(_HandBackTokenizer):
+    """Owner of an ac_tokenizer handle of a SentencePiece Unigram tokenizer of the XLM-RoBERTa shape (xlm-roberta-*, bge-m3,
+    multilingual-e5-*, jina-embeddings-v3; tokenizer.unigram_spec): `tokenizer(texts, max_length=..., truncation=True,
+    padding=True)` computed on the device with identical ids.  A text with a kept word longer than AC_UNIGRAM_MAX_WORD bytes
+    is tokenized by `tokenizer` itself, on the host."""
+    _spec_struct = staticmethod(unigram_spec_struct)
+
+    @staticmethod
+    def _create_fn(L):
+        return L.ac_tokenizer_create_unigram
+
+    @staticmethod
+    def _spec(tokenizer):
+        from .tokenizer import unigram_spec
+        return unigram_spec(tokenizer)
 
 
 def proto_class_scores(d, idx, row_class=None, n_classes: Optional[int] = None):

@@ -73,11 +73,12 @@ class AdaptiveClassifier:
         self._max_tokens = int(self.config.config.get("b200_max_tokens", 65536))
         with torch.cuda.device(torch.device(self.device)):
             self.encoder = _cabi.Encoder.from_hf(hf, max_tokens=self._max_tokens, device=self.device)
-            # WordPiece tokenizers of the BERT shape and byte-level BPE tokenizers (RoBERTa, ModernBERT, EuroBERT) run on the
-            # device with identical ids; every other one stays on the host, and so does one whose tables or handle cannot be built
+            # WordPiece tokenizers of the BERT shape, byte-level BPE tokenizers (RoBERTa, ModernBERT, EuroBERT) and Unigram
+            # tokenizers of the XLM-RoBERTa shape run on the device with identical ids; every other one stays on the host, and so
+            # does one whose tables or handle cannot be built
             whys = []
             self.device_tokenizer = None
-            for kind in (_cabi.WordPieceTokenizer, _cabi.BPETokenizer):
+            for kind in (_cabi.WordPieceTokenizer, _cabi.BPETokenizer, _cabi.UnigramTokenizer):
                 try:
                     self.device_tokenizer, why = kind.from_hf(self.tokenizer, device=self.device)
                 except (_cabi.AdaptiveB200Error, ValueError) as e:

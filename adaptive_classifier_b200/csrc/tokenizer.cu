@@ -8,7 +8,8 @@
 // table of the vocab.  The walk stops once max_length - 2 tokens exist: later words cannot change the kept ids.
 //
 // Byte-level BPE tokenizers (RoBERTa, ModernBERT, EuroBERT) run on three kernels further down, sharing the UTF-8 decoding,
-// the handle, the uploads and tokenize_pack_kernel with WordPiece.
+// the handle, the uploads and tokenize_pack_kernel with WordPiece; SentencePiece Unigram tokenizers of the XLM-RoBERTa shape
+// run on two kernels of their own and BPE's added-token trie and gather kernel.
 //
 // The file is plain SIMT C++: with AC_CPU_SHIM defined (tests/cpu_shim) only the kernels and the host-side table builder are
 // compiled, so the control flow runs on the CPU as well.
@@ -488,6 +489,21 @@ __device__ inline bool rust_space_at(const BpeTables &t, const uint8_t *p, int64
     return (t.cls[c] & kRust) != 0;
 }
 
+// the child of `node` over `byte` in a byte trie whose edges (node << 8 | byte, child) sit in an open-addressing table, or -1
+__host__ __device__ inline uint32_t trie_edge_hash(int key) {
+    const uint32_t h = static_cast<uint32_t>(key) * 0x9E3779B1u;
+    return h ^ (h >> 16);
+}
+
+__device__ inline int trie_child(const int2 *edges, uint32_t mask, int node, uint8_t byte) {
+    const int key = (node << 8) | byte;
+    for (uint32_t k = trie_edge_hash(key) & mask;; k = (k + 1) & mask) {
+        const int2 x = edges[k];
+        if (x.x < 0) return -1;
+        if (x.x == key) return x.y;
+    }
+}
+
 // the next added token of `pass` in [from, end) (aho-corasick leftmost-longest), widened by lstrip down to `from` and by
 // rstrip up to `end` over Rust whitespace: returns its terminal code and [*s, *e), or -1 with *s = end
 __device__ inline int next_added(const BpeTables &t, int pass, const uint8_t *p, int64_t from, int64_t end, int64_t *s,
@@ -499,16 +515,8 @@ __device__ inline int next_added(const BpeTables &t, int pass, const uint8_t *p,
         int node = 0, code = -1;
         int64_t stop = i;
         for (int64_t j = i; j < end; ++j) {
-            const int key = (node << 8) | p[j];
-            uint32_t h = static_cast<uint32_t>(key) * 0x9E3779B1u;
-            int child = -1;
-            for (uint32_t k = (h ^ (h >> 16)) & t.edge_mask;; k = (k + 1) & t.edge_mask) {
-                const int2 x = t.edges[k];
-                if (x.x < 0) break;
-                if (x.x == key) { child = x.y; break; }
-            }
-            if (child < 0) break;
-            node = child;
+            node = trie_child(t.edges, t.edge_mask, node, p[j]);
+            if (node < 0) break;
             const int2 tm = t.term[node];
             const int c = pass ? tm.y : tm.x;
             if (c >= 0) { code = c; stop = j + 1; }
@@ -680,18 +688,19 @@ __global__ void __launch_bounds__(128) tokenize_bpe_merge_kernel(BpeTables t, co
     ent.y = -c;
 }
 
-// tokens[b] = [CLS] the entries' tokens [SEP], truncated to max_length; one warp per text
+// tokens[b] = [CLS] the entries' tokens [SEP], truncated to max_length; one warp per text.  Text b's slots start at
+// (offsets[b] - offsets[0] + b) * slots_per_byte: one per byte and one more (BPE), or more (Unigram)
 __global__ void __launch_bounds__(128) tokenize_bpe_gather_kernel(BpeTables t, const int64_t *offsets, int B, int max_length,
                                                                   const int2 *ws_ent, const int32_t *n_ent,
                                                                   const int32_t *ws_tok, int32_t *tokens, int32_t *lengths,
-                                                                  int32_t *max_len) {
+                                                                  int32_t *max_len, int slots_per_byte = 1) {
     const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (b >= B) return;
     const int ne = n_ent[b];
     if (ne < 0) return;
     const int limit = max_length - 2;
     const int2 *ent = ws_ent + static_cast<int64_t>(b) * limit;
-    const int32_t *slots = ws_tok + offsets[b] - offsets[0] + b;
+    const int32_t *slots = ws_tok + (offsets[b] - offsets[0] + b) * slots_per_byte;
     int32_t *row = tokens + static_cast<int64_t>(b) * max_length;
     int done = 0;
     for (int k0 = 0; k0 < ne && done < limit; k0 += 32) {
@@ -729,6 +738,67 @@ inline uint32_t pow2_at_least(size_t n) {
     return static_cast<uint32_t>(s);
 }
 
+// a byte trie built on the host, nodes numbered from the root 0, laid out for trie_child
+struct TrieBuilder {
+    std::vector<std::vector<std::pair<int, int>>> kids{1};
+    size_t n_edges = 0;
+    int size() const { return static_cast<int>(kids.size()); }
+    // the node of key s[0, n), created with its path; -1 once the trie outgrows the 2^23 nodes an edge key can name
+    int insert(const uint8_t *s, int64_t n) {
+        int node = 0;
+        for (int64_t j = 0; j < n; ++j) {
+            int child = -1;
+            for (auto &e : kids[node])
+                if (e.first == s[j]) child = e.second;
+            if (child < 0) {
+                child = static_cast<int>(kids.size());
+                if (child >= (1 << 23)) return -1;
+                kids[node].push_back({s[j], child});
+                kids.emplace_back();
+                ++n_edges;
+            }
+            node = child;
+        }
+        return node;
+    }
+    std::vector<int2> edges(uint32_t &mask) const {
+        const uint32_t em = pow2_at_least(2 * n_edges);
+        std::vector<int2> out(em, int2{-1, 0});
+        for (size_t node = 0; node < kids.size(); ++node)
+            for (auto &e : kids[node]) {
+                const int key = static_cast<int>(node << 8) | e.first;
+                uint32_t i = trie_edge_hash(key) & (em - 1);
+                while (out[i].x >= 0) i = (i + 1) & (em - 1);
+                out[i] = int2{key, e.second};
+            }
+        mask = em - 1;
+        return out;
+    }
+};
+
+// the added tokens into `trie`, with their terminal codes in h.term (one per node), first bytes and ids
+inline const char *add_added_tokens(const uint8_t *bytes, const int64_t *offsets, const int32_t *ids, const uint8_t *flags,
+                                    int n_added, TrieBuilder &trie, BpeHost &h) {
+    h.term.assign(1, int2{-1, -1});
+    memset(h.t.first_byte, 0, sizeof(h.t.first_byte));
+    for (int a = 0; a < n_added; ++a) {
+        const int64_t o0 = offsets[a], n = offsets[a + 1] - o0;
+        if (n <= 0) return "empty added token";
+        const int f = flags[a], pass = f & 1;
+        const int node = trie.insert(bytes + o0, n);
+        if (node < 0) return "added tokens too long";
+        h.term.resize(trie.size(), int2{-1, -1});
+        const int code = (a << 2) | (f & 2) | (f >> 2 & 1);     // lstrip << 1 | rstrip
+        int &slot = pass ? h.term[node].y : h.term[node].x;
+        if (slot < 0) slot = code;                    // the same content twice: the first one's id and flags
+        h.t.first_byte[pass][bytes[o0] >> 5] |= 1u << (bytes[o0] & 31);
+        ++h.t.n_pass[pass];
+        h.added_id.push_back(ids[a]);
+    }
+    if (h.added_id.empty()) h.added_id.push_back(0);
+    return nullptr;
+}
+
 inline const char *build_bpe_host_tables(const ac_bpe_tokenizer_spec &s, BpeHost &h) {
     if (!s.cls || !s.byte_ids || (s.n_merges && !s.merges) || s.n_merges < 0) return "null table";
     if (s.split != kSplitGpt2 && s.split != kSplitLlama3) return "unknown split pattern";
@@ -757,52 +827,12 @@ inline const char *build_bpe_host_tables(const ac_bpe_tokenizer_spec &s, BpeHost
         if (const char *why = hash_byte_strings(s.vocab_bytes, s.vocab_offsets, s.vocab_ids, s.n_vocab, h.words, max_key))
             return why;
     }
-    // trie of the added tokens' bytes, nodes numbered from the root 0; edges in an open-addressing table
-    std::vector<std::vector<std::pair<int, int>>> kids(1);
-    h.term.assign(1, int2{-1, -1});
-    memset(h.t.first_byte, 0, sizeof(h.t.first_byte));
-    for (int a = 0; a < s.n_added; ++a) {
-        const int64_t o0 = s.added_offsets[a], n = s.added_offsets[a + 1] - o0;
-        if (n <= 0) return "empty added token";
-        const int f = s.added_flags[a], pass = f & 1;
-        int node = 0;
-        for (int64_t j = 0; j < n; ++j) {
-            const int byte = s.added_bytes[o0 + j];
-            int child = -1;
-            for (auto &e : kids[node])
-                if (e.first == byte) child = e.second;
-            if (child < 0) {
-                child = static_cast<int>(kids.size());
-                if (child >= (1 << 23)) return "added tokens too long";
-                kids[node].push_back({byte, child});
-                kids.emplace_back();
-                h.term.push_back(int2{-1, -1});
-            }
-            node = child;
-        }
-        const int code = (a << 2) | (f & 2) | (f >> 2 & 1);     // lstrip << 1 | rstrip
-        int &slot = pass ? h.term[node].y : h.term[node].x;
-        if (slot < 0) slot = code;                    // the same content twice: the first one's id and flags
-        h.t.first_byte[pass][s.added_bytes[o0] >> 5] |= 1u << (s.added_bytes[o0] & 31);
-        ++h.t.n_pass[pass];
-        h.added_id.push_back(s.added_ids[a]);
-    }
-    if (h.added_id.empty()) h.added_id.push_back(0);
-    size_t n_edges = 0;
-    for (auto &k : kids) n_edges += k.size();
-    const uint32_t em = pow2_at_least(2 * n_edges);
-    h.edges.assign(em, int2{-1, 0});
-    for (size_t node = 0; node < kids.size(); ++node)
-        for (auto &e : kids[node]) {
-            const int key = static_cast<int>(node << 8) | e.first;
-            const uint32_t x = static_cast<uint32_t>(key) * 0x9E3779B1u;
-            uint32_t i = (x ^ (x >> 16)) & (em - 1);
-            while (h.edges[i].x >= 0) i = (i + 1) & (em - 1);
-            h.edges[i] = int2{key, e.second};
-        }
+    TrieBuilder trie;
+    if (const char *why = add_added_tokens(s.added_bytes, s.added_offsets, s.added_ids, s.added_flags, s.n_added, trie, h))
+        return why;
+    h.edges = trie.edges(h.t.edge_mask);
     h.t.merge_mask = mm - 1;
     h.t.word_mask = static_cast<uint32_t>(h.words.size() - 1);
-    h.t.edge_mask = em - 1;
     h.t.split = s.split;
     h.t.prefix_space = s.add_prefix_space ? 1 : 0;
     h.t.ignore_merges = s.ignore_merges ? 1 : 0;
@@ -822,17 +852,321 @@ inline size_t bpe_workspace_bytes(int B, int64_t text_bytes, int max_length) {
     return bpe_fixed_bytes(B, max_length) + (static_cast<size_t>(text_bytes) + B) * kBpeSlotBytes + 256;
 }
 
+// ================================================================ SentencePiece Unigram (XLM-RoBERTa, bge-m3, multilingual-e5)
+// Two kernels of their own, then tokenize_bpe_gather_kernel.  split: one thread per text matches the added tokens as the BPE
+// split does (normalized = false on the raw text; normalized = true on each gap after normalization), normalizes each gap
+// with the Precompiled charsmap, splits it on whitespace and writes every word, "▁" in front unless it starts with one and
+// cut before every later "▁" (Metaspace, prepend_scheme always, split), into the text's word area; at most max_length - 2
+// entries.  viterbi: one thread per word of the whole batch runs the library's lattice over the word's char boundaries in
+// fp64 and writes its tokens, consecutive unknown chars fused into one unk_id, over the word's slots.
+//
+// Precompiled, as the library runs it: the gap is cut into grapheme clusters; a cluster of fewer than 6 bytes that some key
+// is a prefix of becomes the value of the shortest such key, whole; otherwise each char is replaced by its value when it is
+// a key.  A word longer than kMaxUnigramWord bytes is not tokenized on the device: its text is left to the caller as in BPE.
+constexpr int kMaxUnigramWord = AC_UNIGRAM_MAX_WORD;
+constexpr int kPrecompiledCluster = 6;          // clusters this long or longer are normalized char by char
+constexpr double kUnkPenalty = 10.0;            // an unknown char scores the lowest piece score minus this
+constexpr uint32_t kMetaspace = 0x2581;
+// unigram class bits of a codepoint (tokenizer.unigram_classes); kRust (8) is Rust whitespace as for BPE
+enum { kJoin = 1, kControl = 2, kPrepend = 4 };
+
+struct UnigramTables {
+    BpeTables a;                // cls, the byte trie of the added tokens and the charsmap keys, added ids, special ids
+    const int2 *map_val;        // per node of that trie: (offset, length) of the value of the key ending there; x < 0: none
+    const uint8_t *map_pool;
+    int n_map;                  // 0: no normalizer
+    const int2 *piece_edges;    // byte trie of the pieces
+    uint32_t piece_mask;
+    const int32_t *piece_id;    // per piece-trie node: the id of the piece ending there, or -1
+    const double *piece_score;
+    int grow;                   // charsmap value bytes per key byte, at most (1 without a normalizer)
+    int unk_id;
+    double unk_score;
+};
+
+// per text: (bytes + 1) units; a unit holds `grow` bytes of one normalized gap and grow + 3 word slots (a slot: a word byte,
+// its lattice node's score, start and id)
+constexpr size_t kUniSlotBytes = 1 + 8 + 4 + 4;
+inline size_t unigram_unit_bytes(int grow) { return (grow + 3) * kUniSlotBytes + grow; }
+inline size_t unigram_workspace_bytes(int B, int64_t text_bytes, int max_length, int grow) {
+    return bpe_fixed_bytes(B, max_length) + (static_cast<size_t>(text_bytes) + B) * unigram_unit_bytes(grow) + 256;
+}
+
+// a growing byte area of one text
+struct Area {
+    uint8_t *o;
+    int64_t n, cap;
+    bool over;
+};
+
+__device__ inline void area_put(Area &a, const uint8_t *s, int n) {
+    if (a.n + n > a.cap) { a.over = true; return; }
+    for (int i = 0; i < n; ++i) a.o[a.n + i] = s[i];
+    a.n += n;
+}
+
+// the node of the shortest charsmap key that is a prefix of p[i, end), or -1
+__device__ inline int map_prefix(const UnigramTables &t, const uint8_t *p, int64_t i, int64_t end) {
+    int node = 0;
+    for (int64_t j = i; j < end; ++j) {
+        node = trie_child(t.a.edges, t.a.edge_mask, node, p[j]);
+        if (node < 0) return -1;
+        if (t.map_val[node].x >= 0) return node;
+    }
+    return -1;
+}
+
+// the end of the grapheme cluster at i, by the rules that can make one shorter than kPrecompiledCluster bytes: CR LF,
+// nothing joins a control and a control joins nothing, Extend / ZWJ / SpacingMark join what precedes them, Prepend joins
+// what follows it.  Emoji ZWJ sequences (GB11) are not modelled: "©" + ZWJ + "©" is cut after the ZWJ, where the library
+// keeps one 7-byte cluster; the two differ only for a charsmap key that starts with © or ®, which unigram_spec refuses
+__device__ inline int64_t cluster_end(const UnigramTables &t, const uint8_t *p, int64_t i, int64_t end) {
+    uint32_t c;
+    int64_t j = i + utf8_decode(p + i, p + end, c);
+    if (c == '\r') return j < end && p[j] == '\n' ? j + 1 : j;
+    int prev = t.a.cls[c];
+    if (prev & kControl) return j;
+    while (j < end) {
+        uint32_t d;
+        const int n = utf8_decode(p + j, p + end, d);
+        const int k = t.a.cls[d];
+        if ((k & kControl) || !((k & kJoin) || (prev & kPrepend))) break;
+        j += n;
+        prev = k;
+    }
+    return j;
+}
+
+__device__ inline void put_value(const UnigramTables &t, Area &o, int node) {
+    const int2 v = t.map_val[node];
+    area_put(o, t.map_pool + v.x, v.y);
+}
+
+// Precompiled over raw bytes [a, b) into o (valid UTF-8: an invalid byte becomes U+FFFD, as everywhere in this file)
+__device__ inline void normalize_gap(const UnigramTables &t, const uint8_t *p, int64_t a, int64_t b, Area &o) {
+    uint8_t buf[4];
+    for (int64_t i = a; i < b && !o.over;) {
+        const int64_t j = t.n_map ? cluster_end(t, p, i, b) : b;
+        if (t.n_map && j - i < kPrecompiledCluster) {
+            const int node = map_prefix(t, p, i, j);
+            if (node >= 0) {
+                put_value(t, o, node);
+                i = j;
+                continue;
+            }
+        }
+        for (; i < j && !o.over;) {
+            uint32_t c;
+            const int n = utf8_decode(p + i, p + b, c);
+            const int node = t.n_map ? map_prefix(t, p, i, i + n) : -1;
+            if (node >= 0) put_value(t, o, node);
+            else area_put(o, buf, utf8_encode(c, buf));
+            i += n;
+        }
+    }
+}
+
+// WhitespaceSplit + Metaspace over normalized bytes [a, b) of g: each word into the word area w, one entry each
+__device__ inline void split_words(const UnigramTables &t, const uint8_t *g, int64_t a, int64_t b, Area &w,
+                                   Entries &o) {
+    const uint8_t meta[3] = {0xE2, 0x96, 0x81};
+    int64_t start = -1;
+    for (int64_t i = a; i <= b && !o.huge;) {
+        uint32_t c = ' ';
+        const int n = i < b ? utf8_decode(g + i, g + b, c) : 1;
+        const bool space = i == b || (t.a.cls[c] & kRust);
+        if (start >= 0 && (space || c == kMetaspace)) {               // the word ends
+            const int64_t len = w.n - start;
+            if (len > kMaxUnigramWord) { o.huge = true; return; }
+            o.e[o.n++] = int2{static_cast<int>(start), static_cast<int>(len)};
+            start = -1;
+        }
+        if (!space) {
+            if (start < 0) {
+                if (o.n >= o.limit) return;
+                start = w.n;
+                if (c != kMetaspace) area_put(w, meta, 3);
+            }
+            area_put(w, g + i, n);
+            if (w.over) { o.huge = true; return; }
+        }
+        i += n;
+    }
+}
+
+// entries of text b: ws_ent[b, 0 .. n_ent[b]), words as (first slot, bytes) in the text's word area; n_ent[b] = -1 and
+// lengths[b] = -1 for a text left to the caller
+__global__ void __launch_bounds__(128) tokenize_unigram_split_kernel(UnigramTables t, const uint8_t *text,
+                                                                     const int64_t *offsets, int B, int max_length,
+                                                                     int64_t n_units, int32_t *lengths, int32_t *max_len,
+                                                                     int2 *ws_ent, int32_t *n_ent, uint8_t *ws_words,
+                                                                     uint8_t *ws_gap) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const uint8_t *p = text + offsets[b];
+    const int64_t len = offsets[b + 1] - offsets[b], unit = offsets[b] - offsets[0] + b;
+    const int limit = max_length - 2;
+    Entries o{ws_ent + static_cast<int64_t>(b) * limit, 0, limit, 0, false};
+    Area w{ws_words + unit * (t.grow + 3), 0, (len + 1) * (t.grow + 3), false};
+    Area g{ws_gap + unit * t.grow, 0, (len + 1) * t.grow, false};
+    if (unit + len + 1 > n_units || len >= INT32_MAX / (t.grow + 3)) o.huge = true;   // the workspace holds fewer units
+    for (int64_t g1 = 0; g1 <= len && o.n < o.limit && !o.huge;) {
+        int64_t s1, e1;
+        const int code1 = next_added(t.a, 0, p, g1, len, &s1, &e1);
+        g.n = 0;
+        normalize_gap(t, p, g1, s1, g);
+        if (g.over) o.huge = true;
+        for (int64_t g2 = 0; o.n < o.limit && !o.huge;) {
+            int64_t s2, e2;
+            const int code2 = next_added(t.a, 1, g.o, g2, g.n, &s2, &e2);
+            split_words(t, g.o, g2, s2, w, o);
+            if (code2 < 0) break;
+            emit_added(o, t.a, code2);
+            g2 = e2;
+        }
+        if (code1 < 0 || o.huge) break;
+        emit_added(o, t.a, code1);
+        g1 = e1;
+    }
+    n_ent[b] = o.huge ? -1 : o.n;
+    if (o.huge) {
+        lengths[b] = -1;
+        atomicMax(max_len + 1, 1);
+    }
+}
+
+// the Unigram tokens of entry k of text b (tokenizers' Unigram::encode_optimized): char boundaries left to right, pieces
+// from each shortest first, a candidate kept only when strictly better; a char no one-char piece covers is unk.  The node
+// of the best path ending after byte e sits at slot e; the tokens are written back to front over the word's last slots,
+// which never reach a node still to be read.  The entry becomes (its first token's slot, -tokens).
+__global__ void __launch_bounds__(128) tokenize_unigram_viterbi_kernel(UnigramTables t, const int64_t *offsets, int B,
+                                                                       int max_length, int2 *ws_ent, const int32_t *n_ent,
+                                                                       const uint8_t *ws_words, double *ws_score,
+                                                                       int32_t *ws_start, int32_t *ws_tok) {
+    const int limit = max_length - 2;
+    const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    if (gid >= static_cast<int64_t>(B) * limit) return;
+    const int b = static_cast<int>(gid / limit), k = static_cast<int>(gid - static_cast<int64_t>(b) * limit);
+    if (k >= n_ent[b]) return;
+    int2 &ent = ws_ent[gid];
+    if (ent.y <= 0) return;
+    const int n = ent.y;
+    const int64_t base = (offsets[b] - offsets[0] + b) * (t.grow + 3) + ent.x;
+    const uint8_t *w = ws_words + base;
+    double *sc = ws_score + base;
+    int32_t *st = ws_start + base, *id = ws_tok + base;
+    for (int e = 0; e < n; ++e) st[e] = -1;
+    for (int s = 0; s < n;) {
+        const double here = s ? sc[s - 1] : 0.0;
+        const uint8_t lead = w[s];
+        const int mblen = std::min(lead < 0x80 ? 1 : lead >= 0xF0 ? 4 : lead >= 0xE0 ? 3 : 2, n - s);
+        bool single = false;
+        int node = 0;
+        for (int e = s; e < n; ++e) {
+            node = trie_child(t.piece_edges, t.piece_mask, node, w[e]);
+            if (node < 0) break;
+            const int v = t.piece_id[node];
+            if (v < 0) continue;
+            const double cand = here + t.piece_score[node];
+            if (st[e] < 0 || cand > sc[e]) { sc[e] = cand; st[e] = s; id[e] = v; }
+            if (e + 1 - s == mblen) single = true;
+        }
+        if (!single) {
+            const int e = s + mblen - 1;
+            const double cand = here + t.unk_score;
+            if (st[e] < 0 || cand > sc[e]) { sc[e] = cand; st[e] = s; id[e] = t.unk_id; }
+        }
+        s += mblen;
+    }
+    int c = 0;
+    bool unk = false;
+    for (int e = n; e > 0;) {
+        const int s = st[e - 1], v = id[e - 1];
+        if (!(unk && v == t.unk_id)) id[n - 1 - c++] = v;
+        unk = v == t.unk_id;
+        e = s;
+    }
+    ent.x += n - c;
+    ent.y = -c;
+}
+
+// ---------------------------------------------------------------- host side of the Unigram tables
+struct UnigramHost {
+    BpeHost a;                  // the added tokens' terminal codes, edges (charsmap keys too) and ids
+    std::vector<int2> map_val, piece_edges;
+    std::vector<uint8_t> map_pool;
+    std::vector<int32_t> piece_id;
+    std::vector<double> piece_score;
+    UnigramTables t{};          // scalars filled; pointers left to the owner
+};
+
+inline const char *build_unigram_host_tables(const ac_unigram_tokenizer_spec &s, UnigramHost &h) {
+    if (!s.cls || !s.piece_bytes || !s.piece_offsets || !s.piece_scores || s.n_pieces <= 0) return "null table or no pieces";
+    if (s.n_map < 0 || (s.n_map && (!s.map_keys || !s.map_key_offsets || !s.map_values || !s.map_value_offsets)))
+        return "bad charsmap";
+    if (s.grow < 1 || s.grow > 64) return "charsmap expansion outside 1..64 bytes per byte";
+    if (s.unk_id < 0 || s.unk_id >= s.n_pieces) return "unk_id outside the pieces";
+    if (s.n_added < 0 || (s.n_added && (!s.added_bytes || !s.added_offsets || !s.added_ids || !s.added_flags)))
+        return "bad added tokens";
+    TrieBuilder trie;
+    if (const char *why = add_added_tokens(s.added_bytes, s.added_offsets, s.added_ids, s.added_flags, s.n_added, trie, h.a))
+        return why;
+    for (int k = 0; k < s.n_map; ++k) {
+        const int64_t k0 = s.map_key_offsets[k], kn = s.map_key_offsets[k + 1] - k0;
+        const int64_t v0 = s.map_value_offsets[k], vn = s.map_value_offsets[k + 1] - v0;
+        if (kn <= 0 || vn < 0 || vn > s.grow * kn) return "empty charsmap key, or a value longer than grow allows";
+        const int node = trie.insert(s.map_keys + k0, kn);
+        if (node < 0) return "charsmap too large";
+        h.map_val.resize(trie.size(), int2{-1, 0});
+        if (h.map_pool.size() + vn > INT32_MAX) return "charsmap values over 2 GB";
+        h.map_val[node] = int2{static_cast<int>(h.map_pool.size()), static_cast<int>(vn)};
+        h.map_pool.insert(h.map_pool.end(), s.map_values + v0, s.map_values + v0 + vn);
+    }
+    h.map_val.resize(trie.size(), int2{-1, 0});
+    h.a.term.resize(trie.size(), int2{-1, -1});
+    if (h.map_pool.empty()) h.map_pool.push_back(0);
+    h.a.edges = trie.edges(h.a.t.edge_mask);
+    // the pieces: the library keeps the last id of a repeated piece, and its score; the lowest score of all sets unk's
+    TrieBuilder pieces;
+    double lowest = 0.0;
+    for (int v = 0; v < s.n_pieces; ++v) {
+        const int64_t o0 = s.piece_offsets[v], n = s.piece_offsets[v + 1] - o0;
+        if (n <= 0) return "empty piece";
+        const int node = pieces.insert(s.piece_bytes + o0, n);
+        if (node < 0) return "pieces too large";
+        h.piece_id.resize(pieces.size(), -1);
+        h.piece_score.resize(pieces.size(), 0.0);
+        h.piece_id[node] = v;
+        h.piece_score[node] = s.piece_scores[v];
+        lowest = v ? std::min(lowest, s.piece_scores[v]) : s.piece_scores[v];
+    }
+    h.piece_id.resize(pieces.size(), -1);
+    h.piece_score.resize(pieces.size(), 0.0);
+    h.piece_edges = pieces.edges(h.t.piece_mask);
+    h.t.a = h.a.t;
+    h.t.a.cls_id = s.cls_id;
+    h.t.a.sep_id = s.sep_id;
+    h.t.a.pad_id = s.pad_id;
+    h.t.n_map = s.n_map;
+    h.t.grow = s.grow;
+    h.t.unk_id = s.unk_id;
+    h.t.unk_score = lowest - kUnkPenalty;
+    return nullptr;
+}
+
 }  // namespace tok
 }  // namespace ac
 
 #ifndef AC_CPU_SHIM
 using namespace ac;
 
-// one handle type for both kinds: `bpe` tells which of the two table sets the calls read
+// one handle type for every kind: `kind` tells which table set the calls read
+enum TokKind { kWordPiece, kBpe, kUnigram };
 struct ac_tokenizer {
-    bool bpe;
+    TokKind kind;
     tok::Tables t;
     tok::BpeTables b;
+    tok::UnigramTables u;
     int pad_id;
     std::vector<void *> owned;
 };
@@ -862,7 +1196,7 @@ extern "C" int ac_tokenizer_create(const ac_tokenizer_spec *spec, ac_tokenizer *
         return AC_E_INVALID;
     }
     ac_tokenizer *k = new ac_tokenizer();
-    k->bpe = false;
+    k->kind = kWordPiece;
     k->t = h.t;
     k->pad_id = h.t.pad_id;
     const void *p[8];
@@ -900,7 +1234,7 @@ extern "C" int ac_tokenizer_create_bpe(const ac_bpe_tokenizer_spec *spec, ac_tok
         return AC_E_INVALID;
     }
     ac_tokenizer *k = new ac_tokenizer();
-    k->bpe = true;
+    k->kind = kBpe;
     k->b = h.t;
     k->pad_id = h.t.pad_id;
     const void *p[7];
@@ -927,10 +1261,49 @@ extern "C" int ac_tokenizer_create_bpe(const ac_bpe_tokenizer_spec *spec, ac_tok
     return AC_OK;
 }
 
+extern "C" int ac_tokenizer_create_unigram(const ac_unigram_tokenizer_spec *spec, ac_tokenizer **out) {
+    AC_REQUIRE(spec && out, "ac_tokenizer_create_unigram: null argument");
+    *out = nullptr;
+    tok::UnigramHost h;
+    if (const char *why = tok::build_unigram_host_tables(*spec, h)) {
+        set_error("ac_tokenizer_create_unigram: %s", why);
+        return AC_E_INVALID;
+    }
+    ac_tokenizer *k = new ac_tokenizer();
+    k->kind = kUnigram;
+    k->u = h.t;
+    k->pad_id = spec->pad_id;
+    const void *p[10];
+    int rc = AC_OK;
+    if ((rc = tok_upload(k, spec->cls, tok::kCodepoints, &p[0])) ||
+        (rc = tok_upload(k, h.a.edges.data(), sizeof(int2) * h.a.edges.size(), &p[1])) ||
+        (rc = tok_upload(k, h.a.term.data(), sizeof(int2) * h.a.term.size(), &p[2])) ||
+        (rc = tok_upload(k, h.a.added_id.data(), sizeof(int32_t) * h.a.added_id.size(), &p[3])) ||
+        (rc = tok_upload(k, h.map_val.data(), sizeof(int2) * h.map_val.size(), &p[4])) ||
+        (rc = tok_upload(k, h.map_pool.data(), h.map_pool.size(), &p[5])) ||
+        (rc = tok_upload(k, h.piece_edges.data(), sizeof(int2) * h.piece_edges.size(), &p[6])) ||
+        (rc = tok_upload(k, h.piece_id.data(), sizeof(int32_t) * h.piece_id.size(), &p[7])) ||
+        (rc = tok_upload(k, h.piece_score.data(), sizeof(double) * h.piece_score.size(), &p[8]))) {
+        ac_tokenizer_destroy(k);
+        return rc;
+    }
+    k->u.a.cls = static_cast<const uint8_t *>(p[0]);
+    k->u.a.edges = static_cast<const int2 *>(p[1]);
+    k->u.a.term = static_cast<const int2 *>(p[2]);
+    k->u.a.added_id = static_cast<const int32_t *>(p[3]);
+    k->u.map_val = static_cast<const int2 *>(p[4]);
+    k->u.map_pool = static_cast<const uint8_t *>(p[5]);
+    k->u.piece_edges = static_cast<const int2 *>(p[6]);
+    k->u.piece_id = static_cast<const int32_t *>(p[7]);
+    k->u.piece_score = static_cast<const double *>(p[8]);
+    *out = k;
+    return AC_OK;
+}
+
 extern "C" int ac_tokenize_workspace_bytes(const ac_tokenizer *tok, int B, size_t *bytes) {
     AC_REQUIRE(tok && bytes && B >= 0, "ac_tokenize_workspace_bytes: bad arguments");
-    AC_REQUIRE(!tok->bpe, "ac_tokenize_workspace_bytes: a BPE handle's workspace depends on the text bytes; use "
-                          "ac_tokenize_workspace_bytes_text");
+    AC_REQUIRE(tok->kind == kWordPiece, "ac_tokenize_workspace_bytes: a %s handle's workspace depends on the text bytes; use "
+               "ac_tokenize_workspace_bytes_text", tok->kind == kBpe ? "BPE" : "Unigram");
     *bytes = tok::workspace_bytes(tok->t.max_chars, B);
     return AC_OK;
 }
@@ -938,7 +1311,9 @@ extern "C" int ac_tokenize_workspace_bytes(const ac_tokenizer *tok, int B, size_
 extern "C" int ac_tokenize_workspace_bytes_text(const ac_tokenizer *tok, int B, int64_t text_bytes, int max_length,
                                                 size_t *bytes) {
     AC_REQUIRE(tok && bytes && B >= 0 && text_bytes >= 0 && max_length >= 2, "ac_tokenize_workspace_bytes_text: bad arguments");
-    *bytes = tok->bpe ? tok::bpe_workspace_bytes(B, text_bytes, max_length) : tok::workspace_bytes(tok->t.max_chars, B);
+    *bytes = tok->kind == kBpe       ? tok::bpe_workspace_bytes(B, text_bytes, max_length)
+             : tok->kind == kUnigram ? tok::unigram_workspace_bytes(B, text_bytes, max_length, tok->u.grow)
+                                     : tok::workspace_bytes(tok->t.max_chars, B);
     return AC_OK;
 }
 
@@ -970,13 +1345,48 @@ static int tokenize_bpe(const ac_tokenizer *tok, const uint8_t *text, const int6
     return AC_OK;
 }
 
+static int tokenize_unigram(const ac_tokenizer *tok, const uint8_t *text, const int64_t *offsets, int B, int max_length,
+                            int32_t *tokens, int32_t *lengths, int32_t *max_len, void *workspace, size_t workspace_bytes,
+                            cudaStream_t s) {
+    const tok::UnigramTables &u = tok->u;
+    const size_t fixed = tok::bpe_fixed_bytes(B, max_length);
+    AC_REQUIRE(workspace && workspace_bytes >= tok::unigram_workspace_bytes(B, 0, max_length, u.grow),
+               "ac_tokenize: workspace too small");
+    // the units the workspace holds; a text past them is left to the caller like a text with a huge word
+    const int64_t n_units = static_cast<int64_t>((workspace_bytes - fixed - 256) / tok::unigram_unit_bytes(u.grow));
+    const int64_t n_slots = n_units * (u.grow + 3);
+    int2 *ent = static_cast<int2 *>(workspace);
+    int32_t *n_ent = reinterpret_cast<int32_t *>(ent + static_cast<size_t>(B) * (max_length - 2));
+    double *ws_score = reinterpret_cast<double *>(static_cast<uint8_t *>(workspace) + fixed);
+    int32_t *ws_start = reinterpret_cast<int32_t *>(ws_score + n_slots);
+    int32_t *ws_tok = ws_start + n_slots;
+    uint8_t *ws_words = reinterpret_cast<uint8_t *>(ws_tok + n_slots);
+    uint8_t *ws_gap = ws_words + n_slots;
+    AC_CUDA(cudaMemsetAsync(max_len, 0, 2 * sizeof(int32_t), s));
+    tok::tokenize_unigram_split_kernel<<<(B + 127) / 128, 128, 0, s>>>(u, text, offsets, B, max_length, n_units, lengths,
+                                                                       max_len, ent, n_ent, ws_words, ws_gap);
+    AC_LAUNCH_CHECK();
+    const int64_t words = static_cast<int64_t>(B) * (max_length - 2);
+    if (words) {
+        tok::tokenize_unigram_viterbi_kernel<<<static_cast<unsigned>((words + 127) / 128), 128, 0, s>>>(
+            u, offsets, B, max_length, ent, n_ent, ws_words, ws_score, ws_start, ws_tok);
+        AC_LAUNCH_CHECK();
+    }
+    tok::tokenize_bpe_gather_kernel<<<(B + 3) / 4, 128, 0, s>>>(u.a, offsets, B, max_length, ent, n_ent, ws_tok, tokens,
+                                                                lengths, max_len, u.grow + 3);
+    AC_LAUNCH_CHECK();
+    return AC_OK;
+}
+
 extern "C" int ac_tokenize(const ac_tokenizer *tok, const uint8_t *text, const int64_t *offsets, int B, int max_length,
                            int32_t *tokens, int32_t *lengths, int32_t *max_len, void *workspace, size_t workspace_bytes,
                            ac_stream_t stream) {
     AC_REQUIRE(tok && text && offsets && tokens && lengths && max_len && B >= 1, "ac_tokenize: bad arguments");
     AC_REQUIRE(max_length >= 2, "ac_tokenize: max_length=%d < 2 leaves no room for the two special tokens", max_length);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (tok->bpe) return tokenize_bpe(tok, text, offsets, B, max_length, tokens, lengths, max_len, workspace, workspace_bytes, s);
+    if (tok->kind == kUnigram)
+        return tokenize_unigram(tok, text, offsets, B, max_length, tokens, lengths, max_len, workspace, workspace_bytes, s);
+    if (tok->kind == kBpe) return tokenize_bpe(tok, text, offsets, B, max_length, tokens, lengths, max_len, workspace, workspace_bytes, s);
     AC_REQUIRE(workspace && workspace_bytes >= tok::workspace_bytes(tok->t.max_chars, B), "ac_tokenize: workspace too small");
     uint32_t *ws_cp = static_cast<uint32_t *>(workspace);
     uint8_t *ws_bytes = reinterpret_cast<uint8_t *>(ws_cp + static_cast<size_t>(B) * (tok->t.max_chars + 1));

@@ -1,4 +1,4 @@
-"""Which Hugging Face tokenizers the device tokenizers (csrc/tokenizer.cu: WordPiece, byte-level BPE) reproduce, and the Unicode
+"""Which Hugging Face tokenizers the device tokenizers (csrc/tokenizer.cu: WordPiece, byte-level BPE, Unigram) reproduce, and the Unicode
 tables they run on.
 
 The tables are derived by probing the installed `tokenizers` library (`normalize_str`, `pre_tokenize_str`), not from Python's
@@ -350,6 +350,36 @@ def _rust_space(ch: str) -> bool:
     return bool(bpe_classes()[ord(ch)] & BPE_RUST)
 
 
+def _added_and_wrapper(tokenizer, bt, added) -> str:
+    """"" when the truncation and padding sides, the added tokens and the Python wrapper are ones the BPE and Unigram split
+    kernels reproduce (added tokens matched in two passes with lstrip / rstrip), else the reason"""
+    if getattr(tokenizer, "truncation_side", "right") != "right" or getattr(tokenizer, "padding_side", "right") != "right":
+        return "left truncation or left padding"
+    if getattr(bt, "encode_special_tokens", False):
+        return "encode_special_tokens splits the special tokens"
+    for a in added:
+        if a.get("single_word", False):
+            return f"added token {a.get('content')!r} with single_word=True"
+        if not a.get("content"):
+            return "empty added token"
+    for norm in (False, True):
+        group = [a for a in added if bool(a.get("normalized", True)) == norm]
+        if any(a.get("rstrip") for a in group) and any(_rust_space(a["content"][0]) for a in group):
+            # the library resumes its scan inside the whitespace an rstrip token took, where such a token may match
+            return "an rstrip added token next to one that starts with whitespace"
+    if tokenizer.pad_token_id is None:
+        return "no pad token"
+    probe = _REPRESENTATIVE + [f"x{a['content']}y {a['content']} " for a in added]
+    try:
+        wrapped = tokenizer(probe)["input_ids"]
+        backend = [e.ids for e in bt.encode_batch(probe)]
+    except Exception as e:                       # noqa: BLE001 -- any failure means: not a shape we reproduce
+        return f"probe encoding failed: {e}"
+    if wrapped != backend:
+        return "the Python wrapper changes the text before the backend sees it"
+    return ""
+
+
 def bpe_spec(tokenizer) -> Tuple[Optional[dict], str]:
     """(spec, "") when the tokenizer is a byte-level BPE tokenizer the device kernels reproduce id for id, else (None, reason).
     Read from `backend_tokenizer.to_str()`; accepts nothing looser than: a BPE model without dropout, affixes or byte fallback
@@ -396,31 +426,10 @@ def bpe_spec(tokenizer) -> Tuple[Optional[dict], str]:
     pair, why = _special_pair(post)
     if pair is None:
         return None, why
-    if getattr(tokenizer, "truncation_side", "right") != "right" or getattr(tokenizer, "padding_side", "right") != "right":
-        return None, "left truncation or left padding"
-    if getattr(bt, "encode_special_tokens", False):
-        return None, "encode_special_tokens splits the special tokens"
     added = j.get("added_tokens") or []
-    for a in added:
-        if a.get("single_word", False):
-            return None, f"added token {a.get('content')!r} with single_word=True"
-        if not a.get("content"):
-            return None, "empty added token"
-    for norm in (False, True):
-        group = [a for a in added if bool(a.get("normalized", True)) == norm]
-        if any(a.get("rstrip") for a in group) and any(_rust_space(a["content"][0]) for a in group):
-            # the library resumes its scan inside the whitespace an rstrip token took, where such a token may match
-            return None, "an rstrip added token next to one that starts with whitespace"
-    if tokenizer.pad_token_id is None:
-        return None, "no pad token"
-    probe = _REPRESENTATIVE + [f"x{a['content']}y {a['content']} " for a in added]
-    try:
-        wrapped = tokenizer(probe)["input_ids"]
-        backend = [e.ids for e in bt.encode_batch(probe)]
-    except Exception as e:                       # noqa: BLE001 -- any failure means: not a shape we reproduce
-        return None, f"probe encoding failed: {e}"
-    if wrapped != backend:
-        return None, "the Python wrapper changes the text before the backend sees it"
+    why = _added_and_wrapper(tokenizer, bt, added)
+    if why:
+        return None, why
     merges = []
     for m in model.get("merges") or []:
         a, b = m.split(" ", 1) if isinstance(m, str) else m
@@ -451,3 +460,208 @@ def pack_strings(strings) -> Tuple[np.ndarray, np.ndarray]:
     off = np.zeros(len(enc) + 1, dtype=np.int64)
     np.cumsum([len(e) for e in enc], out=off[1:])
     return np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8), off
+
+
+# ================================================================ SentencePiece Unigram, XLM-R shape (csrc/tokenizer.cu, tokenize_unigram_*)
+G_JOIN, G_CONTROL, G_PREPEND = 1, 2, 4      # grapheme class bits; BPE_RUST (8) is Rust whitespace, as in bpe_classes
+METASPACE = "▁"
+# the Extended_Pictographic chars shorter than 3 bytes: "©" + ZWJ is a 5-byte prefix of a longer emoji ZWJ cluster (GB11),
+# which the device does not model, so it reads "©‍©" as "©‍" + "©"; that differs from the library only when a charsmap key
+# starts with one of them (none of sentencepiece's built-in rules has such a key)
+_EXT_PICT_2BYTE = ("©".encode(), "®".encode())
+UNIGRAM_MAX_WORD = 4096                     # AC_UNIGRAM_MAX_WORD
+
+
+def decode_charsmap(blob: bytes) -> list:
+    """[(key bytes, value bytes)] of a SentencePiece `precompiled_charsmap`: a 4-byte little-endian trie size, a double-array
+    trie of uint32 units (darts-clone layout: bits 0-7 the label, bit 8 has-leaf, bit 9 scales the offset in bits 10-31; a
+    leaf unit's bits 0-30 are the value) and the pool of NUL-terminated values the leaves point into.  Walked breadth first,
+    every live node against every byte at once."""
+    n = int.from_bytes(blob[:4], "little")
+    if n % 4 or 4 + n > len(blob):
+        raise ValueError("precompiled_charsmap: trie size past the blob")
+    units = np.frombuffer(blob, dtype="<u4", count=n // 4, offset=4).astype(np.int64)
+    pool = blob[4 + n:]
+    if not len(units):
+        return []
+
+    def offset(u):
+        return (u >> 10) << ((u & (1 << 9)) >> 6)
+
+    labels = np.arange(1, 256, dtype=np.int64)
+    pos = np.asarray([offset(units[0])], dtype=np.int64)
+    keys = [b""]
+    out = []
+    for _ in range(64):                         # no key is longer; a deeper walk means a corrupt trie
+        if not len(pos):
+            break
+        child = pos[:, None] ^ labels[None, :]
+        inside = child < len(units)
+        u = np.where(inside, units[np.where(inside, child, 0)], -1)
+        hit = inside & ((u & ((1 << 31) | 0xFF)) == labels[None, :])
+        pi, li = np.nonzero(hit)
+        ch, uu = child[pi, li], u[pi, li]
+        nxt = ch ^ offset(uu)
+        if (nxt >= len(units)).any():
+            raise ValueError("precompiled_charsmap: node past the trie")
+        new_keys = [keys[p] + bytes([int(labels[l])]) for p, l in zip(pi.tolist(), li.tolist())]
+        for k, leaf, q in zip(new_keys, ((uu >> 8) & 1).tolist(), nxt.tolist()):
+            if leaf:
+                v = int(units[q] & 0x7FFFFFFF)
+                end = pool.find(b"\0", v)
+                if v > len(pool) or end < 0:
+                    raise ValueError("precompiled_charsmap: value past the pool")
+                out.append((k, bytes(pool[v:end])))
+        pos, keys = nxt, new_keys
+    else:
+        raise ValueError("precompiled_charsmap: key longer than 64 bytes")
+    return sorted(out)
+
+
+def charsmap_tables(blob: bytes) -> dict:
+    """decoded charsmap of a Precompiled normalizer: pairs, and the largest expansion in value bytes per key byte (rounded up,
+    at least 1), which sizes the device workspace.  Every single-codepoint key is checked against the library's
+    normalize_str: a blob this decoder misreads is refused rather than tokenized differently.  Kept per blob in the process."""
+    key = ("charsmap", hashlib.sha256(blob).hexdigest())
+    if key in _CACHE:
+        return _CACHE[key]
+    from tokenizers import normalizers
+    pairs = decode_charsmap(blob)
+    single = [(k.decode("utf-8"), v.decode("utf-8")) for k, v in pairs if len(k.decode("utf-8", "replace")) == 1]
+    nz = normalizers.Precompiled(blob)
+    bad = [k for k, v in single if nz.normalize_str(k) != v]
+    if bad:
+        raise ValueError(f"precompiled_charsmap decoded differently from the library for {len(bad)} keys, e.g. {bad[0]!r}")
+    grow = max([1] + [-(-len(v) // len(k)) for k, v in pairs])
+    res = dict(pairs=pairs, grow=grow)
+    _CACHE[key] = res
+    return res
+
+
+def all_to_b_charsmap() -> bytes:
+    """a charsmap that maps every codepoint but NUL and the surrogates to 'b' ('b' included), compiled by sentencepiece from a
+    rule table: under it, normalize_str of a string shorter than 6 bytes has one char per grapheme cluster the library cuts
+    it into (a cluster that holds NUL is NUL alone)"""
+    import io
+    import sentencepiece as spm
+    from sentencepiece import sentencepiece_model_pb2
+    with tempfile.TemporaryDirectory() as d:
+        rules = os.path.join(d, "rules.tsv")
+        with open(rules, "w") as f:
+            f.writelines(f"{c:X}\t62\n" for c in probe_codepoints().tolist() if c)
+        corpus = [f"probe line {i} of the grapheme class table" for i in range(200)]
+        model = io.BytesIO()
+        spm.SentencePieceTrainer.train(sentence_iterator=iter(corpus), model_writer=model, vocab_size=60, model_type="unigram",
+                                       hard_vocab_limit=False, normalization_rule_tsv=rules, minloglevel=2)
+    m = sentencepiece_model_pb2.ModelProto()
+    m.ParseFromString(model.getvalue())
+    return m.normalizer_spec.precompiled_charsmap
+
+
+def unigram_classes() -> np.ndarray:
+    """uint8 [N_CODEPOINTS] in the layout of ac_unigram_tokenizer_spec.cls: the grapheme cluster classes of the library's
+    segmentation (unicode-segmentation) that can change a Precompiled result, and Rust whitespace (WhitespaceSplit, lstrip /
+    rstrip).  Under a charsmap mapping every codepoint to 'b', one 'b' means one cluster:
+      G_JOIN     'a' + c is one cluster (Extend, ZWJ, SpacingMark);
+      G_CONTROL  c + U+0301 is two (Control, CR, LF: nothing joins them, and they join nothing);
+      G_PREPEND  c + 'x' is one (Prepend).
+    Clusters of 6 bytes or more are normalized char by char, so the rules that only build such clusters (Hangul, regional
+    indicators, emoji ZWJ sequences, conjuncts) need no class; unigram_spec refuses the one charsmap shape where that would
+    show (see _EXT_PICT_2BYTE).  The count of output chars, not which char comes out, decides each bit, so the mapping target
+    is probed like any other codepoint.  Kept in the process and on disk."""
+    import tokenizers
+    key = ("unigram", tokenizers.__version__)
+    if key in _CACHE:
+        return _CACHE[key]
+    path = _disk_cache_path(key[1:], "unigram")
+    try:
+        with np.load(path) as z:
+            cls = z["cls"]
+    except (OSError, KeyError, ValueError):
+        from tokenizers import normalizers, pre_tokenizers
+        nz = normalizers.Precompiled(all_to_b_charsmap())
+        cps = probe_codepoints()
+        chars = list(map(chr, cps.tolist()))
+
+        def clusters(s):
+            return len(nz.normalize_str(s))
+
+        sub = np.zeros(len(chars), dtype=np.uint8)
+        sub |= np.fromiter((clusters("a" + c) == 1 for c in chars), dtype=bool, count=len(chars)).astype(np.uint8) * G_JOIN
+        sub |= np.fromiter((len(c.encode()) < 4 and clusters(c + "́") == 2 for c in chars), dtype=bool,
+                           count=len(chars)).astype(np.uint8) * G_CONTROL
+        sub |= np.fromiter((clusters(c + "x") == 1 for c in chars), dtype=bool, count=len(chars)).astype(np.uint8) * G_PREPEND
+        sub |= np.where(_uncovered(pre_tokenizers.WhitespaceSplit(), chars), BPE_RUST, 0).astype(np.uint8)
+        if clusters("\r\n") != 1:
+            raise ValueError("CR LF is not one grapheme cluster to this library")
+        cls = np.zeros(N_CODEPOINTS, dtype=np.uint8)
+        cls[cps] = sub
+        try:
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+            fd, tmp = tempfile.mkstemp(dir=os.path.dirname(path), suffix=".npz")
+            with os.fdopen(fd, "wb") as f:
+                np.savez(f, cls=cls)
+            os.replace(tmp, path)
+        except OSError as e:
+            logger.debug(f"tokenizer tables not cached on disk: {e}")
+    _CACHE[key] = cls
+    return cls
+
+
+def unigram_spec(tokenizer) -> Tuple[Optional[dict], str]:
+    """(spec, "") when the tokenizer is a SentencePiece Unigram tokenizer of the XLM-RoBERTa shape that the device kernels
+    reproduce id for id, else (None, reason).  Read from `backend_tokenizer.to_str()` (what AutoTokenizer actually runs);
+    accepts nothing looser than: a Unigram model without byte_fallback and with an unk_id, no normalizer or Precompiled, the
+    pre-tokenizer Sequence[WhitespaceSplit, Metaspace('▁', prepend_scheme 'always', split)], a '[special] A [special]'
+    post-processor with type id 0, right truncation and padding, added tokens with single_word = false, and a Python wrapper
+    that passes the text through unchanged."""
+    import base64
+    bt = getattr(tokenizer, "backend_tokenizer", None)
+    if bt is None:
+        return None, "no Rust `tokenizers` backend (slow tokenizer)"
+    j = json.loads(bt.to_str())
+    model, nrm, pre, post = j.get("model") or {}, j.get("normalizer"), j.get("pre_tokenizer") or {}, j.get("post_processor") or {}
+    if model.get("type") != "Unigram":
+        return None, f"model {model.get('type')!r} is not Unigram"
+    if model.get("byte_fallback"):
+        return None, "Unigram byte_fallback"
+    if model.get("unk_id") is None:
+        return None, "Unigram without unk_id"
+    if nrm is not None and nrm.get("type") != "Precompiled":
+        return None, f"normalizer {nrm.get('type')!r} is not Precompiled (or none)"
+    seq = pre.get("pretokenizers") or []
+    if pre.get("type") != "Sequence" or [p.get("type") for p in seq] != ["WhitespaceSplit", "Metaspace"]:
+        return None, f"pre_tokenizer {pre.get('type')!r} is not Sequence[WhitespaceSplit, Metaspace]"
+    ms = seq[1]
+    if ms.get("replacement") != METASPACE or ms.get("prepend_scheme") != "always" or not ms.get("split", True):
+        return None, "Metaspace is not ('▁', prepend_scheme 'always', split)"
+    pair, why = _special_pair(post)
+    if pair is None:
+        return None, why
+    vocab = model.get("vocab") or []
+    if not vocab or any(not p for p, _ in vocab):
+        return None, "empty Unigram vocab or an empty piece"
+    unk_id = int(model["unk_id"])
+    if not 0 <= unk_id < len(vocab):
+        return None, "unk_id outside the vocab"
+    added = j.get("added_tokens") or []
+    why = _added_and_wrapper(tokenizer, bt, added)
+    if why:
+        return None, why
+    try:
+        cmap = charsmap_tables(base64.b64decode(nrm["precompiled_charsmap"])) if nrm else dict(pairs=[], grow=1)
+    except (ValueError, KeyError, TypeError) as e:
+        return None, f"precompiled_charsmap: {e}"
+    if any(k.startswith(_EXT_PICT_2BYTE) for k, _ in cmap["pairs"]):
+        return None, "a charsmap key starts with \u00a9 or \u00ae, where emoji ZWJ sequences would change its clusters"
+    try:
+        unigram_classes()
+    except ImportError as e:
+        return None, f"the grapheme class table is probed through sentencepiece, which is not installed ({e})"
+    spec = dict(pieces=[(p.encode("utf-8"), float(s)) for p, s in vocab], unk_id=unk_id, charsmap=cmap["pairs"],
+                grow=cmap["grow"],
+                added=[(a["content"], int(a["id"]), bool(a.get("normalized", True)), bool(a.get("lstrip", False)),
+                        bool(a.get("rstrip", False))) for a in added],
+                cls_id=pair[0], sep_id=pair[1], pad_id=int(tokenizer.pad_token_id),
+                type_ids="token_type_ids" in getattr(tokenizer, "model_input_names", ()))
+    return spec, ""

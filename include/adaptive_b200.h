@@ -527,6 +527,44 @@ int ac_tokenizer_create_bpe(const ac_bpe_tokenizer_spec *spec, ac_tokenizer **ou
 /* bytes of workspace ac_tokenize needs for B texts of text_bytes bytes in all (offsets[B] - offsets[0]) at max_length */
 int ac_tokenize_workspace_bytes_text(const ac_tokenizer *tok, int B, int64_t text_bytes, int max_length, size_t *bytes);
 
+/* SentencePiece Unigram tokenizers of the XLM-RoBERTa shape (xlm-roberta-*, bge-m3, multilingual-e5-*, jina-embeddings-v3,
+ * snowflake-arctic-embed-l-v2.0) as AutoTokenizer loads them: the normalizer Precompiled(charsmap) or none, the pre-tokenizer
+ * Sequence[WhitespaceSplit, Metaspace("▁", prepend_scheme always, split)], a Unigram model without byte fallback,
+ * "[special] A [special]", right truncation and padding, added tokens with single_word = false.  The same handle type and
+ * calls as BPE: ac_tokenize_workspace_bytes refuses the handle, ac_tokenize takes max_len int32[2] and leaves to the caller
+ * (lengths[i] = -1, max_len[1] = 1) the texts among whose first max_length - 2 words is one longer than AC_UNIGRAM_MAX_WORD
+ * bytes ("▁" included) or whose normalized words do not fit the workspace. */
+#define AC_UNIGRAM_MAX_WORD 4096
+
+typedef struct {
+    /* HOST class byte of every codepoint c < AC_TOKENIZER_CODEPOINTS: bit 0 c joins the grapheme cluster before it (Extend,
+       ZWJ, SpacingMark), bit 1 a control (Control, CR, LF), bit 2 Prepend, bit 3 Rust char::is_whitespace */
+    const uint8_t *cls;
+    /* the Precompiled charsmap as (key, value) pairs, key k = map_keys[map_key_offsets[k] .. map_key_offsets[k + 1]) and its
+       value likewise; n_map = 0 for a tokenizer without a normalizer */
+    const uint8_t *map_keys;
+    const int64_t *map_key_offsets;
+    const uint8_t *map_values;
+    const int64_t *map_value_offsets;
+    int n_map;
+    int grow;                    /* no value is longer than grow bytes per key byte (1 .. 64; 1 without a normalizer) */
+    /* the model vocab in id order: piece v = piece_bytes[piece_offsets[v] .. piece_offsets[v + 1]) with score piece_scores[v] */
+    const uint8_t *piece_bytes;
+    const int64_t *piece_offsets;
+    const double *piece_scores;
+    int n_pieces;
+    int unk_id;
+    /* added tokens as in ac_bpe_tokenizer_spec */
+    const uint8_t *added_bytes;
+    const int64_t *added_offsets;
+    const int32_t *added_ids;
+    const uint8_t *added_flags;
+    int n_added;
+    int cls_id, sep_id, pad_id;
+} ac_unigram_tokenizer_spec;
+
+int ac_tokenizer_create_unigram(const ac_unigram_tokenizer_spec *spec, ac_tokenizer **out);
+
 /* ------------------------------------------------------------------------------------------
  * predict_batch() glue on the device (classifier.py:1329-1384) and the end-to-end pipeline.
  * ------------------------------------------------------------------------------------------ */
